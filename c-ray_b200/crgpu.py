@@ -51,6 +51,18 @@ class Stats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "pad"}
 
 
+class TraceOpts(C.Structure):
+    """struct crgpu_trace_opts: the launch variant of the traversal kernel (crgpu_trace_rays)"""
+    _fields_ = [(n, C.c_int32) for n in ("count", "minb", "defer", "refill", "burst", "inst_min")] + [("order", C.c_void_p)]
+
+
+# struct crgpu_ray_record
+RAY_RECORD_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("inst", "<i4"), ("poly", "<i4"), ("key", "<u4"),
+                             ("prim", "<u4"), ("pad", "<u4")])
+assert RAY_RECORD_DTYPE.itemsize == 32
+# the frame path's defaults (crg_trace_knobs_env); burst is 4 when leaves are deferred
+TRACE_DEFAULTS = dict(count=0, minb=3, defer=0, refill=16, burst=3, inst_min=8)
+
 _lib = None
 
 
@@ -79,6 +91,7 @@ def lib():
         L.crgpu_framebuffer_to_srgb8.argtypes = [P, P]
         L.crgpu_framebuffer_device_ptr.argtypes = [P, C.POINTER(P), C.POINTER(C.c_size_t)]
         L.crgpu_trace_kat.argtypes = [P, P, C.c_int, P]
+        L.crgpu_trace_rays.argtypes = [P, P, C.c_uint32, C.POINTER(TraceOpts), P, P, C.POINTER(C.c_uint32), C.POINTER(Stats)]
         L.crgpu_scene_create_prepared.argtypes = [P, C.c_int, C.POINTER(P)]
         L.crgpu_scene_info.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.crgpu_device_trim.argtypes = [C.c_int]
@@ -87,7 +100,7 @@ def lib():
         L.crscene_set_config.argtypes = [C.POINTER(FlatScene)] + [C.c_int] * 4
         for f in ("crgpu_device_count", "crgpu_scene_create", "crgpu_scene_destroy", "crgpu_set_max_paths_in_flight",
                   "crgpu_render_tile", "crgpu_render_tiles", "crgpu_set_stream", "crgpu_use_own_stream", "crgpu_get_stats", "crgpu_framebuffer_clear", "crgpu_framebuffer_read", "crgpu_framebuffer_write",
-                  "crgpu_framebuffer_to_srgb8", "crgpu_framebuffer_device_ptr", "crgpu_trace_kat", "crscene_load",
+                  "crgpu_framebuffer_to_srgb8", "crgpu_framebuffer_device_ptr", "crgpu_trace_kat", "crgpu_trace_rays", "crscene_load",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
                   "crscene_set_config"):
             getattr(L, f).restype = C.c_int
@@ -223,6 +236,29 @@ class GpuScene:
         out = np.zeros(len(xyp) * 160, dtype=np.uint8)
         _check(lib().crgpu_trace_kat(self.handle, xyp.ctypes.data, len(xyp), out.ctypes.data), "crgpu_trace_kat")
         return out
+
+    def trace_rays(self, rays, order=None, **knobs):
+        """Closest hits of rays (n x 6 float32: origin, direction) through the frame's traversal kernel and bucket sort.
+        knobs: count, minb, defer, refill, burst, inst_min (TRACE_DEFAULTS); order: a permutation K2 takes the rays in.
+        Returns (records, perm, misses, stats)."""
+        rays = np.ascontiguousarray(rays, dtype=np.float32).reshape(-1, 6)
+        n = len(rays)
+        k = dict(TRACE_DEFAULTS)
+        if knobs.get("defer"):
+            k["burst"] = 4
+        k.update(knobs)
+        opts = TraceOpts(**{f: int(k[f]) for f in TRACE_DEFAULTS})
+        if order is not None:
+            order = np.ascontiguousarray(order, dtype=np.uint32)
+            assert order.shape == (n,)
+            opts.order = order.ctypes.data
+        rec = np.zeros(n, dtype=RAY_RECORD_DTYPE)
+        perm = np.zeros(n, dtype=np.uint32)
+        misses = C.c_uint32(0)
+        st = Stats()
+        _check(lib().crgpu_trace_rays(self.handle, rays.ctypes.data, n, C.byref(opts), rec.ctypes.data, perm.ctypes.data,
+                                      C.byref(misses), C.byref(st)), "crgpu_trace_rays")
+        return rec, perm, misses.value, st.as_dict()
 
     def set_max_paths(self, n):
         _check(lib().crgpu_set_max_paths_in_flight(self.handle, int(n)), "crgpu_set_max_paths_in_flight")

@@ -700,7 +700,7 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 			stage.insert(stage.end(), pairs.begin() + b.pair_offset, pairs.begin() + b.pair_offset + cnt);
 		};
 		/* shared memory and L1 share 228 KB per SM: every staged KB is a KB of L1 the traversal loses, so the default
-		 * stages only the very top (128 nodes = 8 KB); CRGPU_TRACE_STAGE=<pairs> (0..1024) overrides */
+		 * stages nothing; CRGPU_TRACE_STAGE=<pairs> (0..1024, read at every prepare) stages the top nodes of every BVH */
 		const char *env = getenv("CRGPU_TRACE_STAGE");
 		uint32_t total_budget = env ? (uint32_t)atoi(env) : 0u;
 		if (total_budget > CRG_STAGE_PAIRS) total_budget = CRG_STAGE_PAIRS;
@@ -957,6 +957,7 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	const int maxDepth = (int)s->dev.bounces;
 	const int grid = s->sm_count * 8;
 	const int dirmode = crg_dir_mode();
+	const TraceKnobs &knobs = crg_trace_knobs_env();
 	uint64_t launches = 0;
 	float trace_ms = 0.f, shade_ms = 0.f;
 	if (timing) CU(cudaEventRecord(s->ev[0], s->stream));
@@ -982,7 +983,7 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 		for (int depth = 0; depth < maxDepth; ++depth) {
 			if (depth >= CRG_TAIL_FROM && !count) { crg_launch_tail(s->dev_copy, wb, cur, depth, maxDepth, s->xnodes, st); ++launches; }
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
-			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, grid, st);
+			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, knobs, st);
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
 			crg_launch_bucket(wb, cur, grid, st);
 			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
@@ -1177,6 +1178,68 @@ extern "C" int crgpu_scene_info(crgpu_scene *s, int *device, int *width, int *he
 	if (width) *width = (int)s->dev.image_width;
 	if (height) *height = (int)s->dev.image_height;
 	return CRGPU_OK;
+}
+
+/* Closest hits of a ray batch through the production K2 (k_trace, by the launch path and launch shape of a frame) and K4. */
+extern "C" int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, const struct crgpu_trace_opts *opts,
+								struct crgpu_ray_record *records_out, uint32_t *perm_out, uint32_t *misses_out, struct crgpu_stats *stats_out) {
+	if (!s || !opts || (n && (!rays || !records_out || !perm_out)) || n > (1u << 30)) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad argument");
+	TraceKnobs kn;
+	kn.minb = opts->minb; kn.defer = opts->defer; kn.refill = opts->refill; kn.burst = opts->burst; kn.inst_min = opts->inst_min;
+	if (kn.minb < 2 || kn.minb > 4 || kn.defer < 0 || kn.defer > 2 || kn.refill < 1 || kn.refill > 32 || kn.burst < 1 || kn.inst_min < 1 || kn.inst_min > 32)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "trace options out of range");
+	if (opts->order) {                                  /* K2 reads rays through the order: it must be a permutation of [0, n) */
+		std::vector<uint8_t> seen(n, 0);
+		for (uint32_t i = 0; i < n; ++i) {
+			if (opts->order[i] >= n || seen[opts->order[i]]) return fail(CRGPU_ERR_BAD_ARGUMENT, "order is not a permutation of [0, %u)", n);
+			seen[opts->order[i]] = 1;
+		}
+	}
+	CU(cudaSetDevice(s->device));
+	int rc = crgpu_get_stats(s, nullptr);               /* earlier work done and its counters taken: the deltas below are this batch's */
+	if (rc) return rc;
+	rc = alloc_wave(s, n ? n : 1, 1);
+	if (rc) return rc;
+	const WaveBuffers &wb = s->wb;
+	cudaStream_t st = s->stream;
+	const int grid = s->sm_count * 8;
+	std::vector<float4> a(n), b(n);
+	for (uint32_t i = 0; i < n; ++i) {
+		const float *r = rays + 6 * (size_t)i;
+		a[i] = make_float4(r[0], r[1], r[2], r[3]);
+		b[i] = make_float4(r[4], r[5], 1.0f, 1.0f);
+	}
+	const unsigned counts[5] = { n, 0u, 0u, 0u, 0u };
+	CU(cudaMemcpyAsync(wb.stA[0], a.data(), (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(wb.stB[0], b.data(), (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
+	if (opts->order) CU(cudaMemcpyAsync(wb.perm2, opts->order, (size_t)n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(wb.counts, counts, sizeof counts, cudaMemcpyHostToDevice, st));
+	CU(cudaMemsetAsync(wb.hist, 0, 1024 * sizeof(unsigned), st));
+	/* poison: no write-back produces a negative distance or the instance index -1515870811, and K4 must overwrite all of perm.
+	 * Every 8-bit value is some ray's key, so a key left behind shows only as a key that differs from the expected one; the
+	 * write-back stores hit, instance and key together, so a ray it missed also keeps the hit and instance poison */
+	CU(cudaMemsetAsync(wb.hit, 0xA5, (size_t)n * sizeof(float4), st));
+	CU(cudaMemsetAsync(wb.hitInst, 0xA5, (size_t)n * sizeof(int), st));
+	CU(cudaMemsetAsync(wb.hitKey, 0xA5, (size_t)n, st));
+	CU(cudaMemsetAsync(wb.perm, 0xFF, (size_t)n * sizeof(unsigned), st));
+	crg_launch_trace(s->dev, wb, 0, opts->count != 0, opts->order != nullptr, kn, st);
+	crg_launch_bucket(wb, 0, grid, st);
+	CU(cudaGetLastError());
+	void *drec = nullptr;
+	if (n) {
+		CU(cudaMalloc(&drec, (size_t)n * sizeof(struct crgpu_ray_record)));
+		crg_launch_trace_records(s->dev, wb, n, drec, grid, st);
+	}
+	unsigned cnt[5];
+	cudaError_t e = cudaGetLastError();
+	if (e == cudaSuccess && n) e = cudaMemcpyAsync(records_out, drec, (size_t)n * sizeof(struct crgpu_ray_record), cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess && n) e = cudaMemcpyAsync(perm_out, wb.perm, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, wb.counts, sizeof cnt, cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+	if (drec) cudaFree(drec);
+	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "trace_rays: %s", cudaGetErrorString(e));
+	if (misses_out) *misses_out = cnt[4];
+	return crgpu_get_stats(s, stats_out);               /* fails if the traversal watchdog fired */
 }
 
 extern "C" int crgpu_trace_kat(crgpu_scene *s, const int32_t *xyp, int count, void *records_out) {

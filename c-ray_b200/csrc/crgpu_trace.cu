@@ -201,7 +201,7 @@ void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDe
 #define CRG_MAX_DEVICES 64
 #endif
 template <bool COUNT, int MINB, int DEFER>
-static void launch_trace_variant(const DevScene &sc, const WaveBuffers &wb, int cur, bool sorted, cudaStream_t st) {
+static void launch_trace_variant(const DevScene &sc, const WaveBuffers &wb, int cur, bool sorted, const TraceKnobs &kn, cudaStream_t st) {
 	/* launch shape per DEVICE: the host mirror drives several GPUs from one process (one thread each), and both the
 	 * occupancy answer and the opt-in shared-memory attribute belong to a device, not to the process */
 	struct Shape { int grid; size_t smem; };
@@ -224,30 +224,56 @@ static void launch_trace_variant(const DevScene &sc, const WaveBuffers &wb, int 
 		}
 		grid = sh.grid;
 	}
-	static const int refill = [] { const char *e = getenv("CRGPU_TRACE_REFILL"); const int v = e ? atoi(e) : CRG_REFILL; return v >= 1 && v <= 32 ? v : CRG_REFILL; }();
-	static const int burst = [] { const char *e = getenv("CRGPU_TRACE_BURST"); const int v = e ? atoi(e) : (DEFER ? 4 : CRG_NODE_BURST); return v >= 1 ? v : CRG_NODE_BURST; }();
-	static const int inst_min = [] { const char *e = getenv("CRGPU_TRACE_INSTMIN"); const int v = e ? atoi(e) : 8; return v >= 1 && v <= 32 ? v : 8; }();
-	k_trace<COUNT, MINB, DEFER><<<grid, 256, smem, st>>>(sc, wb, cur, refill, burst, sorted ? 1 : 0, inst_min);
+	k_trace<COUNT, MINB, DEFER><<<grid, 256, smem, st>>>(sc, wb, cur, kn.refill, kn.burst, sorted ? 1 : 0, kn.inst_min);
 }
 
-void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, int grid, cudaStream_t st) {
-	(void)grid;
-	static const int minb = [] { const char *e = getenv("CRGPU_TRACE_MINB"); const int v = e ? atoi(e) : 3; return v >= 2 && v <= 4 ? v : 3; }();
-	/* CRGPU_TRACE_DEFER: 0 = triangles tested inside the node step, 1 = lanes wait and test their own leaf after the burst,
-	 * 2 = lanes wait and the warp deals the (ray, triangle) pairs over its 32 lanes (cr_coop_leaves) */
-	static const int defer = [] { const char *e = getenv("CRGPU_TRACE_DEFER"); const int v = e ? atoi(e) : CRG_DEFER_DEFAULT; return v >= 0 && v <= 2 ? v : CRG_DEFER_DEFAULT; }();
+/* the frame path's knobs: parsed once per process; out-of-range values fall back to the defaults */
+const TraceKnobs &crg_trace_knobs_env(void) {
+	static const TraceKnobs kn = [] {
+		auto env = [](const char *name, int dflt, int lo, int hi) { const char *e = getenv(name); const int v = e ? atoi(e) : dflt; return v >= lo && v <= hi ? v : dflt; };
+		TraceKnobs k;
+		k.minb = env("CRGPU_TRACE_MINB", 3, 2, 4);
+		k.defer = env("CRGPU_TRACE_DEFER", CRG_DEFER_DEFAULT, 0, 2);
+		k.refill = env("CRGPU_TRACE_REFILL", CRG_REFILL, 1, 32);
+		k.burst = env("CRGPU_TRACE_BURST", k.defer ? 4 : CRG_NODE_BURST, 1, 1 << 30);
+		k.inst_min = env("CRGPU_TRACE_INSTMIN", 8, 1, 32);
+		return k;
+	}();
+	return kn;
+}
+
+void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, const TraceKnobs &kn, cudaStream_t st) {
 	if (count) {
-		if (defer == 2) launch_trace_variant<true, 3, 2>(sc, wb, cur, sorted, st);
-		else if (defer == 1) launch_trace_variant<true, 3, 1>(sc, wb, cur, sorted, st);
-		else launch_trace_variant<true, 3, 0>(sc, wb, cur, sorted, st);
+		if (kn.defer == 2) launch_trace_variant<true, 3, 2>(sc, wb, cur, sorted, kn, st);
+		else if (kn.defer == 1) launch_trace_variant<true, 3, 1>(sc, wb, cur, sorted, kn, st);
+		else launch_trace_variant<true, 3, 0>(sc, wb, cur, sorted, kn, st);
 		return;
 	}
 #define CRG_TRACE_DISPATCH(D) do { \
-		if (minb == 4) launch_trace_variant<false, 4, D>(sc, wb, cur, sorted, st); \
-		else if (minb == 2) launch_trace_variant<false, 2, D>(sc, wb, cur, sorted, st); \
-		else launch_trace_variant<false, 3, D>(sc, wb, cur, sorted, st); } while (0)
-	if (defer == 2) CRG_TRACE_DISPATCH(2);
-	else if (defer == 1) CRG_TRACE_DISPATCH(1);
+		if (kn.minb == 4) launch_trace_variant<false, 4, D>(sc, wb, cur, sorted, kn, st); \
+		else if (kn.minb == 2) launch_trace_variant<false, 2, D>(sc, wb, cur, sorted, kn, st); \
+		else launch_trace_variant<false, 3, D>(sc, wb, cur, sorted, kn, st); } while (0)
+	if (kn.defer == 2) CRG_TRACE_DISPATCH(2);
+	else if (kn.defer == 1) CRG_TRACE_DISPATCH(1);
 	else CRG_TRACE_DISPATCH(0);
 #undef CRG_TRACE_DISPATCH
 }
+
+/* crgpu_trace_rays: K2's write-back as one record per ray.  A hit record (t, u, v, prim slot) and its instance are written
+ * together, so the slot is only followed into slot_poly for an instance index K2 can have written. */
+struct TraceRecord { float t, u, v; int inst, poly; unsigned key, prim, pad; };
+__global__ void __launch_bounds__(256) k_trace_records(DevScene sc, WaveBuffers wb, unsigned n, TraceRecord *__restrict__ out) {
+	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const float4 h = wb.hit[i];
+		const int inst = wb.hitInst[i];
+		TraceRecord r;
+		r.t = h.x; r.u = h.y; r.v = h.z; r.inst = inst; r.prim = __float_as_uint(h.w); r.key = wb.hitKey[i]; r.pad = 0u;
+		r.poly = -1;
+		if (inst >= 0 && (unsigned)inst < sc.instance_count && sc.instances[inst].kind == CRS_INST_MESH) r.poly = (int)sc.slot_poly[r.prim];
+		out[i] = r;
+	}
+}
+void crg_launch_trace_records(const DevScene &sc, const WaveBuffers &wb, unsigned n, void *out, int grid, cudaStream_t st) {
+	k_trace_records<<<grid, 256, 0, st>>>(sc, wb, n, static_cast<TraceRecord *>(out));
+}
+static_assert(sizeof(TraceRecord) == 32, "TraceRecord must match struct crgpu_ray_record (include/crgpu.h)");

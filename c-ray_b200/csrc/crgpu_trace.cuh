@@ -64,7 +64,7 @@ CRD void cr_camera_ray(const DevCamera &cam, int x, int y, uint64_t &rng, v3 &o,
 struct RaySetup {
 	v3 invDir, scaledStart;
 	bool ox, oy, oz;
-	unsigned deg;      /* bit a set: 1/d[a] is +-inf (d[a] is +-0 or denormal) — see cr_node_test */
+	unsigned deg;      /* bit a set: -o[a]/d[a] is not finite (1/d[a] is +-inf, or o[a]*(1/d[a]) overflows) — see cr_node_test */
 };
 
 CRD RaySetup cr_ray_setup(v3 o, v3 d) {                                                /* bvh.c:369-376 */
@@ -74,16 +74,19 @@ CRD RaySetup cr_ray_setup(v3 o, v3 d) {                                         
 	s.oz = (__float_as_uint(d.z) >> 31) != 0u;
 	s.invDir = v3make(cr_div(1.0f, d.x), cr_div(1.0f, d.y), cr_div(1.0f, d.z));
 	s.scaledStart = v3scale(v3mul(o, s.invDir), -1.0f);
-	s.deg = (isinf(s.invDir.x) ? 1u : 0u) | (isinf(s.invDir.y) ? 2u : 0u) | (isinf(s.invDir.z) ? 4u : 0u);
+	s.deg = (isfinite(s.scaledStart.x) ? 0u : 1u) | (isfinite(s.scaledStart.y) ? 0u : 2u) | (isfinite(s.scaledStart.z) ? 0u : 4u);
 	return s;
 }
 
 /* bvh.c:318-324: `fastMultiplyAdd` is fmaf() when the compiler defines FP_FAST_FMAF (the reference's stock
  * -march=native build) and a*b+c otherwise (the strict oracle build).  The slab test only decides which nodes
- * are ENTERED, never a hit distance, and both variants are conservative; the survey measured bit-identical
- * framebuffers between them on hdr.json and venus.json, and tests/test_gpu_parity.py holds the fused variant to
- * exact hit records against the un-fused oracle.  Fused = 6 FFMA per child instead of 6 FMUL + 6 FADD.
- * Build with -DCRG_SLAB_UNFUSED to get the two-rounding form. */
+ * are ENTERED, never a hit distance; the survey measured bit-identical framebuffers between them on hdr.json and
+ * venus.json.  The two differ (a) by one rounding where a ray grazes a box face, which can decide whether a box of zero
+ * thickness (a planar, axis-aligned leaf) is entered, and (b) where o*(1/d) overflows: the un-fused b*(1/d) + -inf is
+ * NaN once b*(1/d) overflows too, and the reference's min/max chain drops that axis, while the fused result is -inf
+ * and would reject every box.  Case (b) is culled exactly (below).  tests/test_gpu_trace.py holds K2 to the oracle in
+ * these semantics.  Fused = 6 FFMA per child instead of 6 FMUL + 6 FADD.  Build with -DCRG_SLAB_UNFUSED to get the
+ * two-rounding form. */
 #ifdef CRG_SLAB_UNFUSED
 #define CR_SLAB_MAD(a, b, c) ((a) * (b) + (c))
 #else
@@ -97,11 +100,14 @@ CRD RaySetup cr_ray_setup(v3 o, v3 d) {                                         
  * propagation, the x or y axis before it), so such a ray "enters" a large part of the BVH — up to
  * ~115,000 of Venus' 229,087 nodes per ray (measured with the oracle on hdr.json, horizon rays with
  * d.y == 0).  That is harmless on a CPU (~1 ms) but one GPU thread would need ~50-150 ms while the
- * whole wavefront waits.  The reference's degenerate test is a pure superset of the exact slab test and
- * the Möller–Trumbore test decides every hit on its own, so culling with the exact test (axis with
- * d == 0: inside the slab iff lo <= o <= hi) returns the same closest hit; the two could only differ
- * for a ray that grazes a triangle within one ulp of its leaf's bounding box, on an already
- * measure-zero ray (~1e-13 per ray).  Rays without a zero component take the verbatim path. */
+ * whole wavefront waits.  The same happens on an axis whose 1/d is finite but so large that o*(1/d)
+ * overflows (|d| below ~|o| / 3.4e38, e.g. d = FLT_MIN): there the fused form would even give -inf for
+ * both planes and reject every box, missing hits the reference finds.  So every axis whose -o*(1/d) is
+ * not finite is culled with the exact test (inside the slab iff lo <= o <= hi; along such an axis the
+ * ray moves by less than |o| even at t = FLT_MAX).  The reference's degenerate test is
+ * a superset of the exact one and the Möller–Trumbore test decides every hit on its own, so the closest
+ * hit is the same; they could only differ for a ray that grazes a triangle within one ulp of its leaf's
+ * bounding box.  All other rays take the verbatim path. */
 CRD bool cr_node_test(const float *b, const RaySetup &r, v3 o, float maxDist, float &tEntry) {
 	float tMinX = CR_SLAB_MAD((r.ox ? b[1] : b[0]), r.invDir.x, r.scaledStart.x);
 	float tMaxX = CR_SLAB_MAD((r.ox ? b[0] : b[1]), r.invDir.x, r.scaledStart.x);

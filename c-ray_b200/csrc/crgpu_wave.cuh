@@ -55,10 +55,23 @@ __device__ __forceinline__ void crg_pixel_xy(const TileDesc &td, unsigned px, in
 	else { x = td.x0 + (int)(px % (unsigned)td.tw); y = td.y0 + (int)(px / (unsigned)td.tw); }
 }
 
+/* Launch variant of K2.  Every variant computes the same hit records; they differ in how a warp schedules its work.
+ *   minb      blocks per SM the compiler makes room for: 2, 3 or 4 (the instrumented kernel, count = true, always uses 3)
+ *   defer     0 = leaf triangles tested inside the node step, 1 = after the node burst by each lane, 2 = dealt over the warp
+ *   refill    a warp fetches new rays when fewer than `refill` lanes are busy (1..32)
+ *   burst     child-pair steps per node phase (>= 1)
+ *   inst_min  lanes that must want an instance step before the warp takes one (1..32)
+ * The frame path reads them once from CRGPU_TRACE_MINB / _DEFER / _REFILL / _BURST / _INSTMIN (crg_trace_knobs_env);
+ * crgpu_trace_rays passes its own. */
+struct TraceKnobs { int minb, defer, refill, burst, inst_min; };
+const TraceKnobs &crg_trace_knobs_env(void);
+
 /* launchers (defined in crgpu_trace.cu / crgpu_shade.cu); `dsc` is the device copy of `sc` */
 void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, cudaStream_t st);
 void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st);
-void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, int grid, cudaStream_t st);
+void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, const TraceKnobs &kn, cudaStream_t st);
+/* per-ray records of K2's write-back (crgpu_trace_rays): t, u, v, instance, poly (-1 for spheres and misses), key */
+void crg_launch_trace_records(const DevScene &sc, const WaveBuffers &wb, unsigned n, void *out, int grid, cudaStream_t st);
 void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int grid, cudaStream_t st);
 int crg_dir_mode(void);   /* 0 = off, 1 = octant (8 bins), 2 = octant x major axis (24 bins), 3 = octant x origin cell (256 bins) */
 void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st);

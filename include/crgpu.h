@@ -135,6 +135,31 @@ int crgpu_scene_info(crgpu_scene *s, int *device, int *width, int *height);
  * (x, y, pass) triples, in the 160-byte record layout of oracle/ref_harness.c `struct hit_kat`. */
 int crgpu_trace_kat(crgpu_scene *s, const int32_t *xyp, int count, void *records_out);
 
+/* Test entry point of the traversal kernel that renders frames: closest hits of `n` rays (rays: n x 6 floats, origin then
+ * direction) through K2 (k_trace, launched as a frame launches it) and K4 (the counting sort by shading key).  Returns per ray
+ * its record, `perm_out` (n ray indices in K4's bucket order: the misses first), `*misses_out` (the number of misses) and in
+ * `stats_out` the rays and, with `count`, P/T/S/I.  Fails when the traversal watchdog fired.  Staging of the top BVH nodes
+ * follows CRGPU_TRACE_STAGE at crgpu_prepare time and engages for batches of at least 65,536 rays, as in a frame. */
+struct crgpu_trace_opts {
+	int32_t count;             /* 1: the instrumented kernel, which fills P/T/S/I (it is always built for 3 blocks per SM) */
+	int32_t minb;              /* blocks per SM: 2, 3 or 4 */
+	int32_t defer;             /* leaf triangles: 0 = in the node step, 1 = after the node burst, 2 = dealt over the warp */
+	int32_t refill;            /* a warp fetches rays when fewer than this many lanes are busy: 1..32 */
+	int32_t burst;             /* child-pair steps per node phase: >= 1 */
+	int32_t inst_min;          /* lanes that must want an instance step before the warp takes one: 1..32 */
+	const uint32_t *order;     /* NULL, or a permutation of [0, n): the order K2 takes the rays in (the direction-sorted read) */
+};
+struct crgpu_ray_record {
+	float t, u, v;             /* distance (FLT_MAX for a miss), barycentric u, v of the winning triangle */
+	int32_t inst;              /* instance index, -1 = miss */
+	int32_t poly;              /* global poly index; -1 for spheres and misses */
+	uint32_t key;              /* shading key: 0 for a miss, else min(material + 1, 255) */
+	uint32_t prim;             /* triangle slot */
+	uint32_t pad;
+};
+int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, const struct crgpu_trace_opts *opts,
+                     struct crgpu_ray_record *records_out, uint32_t *perm_out, uint32_t *misses_out, struct crgpu_stats *stats_out);
+
 /* SURVEY §8(f1): the reference's binned-SAH BVH build (reference src/accelerators/bvh.c:96-296: partitionPrimitives,
  * buildBvhRecursive, buildBvhGeneric) on device `device`, level-synchronous (c-ray_b200/csrc/crgpu_bvh_build.cu).  Produces the
  * SAME tree as the reference and as the host builder (crloader_build_bvh): node order, leaf ranges, primitive order, bounds.

@@ -155,6 +155,7 @@ struct hit {
 	int material;      /* global material index (the reference copies the 144-byte struct) */
 	v3 p, n;
 	v2 uv;
+	v2 bary;           /* barycentric (u, v) of the winning triangle, before texmap_mesh replaces uv */
 	float dist;
 	int poly;          /* global poly index or -1 */
 	int inst;
@@ -273,7 +274,37 @@ static inline bool node_test(const struct crs_bvh_node *node, v3 invDir, v3 scal
  * tools/k2_warp_model.py to study warp scheduling policies offline.  Event bytes: 0 = top-level child-pair step,
  * 1 = mesh instance step, 2 = sphere instance step, 64+k = bottom-level child-pair step that tested k triangles (k <= 63). */
 struct cro_trace { uint8_t *buf; size_t cap, len; size_t pair_at; uint16_t x, y, pass; };
-struct trav_ctx { const struct crs_scene *s; struct cro_counters *ctr; struct cro_trace *tr; };
+/* dev = 1: the device traversal's slab test (cro_closest_hit semantics 1); 0 everywhere else */
+struct trav_ctx { const struct crs_scene *s; struct cro_counters *ctr; struct cro_trace *tr; int dev; };
+
+/* The slab test of the device traversal (cr_node_test, crgpu_trace.cuh), which deviates from node_test in exactly two ways
+ * (DESIGN.md §2): every bound*invDir+scaledStart is ONE fused rounding (fmaf), and an axis whose scaledStart = -o/d is not
+ * finite (1/d is +-inf, or o*(1/d) overflows) is culled exactly, inside the slab iff lo <= o <= hi, instead of through the
+ * NaN-tolerant min/max chain. */
+static inline bool node_test_dev(const struct crs_bvh_node *node, v3 o, v3 invDir, v3 scaledStart, const int *oct,
+								 float maxDist, float *tEntry) {
+	const float *b = node->bounds;
+	float tMinX = fmaf(b[0 + oct[0]], invDir.x, scaledStart.x);
+	float tMaxX = fmaf(b[0 + 1 - oct[0]], invDir.x, scaledStart.x);
+	float tMinY = fmaf(b[2 + oct[1]], invDir.y, scaledStart.y);
+	float tMaxY = fmaf(b[2 + 1 - oct[1]], invDir.y, scaledStart.y);
+	float tMinZ = fmaf(b[4 + oct[2]], invDir.z, scaledStart.z);
+	float tMaxZ = fmaf(b[4 + 1 - oct[2]], invDir.z, scaledStart.z);
+	if (!isfinite(scaledStart.x)) { const bool in = b[0] <= o.x && o.x <= b[1]; tMinX = in ? -INFINITY : INFINITY; tMaxX = in ? INFINITY : -INFINITY; }
+	if (!isfinite(scaledStart.y)) { const bool in = b[2] <= o.y && o.y <= b[3]; tMinY = in ? -INFINITY : INFINITY; tMaxY = in ? INFINITY : -INFINITY; }
+	if (!isfinite(scaledStart.z)) { const bool in = b[4] <= o.z && o.z <= b[5]; tMinZ = in ? -INFINITY : INFINITY; tMaxZ = in ? INFINITY : -INFINITY; }
+	float tMin = tMinX > tMinY ? tMinX : tMinY;
+	float tMax = tMaxX < tMaxY ? tMaxX : tMaxY;
+	tMin = tMin > tMinZ ? tMin : tMinZ;
+	tMax = tMax < tMaxZ ? tMax : tMaxZ;
+	tMin = tMin > 0 ? tMin : 0;
+	tMax = tMax < maxDist ? tMax : maxDist;
+	*tEntry = tMin;
+	return tMin <= tMax;
+}
+#define NODE_TEST(c, nd, o, invDir, scaledStart, oct, maxDist, tEntry) \
+	((c)->dev ? node_test_dev((nd), (o), (invDir), (scaledStart), (oct), (maxDist), (tEntry)) \
+	          : node_test((nd), (invDir), (scaledStart), (oct), (maxDist), (tEntry)))
 static inline void tr_event(const struct trav_ctx *c, uint8_t code) {
 	if (c->tr && c->tr->len < c->tr->cap) { c->tr->pair_at = c->tr->len; c->tr->buf[c->tr->len++] = code; }
 }
@@ -351,6 +382,7 @@ static bool intersect_mesh_inst(const struct trav_ctx *c, const struct crs_insta
 	if (c->ctr) c->ctr->inst_visits++;
 	tr_event(c, 1);
 	if (traverse(c, mesh->bvh, (int)inst->object, &copy, isect)) {
+		isect->bary = isect->uv;
 		isect->uv = texmap_mesh(c->s, mesh, isect);
 		isect->material = (int)(mesh->material_offset + c->s->polys[isect->poly].material);
 		isect->p = xf_point(inst->A, isect->p);
@@ -399,7 +431,7 @@ static bool traverse(const struct trav_ctx *c, uint32_t bvhIdx, int meshIdx, con
 	if (bvh->node_count == 1) {                                                             /* bvh.c:382-387 */
 		float tEntry;
 		if (mesh) tr_event(c, 64);                               /* single-leaf BVH: one step that tests the leaf's triangles */
-		if (node_test(nodes, invDir, scaledStart, oct, maxDist, &tEntry)) return LEAF(nodes);
+		if (NODE_TEST(c, nodes, ray->o, invDir, scaledStart, oct, maxDist, &tEntry)) return LEAF(nodes);
 		return false;
 	}
 	const struct crs_bvh_node *node = nodes;
@@ -411,8 +443,8 @@ static bool traverse(const struct trav_ctx *c, uint32_t bvhIdx, int meshIdx, con
 		if (c->ctr) c->ctr->node_pairs++;
 		tr_event(c, mesh ? 64 : 0);
 		float tL, tR;
-		bool hitL = node_test(left, invDir, scaledStart, oct, maxDist, &tL);
-		bool hitR = node_test(right, invDir, scaledStart, oct, maxDist, &tR);
+		bool hitL = NODE_TEST(c, left, ray->o, invDir, scaledStart, oct, maxDist, &tL);
+		bool hitR = NODE_TEST(c, right, ray->o, invDir, scaledStart, oct, maxDist, &tR);
 		if (hitL) {
 			if (left->prim_count_leaf & CRS_BVH_LEAF_BIT) {
 				if (LEAF(left)) { maxDist = isect->dist; hasHit = true; }
@@ -803,7 +835,7 @@ struct job {
 static void *render_rows(void *arg) {
 	struct job *j = arg;
 	const struct crs_scene *s = j->s;
-	struct trav_ctx c = { s, j->count ? &j->ctr : NULL, NULL };
+	struct trav_ctx c = { s, j->count ? &j->ctr : NULL, NULL, 0 };
 	const int W = (int)s->prefs.image_width, H = (int)s->prefs.image_height;
 	const int maxPasses = (int)s->prefs.sample_count, bounces = (int)s->prefs.bounces;
 	for (int y = j->yend - 1; y > j->ybegin - 1; --y) {
@@ -841,7 +873,7 @@ static void *run_chunks(void *arg) {
  * Returns the number of bytes written (records are dropped, not truncated, once the buffer is full). */
 size_t cro_trace_region(const struct crs_scene *s, int x0, int y0, int x1, int y1, int pass_begin, int pass_count, uint8_t *buf, size_t cap) {
 	struct cro_trace tr = { buf, cap, 0, 0, 0, 0, 0 };
-	struct trav_ctx c = { s, NULL, &tr };
+	struct trav_ctx c = { s, NULL, &tr, 0 };
 	const int W = (int)s->prefs.image_width;
 	const int maxPasses = (int)s->prefs.sample_count, bounces = (int)s->prefs.bounces;
 	for (int y = y0; y < y1; ++y)
@@ -906,7 +938,7 @@ void cro_sampler_kat(uint32_t pixIdx, int pass, int maxPasses, int n, float *out
 void cro_trace_kat(const struct crs_scene *s, int x, int y, int pass, struct cro_hit_kat *k) {
 	memset(k, 0, sizeof *k);
 	const int W = (int)s->prefs.image_width;
-	struct trav_ctx c = { s, NULL, NULL };
+	struct trav_ctx c = { s, NULL, NULL, 0 };
 	k->x = x; k->y = y; k->pixIdx = y * W + x;
 	struct rng r = { 0, NULL };
 	rng_init(&r, (uint32_t)k->pixIdx, pass, (int)s->prefs.sample_count);
@@ -931,6 +963,58 @@ void cro_trace_kat(const struct crs_scene *s, int x, int y, int pass, struct cro
 	k->out[0] = smp.out.x; k->out[1] = smp.out.y; k->out[2] = smp.out.z;
 	k->color[0] = smp.color.r; k->color[1] = smp.color.g; k->color[2] = smp.color.b; k->color[3] = smp.color.a;
 	k->nextDraw = draw(&r);
+}
+
+/* ---- per-ray closest hit (getClosestIsect, pathtrace.c:26-30) over a batch of rays ------------------------------------------------ */
+struct ray_job { const struct crs_scene *s; const float *rays; struct cro_ray_record *out; size_t lo, hi; int dev; struct cro_counters ctr; bool count; };
+
+static void *closest_hit_rows(void *arg) {
+	struct ray_job *j = arg;
+	struct trav_ctx c = { j->s, j->count ? &j->ctr : NULL, NULL, j->dev };
+	for (size_t i = j->lo; i < j->hi; ++i) {
+		const float *r = j->rays + 6 * i;
+		const struct ray ray = { { r[0], r[1], r[2] }, { r[3], r[4], r[5] } };
+		const struct hit h = closest_isect(&c, &ray);
+		struct cro_ray_record *o = &j->out[i];
+		o->t = h.dist;
+		o->u = h.bary.x; o->v = h.bary.y;
+		o->inst = h.inst;
+		o->poly = -1; o->material = -1;
+		if (h.inst >= 0) {
+			o->poly = j->s->instances[h.inst].kind == CRS_INST_MESH ? h.poly : -1;
+			o->material = h.material;
+		}
+	}
+	return NULL;
+}
+
+int cro_closest_hit(const struct crs_scene *s, size_t n, const float *rays, int semantics, int threads,
+					struct cro_ray_record *out, struct cro_counters *counters) {
+	if (semantics != 0 && semantics != 1) return -1;
+	if (counters) memset(counters, 0, sizeof *counters);
+	if (n == 0) return 0;
+	if (threads < 1) threads = 1;
+	if ((size_t)threads > n) threads = (int)n;
+	struct ray_job *jobs = calloc((size_t)threads, sizeof *jobs);
+	pthread_t *tids = calloc((size_t)threads, sizeof *tids);
+	if (!jobs || !tids) { free(jobs); free(tids); return -1; }
+	for (int t = 0; t < threads; ++t) {
+		jobs[t] = (struct ray_job){ .s = s, .rays = rays, .out = out, .lo = n * (size_t)t / (size_t)threads,
+			.hi = n * (size_t)(t + 1) / (size_t)threads, .dev = semantics, .count = counters != NULL };
+		pthread_create(&tids[t], NULL, closest_hit_rows, &jobs[t]);
+	}
+	for (int t = 0; t < threads; ++t) pthread_join(tids[t], NULL);
+	if (counters) {
+		for (int t = 0; t < threads; ++t) {
+			const struct cro_counters *k = &jobs[t].ctr;
+			counters->rays += k->rays; counters->node_pairs += k->node_pairs; counters->tri_tests += k->tri_tests;
+			counters->sphere_tests += k->sphere_tests; counters->inst_visits += k->inst_visits;
+			if (k->max_stack > counters->max_stack) counters->max_stack = k->max_stack;
+			if (k->max_pairs_ray > counters->max_pairs_ray) counters->max_pairs_ray = k->max_pairs_ray;
+		}
+	}
+	free(tids); free(jobs);
+	return 0;
 }
 
 void cro_to_srgb8(const float *rgb, uint8_t *out, size_t pixels) {

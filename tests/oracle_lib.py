@@ -88,6 +88,11 @@ HIT_KAT_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("pixIdx", "<i4"), ("instI
                           ("out", "<f4", 3), ("color", "<f4", 4), ("nextDraw", "<f4"), ("pad", "<f4", 9)])
 assert HIT_KAT_DTYPE.itemsize == 160
 
+# struct cro_ray_record: one closest-hit record per ray (cro_closest_hit)
+RAY_RECORD_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("inst", "<i4"), ("poly", "<i4"), ("material", "<i4")])
+assert RAY_RECORD_DTYPE.itemsize == 24
+SEM_REFERENCE, SEM_DEVICE = 0, 1
+
 _lib = None
 
 
@@ -107,6 +112,10 @@ def lib():
         L.cro_sampler_kat.argtypes = [C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_void_p]
         L.cro_trace_kat.argtypes = [C.POINTER(Scene), C.c_int, C.c_int, C.c_int, C.c_void_p]
         L.cro_to_srgb8.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.cro_closest_hit.argtypes = [C.POINTER(Scene), C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(Counters)]
+        L.cro_closest_hit.restype = C.c_int
+        L.cro_trace_region.argtypes = [C.POINTER(Scene)] + [C.c_int] * 6 + [C.c_void_p, C.c_size_t]
+        L.cro_trace_region.restype = C.c_size_t
         _lib = L
     return _lib
 
@@ -136,6 +145,29 @@ class OracleScene:
         out = np.zeros(1, dtype=HIT_KAT_DTYPE)
         lib().cro_trace_kat(C.byref(self.s), x, y, p, out.ctypes.data)
         return out[0]
+
+    def closest_hit(self, rays, semantics=SEM_DEVICE, threads=None):
+        """Closest-hit records of rays (n x 6 float32: origin, direction) and the batch's counters (P/T/S/I, rays)."""
+        rays = np.ascontiguousarray(rays, dtype=np.float32).reshape(-1, 6)
+        out = np.zeros(len(rays), dtype=RAY_RECORD_DTYPE)
+        ctr = Counters()
+        rc = lib().cro_closest_hit(C.byref(self.s), len(rays), rays.ctypes.data, semantics, threads or os.cpu_count() or 1,
+                                   out.ctypes.data, C.byref(ctr))
+        if rc != 0:
+            raise RuntimeError(f"cro_closest_hit failed ({rc})")
+        return out, ctr.as_dict()
+
+    def path_rays(self, x0, y0, x1, y1, passes=(0, 1), cap=64 << 20):
+        """Every ray of every bounce of the paths of a region (cro_trace_region), n x 6 float32, in path order."""
+        buf = np.zeros(cap, dtype=np.uint8)
+        n = lib().cro_trace_region(C.byref(self.s), x0, y0, x1, y1, passes[0], passes[1], buf.ctypes.data, cap)
+        assert n + 4096 < cap, "trace buffer too small for the region"
+        rays, pos = [], 0
+        while pos < n:
+            ev = int(buf[pos + 8:pos + 12].view(np.uint32)[0])
+            rays.append(buf[pos + 12:pos + 36].view(np.float32))
+            pos += 36 + ev
+        return np.array(rays, dtype=np.float32).reshape(-1, 6)
 
     def close(self):
         lib().crscene_free(C.byref(self.s))

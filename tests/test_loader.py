@@ -166,6 +166,18 @@ def test_loader_errors(tmp_path):
         crscene.load_json(str(sc))
 
 
+def test_mesh_without_polygons_is_rejected(tmp_path):
+    """An OBJ with vertices but no faces: the loader refuses the instance, so the traversal's empty-BVH case (bvh.c:362-365,
+    which resets the instance of an earlier hit) is not reachable from a scene file.  Should the loader ever accept such a
+    mesh, tests/test_gpu_trace.py has to cover that case."""
+    (tmp_path / "empty.obj").write_text("v 0 0 0\nv 1 0 0\nv 0 1 0\n")
+    sc = tmp_path / "empty.json"
+    sc.write_text(json.dumps({"renderer": {"width": 4, "height": 4}, "camera": {},
+                              "scene": {"meshes": [{"fileName": "empty.obj", "instances": [{}]}]}}))
+    with pytest.raises(RuntimeError, match="without polygons"):
+        crscene.load_json(str(sc))
+
+
 def test_loader_defaults_and_clamps(tmp_path):
     """parsePrefs / parseCamera defaults (sceneloader.c:190-208, :539-545) and clamps."""
     p = tmp_path / "min.json"

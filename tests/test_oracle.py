@@ -161,6 +161,57 @@ def test_glass_total_internal_reflection_with_draw_of_exactly_one(tmp_path):
     sc.close()
 
 
+@pytest.mark.parametrize("name", GOLDEN_FLAT)
+def test_closest_hit_records_match_reference_hits(name):
+    """cro_closest_hit on the camera rays of the reference's own known-answer records: semantics 0 (the reference's traversal)
+    reproduces instIndex, polyIndex and distance bit for bit, and semantics 1 (the device traversal's slab test) gives the same
+    records on those rays."""
+    sc = O.OracleScene(os.path.join(GOLDEN, name + ".crscene"))
+    h = np.fromfile(os.path.join(GOLDEN, name + ".hits.bin"), dtype=O.HIT_KAT_DTYPE)
+    rays = np.concatenate([h["o"], h["d"]], axis=1)
+    ref, c0 = sc.closest_hit(rays, O.SEM_REFERENCE)
+    assert np.array_equal(ref["inst"], h["instIndex"])
+    assert np.array_equal(ref["poly"], h["polyIndex"])
+    hit = h["instIndex"] >= 0
+    assert hit.any()
+    assert np.array_equal(ref["t"][hit].view(np.uint32), h["distance"][hit].view(np.uint32))
+    assert (ref["t"][~hit] == np.float32(np.finfo(np.float32).max)).all()
+    dev, c1 = sc.closest_hit(rays, O.SEM_DEVICE)
+    assert dev.tobytes() == ref.tobytes()
+    assert c0["rays"] == c1["rays"] == len(rays) and c0["tri_tests"] + c0["sphere_tests"] > 0
+    # the batch is split over threads: the records and the totals do not depend on how
+    one, c1b = sc.closest_hit(rays, O.SEM_DEVICE, threads=1)
+    assert one.tobytes() == dev.tobytes() and c1b == c1
+    sc.close()
+
+
+def test_device_semantics_cull_zero_direction_components_exactly():
+    """A horizon ray (d.y == +0) through the middle of the scene: the reference's slab test turns the y axis into NaNs and drops it,
+    entering every box the ray's x/z projection crosses; semantics 1 culls that axis exactly and visits fewer node pairs, with
+    the same hit.  Also -0 and a denormal direction component, which overflow 1/d to +-inf the same way."""
+    sc = O.OracleScene(os.path.join(GOLDEN, "g_legacy.crscene"))
+    o = np.fromfile(os.path.join(GOLDEN, "g_legacy.hits.bin"), dtype=O.HIT_KAT_DTYPE)["o"][0]     # the camera position
+    for dy in (0.0, -0.0, 1e-45):
+        rays = np.array([[o[0], o[1], o[2], 0.3, dy, 1.0]], np.float32)
+        r0, c0 = sc.closest_hit(rays, O.SEM_REFERENCE, threads=1)
+        r1, c1 = sc.closest_hit(rays, O.SEM_DEVICE, threads=1)
+        assert c1["node_pairs"] < c0["node_pairs"], (dy, c0, c1)
+        assert r0.tobytes() == r1.tobytes(), (dy, r0, r1)
+    sc.close()
+
+
+def test_path_rays_start_with_the_camera_ray():
+    """cro_trace_region lists every ray of every bounce of a region's paths; the first ray of a path is its camera ray."""
+    sc = O.OracleScene(os.path.join(GOLDEN, "g_single.crscene"))
+    rays = sc.path_rays(3, 2, 4, 3, passes=(1, 1))
+    k = sc.trace_kat(3, 2, 1)
+    assert 1 <= len(rays) <= sc.s.prefs.bounces
+    assert np.array_equal(rays[0].view(np.uint32), np.concatenate([k["o"], k["d"]]).view(np.uint32))
+    rec, _ = sc.closest_hit(rays[:1], O.SEM_REFERENCE)
+    assert rec["inst"][0] == k["instIndex"] and rec["poly"][0] == k["polyIndex"]
+    sc.close()
+
+
 def test_zero_bounces_is_black():
     """prefs.bounces == 0: pathTrace's loop never runs (pathtrace.c:36-59) — the reference renders an all-zero frame
     (checked against cray_ref_strict with "bounces": 0 in the JSON)."""
