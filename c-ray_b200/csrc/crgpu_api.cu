@@ -839,16 +839,18 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->fb_floats = (size_t)d.image_width * d.image_height * 3u;
 	{ void *q = nullptr; FAIL_IF(ctx_alloc(device, s->fb_floats * sizeof(float), &q)); s->fb = static_cast<float *>(q); }
 	CUS(cudaMemsetAsync(s->fb, 0, s->fb_floats * sizeof(float), s->stream));
-	{	/* per wave set: hist[1024] + counts[64]; then the shared stats[80] */
-		const size_t set_bytes = 1024 * sizeof(unsigned) + 256;
+	{	/* per wave set: hist[1024] + counts[64] + box[CRG_BOX_SLOTS][12]; then the shared stats[80] */
+		const size_t set_bytes = 1024 * sizeof(unsigned) + 256 + CRG_BOX_SLOTS * 12 * sizeof(unsigned);
 		s->small_bytes = 2 * set_bytes + 80 * sizeof(unsigned long long);
 		FAIL_IF(ctx_alloc(device, s->small_bytes, &s->small));
 		CUS(cudaMemsetAsync(s->small, 0, s->small_bytes, s->stream));
 		uint8_t *sm = static_cast<uint8_t *>(s->small);
 		s->wb.hist = reinterpret_cast<unsigned *>(sm);
 		s->wb.counts = s->wb.hist + 1024;
+		s->wb.box = s->wb.hist + 1024 + 64;
 		s->wb2.hist = reinterpret_cast<unsigned *>(sm + set_bytes);
 		s->wb2.counts = s->wb2.hist + 1024;
+		s->wb2.box = s->wb2.hist + 1024 + 64;
 		s->wb.stats = s->wb2.stats = reinterpret_cast<unsigned long long *>(sm + 2 * set_bytes);
 	}
 	{
@@ -988,7 +990,10 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 			crg_launch_bucket(wb, cur, grid, st);
 			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
 			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, grid, st);
-			if (sort_next) { crg_launch_dirsort(wb, cur ^ 1, grid, st); ++launches; }    /* K4b: the next bounce's rays by direction bin */
+			if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
+				crg_launch_dirsort(wb, cur ^ 1, dirmode == 4 ? (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1) : -1, grid, st);
+				++launches;
+			}
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
 			launches += 2 + (uint64_t)crg_shade_launches_per_bounce();
 			cur ^= 1;

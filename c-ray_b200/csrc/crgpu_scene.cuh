@@ -113,5 +113,8 @@ struct DevScene {
 	                                   TMA bulk copy (cp.async.bulk) per block; stage_pairs = number of nodes in it */
 	uint32_t          stage_pairs;
 	const float      *u8_to_unit;   /* [256]: (float)i / 255.0f, the byte→float division of texture.c:48-60 done once */
-	float             world_lo[3], world_inv[3];   /* top-level BVH bounds: lower corner and 1/extent (only used to BIN rays by origin cell, K4b) */
+	/* top-level BVH bounds: lower corner and 1/extent.  Only dir mode 3 (K4b) bins origins with them; in a scene whose box is
+	 * stretched by far geometry (hdr.json's emissive spheres, ~1500 units out) every secondary origin lands in one cell, which
+	 * is why mode 4 bins inside the bounds of the origins themselves (WaveBuffers::box) */
+	float             world_lo[3], world_inv[3];
 };

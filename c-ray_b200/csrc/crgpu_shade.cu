@@ -18,10 +18,15 @@
  *              hist[512..767], cursors hist[768..1023], output perm2): K2 hands rays to its lanes in perm2 order, so the 32 rays
  *              of a warp point into the same octant and walk the BVH in the same child order — fewer divergent steps. */
 template <bool DIR>
-__global__ void __launch_bounds__(256) k_bucket(WaveBuffers wb, int cur) {
+__global__ void __launch_bounds__(256) k_bucket(WaveBuffers wb, int cur, int box_slot) {
 	__shared__ unsigned s_base[256], s_cnt[256], s_off[256];
 	const unsigned n = wb.counts[cur];
 	const unsigned t = threadIdx.x;
+	if (DIR && box_slot >= 0 && blockIdx.x == 0u && t < 6u) {   /* K3 is done with this depth's bounds: they key the next batch */
+		unsigned *b = wb.box + 12 * box_slot;
+		b[6 + t] = b[t];
+		b[t] = 0u;
+	}
 	unsigned *__restrict__ sizes = wb.hist + (DIR ? 512 : 0);
 	unsigned *__restrict__ cursors = wb.hist + (DIR ? 768 : 256);
 	const unsigned char *__restrict__ keys = DIR ? wb.dirKey : wb.hitKey;
@@ -106,10 +111,40 @@ CRD bool cr_shade_one(const DevScene &sc, float4 *__restrict__ Lbuf, v3 o, v3 d,
 	return false;
 }
 
+/* order-preserving map of a float to an unsigned (crg_ord(a) < crg_ord(b) iff a < b for non-NaN a, b); never 0 for a finite float */
+CRD unsigned crg_ord(float f) { const unsigned u = __float_as_uint(f); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
+CRD float crg_unord(unsigned e) { return __uint_as_float((e & 0x80000000u) ? (e & 0x7fffffffu) : ~e); }
+
+/* the origin box of dir mode 4: lower corner and 4/extent per axis (0 for a zero or non-finite extent).  Invalid (valid = false)
+ * when no origin was reduced into the slot: the first batch of a wave set, or a depth no ray reached. */
+struct OriginBox { float lo[3], scale[3]; bool valid; };
+CRD OriginBox crg_origin_box(const unsigned *prev) {
+	OriginBox b;
+	b.valid = true;
+	for (int k = 0; k < 3; ++k) {
+		if (prev[k] == 0u || prev[3 + k] == 0u) { b.valid = false; b.lo[k] = 0.f; b.scale[k] = 0.f; continue; }
+		const float lo = crg_unord(~prev[k]), hi = crg_unord(prev[3 + k]);
+		const float e = hi - lo;
+		b.lo[k] = lo;
+		b.scale[k] = (e > 0.f && e < 3.0e38f) ? 4.0f / e : 0.f;
+		if (!(lo <= hi)) b.valid = false;
+	}
+	return b;
+}
+
 /* direction bin of a ray for K4b: sign octant (bvh.c:370-372 picks the near/far planes from exactly these bits), optionally
- * times the major axis.  Any binning is legal: the order rays are traced in never changes a result. */
-CRD unsigned cr_dir_bin(const DevScene &sc, v3 o, v3 d, int mode) {
+ * times the major axis or an origin cell.  Any binning is legal: the order rays are traced in never changes a result. */
+CRD unsigned cr_dir_bin(const DevScene &sc, const OriginBox &box, v3 o, v3 d, int mode) {
 	unsigned key = (__float_as_uint(d.x) >> 31) | ((__float_as_uint(d.y) >> 31) << 1) | ((__float_as_uint(d.z) >> 31) << 2);
+	if (mode == 4) {                             /* + 5-bit Morton cell: 4 x 4 x 4 cells of the box, the top 5 of 6 interleaved bits */
+		if (!box.valid) return key;
+		/* fmaxf(NaN, 0) = 0: a NaN origin or an inf * 0 lands in cell 0 */
+		const unsigned cx = (unsigned)fminf(fmaxf((o.x - box.lo[0]) * box.scale[0], 0.0f), 3.0f);
+		const unsigned cy = (unsigned)fminf(fmaxf((o.y - box.lo[1]) * box.scale[1], 0.0f), 3.0f);
+		const unsigned cz = (unsigned)fminf(fmaxf((o.z - box.lo[2]) * box.scale[2], 0.0f), 3.0f);
+		const unsigned m = (cx & 1u) | ((cy & 1u) << 1) | ((cz & 1u) << 2) | ((cx >> 1) << 3) | ((cy >> 1) << 4) | ((cz >> 1) << 5);
+		return key | ((m >> 1) << 3);
+	}
 	if (mode == 2) {
 		const float ax = fabsf(d.x), ay = fabsf(d.y), az = fabsf(d.z);
 		const unsigned major = (ax >= ay && ax >= az) ? 0u : (ay >= az ? 1u : 2u);
@@ -136,9 +171,9 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 		const unsigned n0 = wb.counts[4];
 		for (unsigned j = blockIdx.x * blockDim.x + threadIdx.x; j < n0; j += stride) {
 			const unsigned i = wb.perm[j];
-			const float4 a = wb.stA[cur][i];
-			const float4 b = wb.stB[cur][i];
-			const uint4 c = wb.stC[cur][i];
+			const float4 a = crg_half(wb.stA, cur)[i];
+			const float4 b = crg_half(wb.stB, cur)[i];
+			const uint4 c = crg_half(wb.stC, cur)[i];
 			unsigned id = c.y;
 			const col4 bg = cr_sample_background<X>(sc, v3make(a.w, b.x, b.y));                 /* pathtrace.c:39-42 */
 			cr_add_radiance(wb.L, id, b.z * bg.r, b.w * bg.g, __uint_as_float(c.x) * bg.b);
@@ -146,7 +181,11 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 		return;
 	}
 	__shared__ unsigned s_dir[256];                               /* direction-bin sizes of the rays this block writes (blockDim.x == 256) */
+	__shared__ unsigned s_box[6];                                 /* dir mode 4: bounds of the origins this block writes (WaveBuffers::box) */
 	s_dir[threadIdx.x] = 0u;
+	if (threadIdx.x < 6u) s_box[threadIdx.x] = 0u;
+	unsigned *box_acc = wb.box + 12 * (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1);
+	const OriginBox obox = dirmode == 4 ? crg_origin_box(box_acc + 6) : OriginBox{};
 	__syncthreads();
 	if (blockIdx.x == 0 && threadIdx.x == 0) wb.counts[2] = 0u;   /* K2's work counter, for the next bounce */
 	if (blockIdx.x == 0) { wb.hist[threadIdx.x] = 0u; wb.hist[256 + threadIdx.x] = 0u; }   /* K2/K4 histogram + cursors (blockDim.x == 256) */
@@ -168,12 +207,12 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 		if (j < n) {
 			const unsigned i = prefetch ? i_cur : wb.perm[j];     /* bucket order: a warp shades one material */
 			if (prefetch && j + stride < n) {
-				crg_prefetch_l2(&wb.stA[cur][i_nxt]); crg_prefetch_l2(&wb.stB[cur][i_nxt]); crg_prefetch_l2(&wb.stC[cur][i_nxt]);
+				crg_prefetch_l2(&crg_half(wb.stA, cur)[i_nxt]); crg_prefetch_l2(&crg_half(wb.stB, cur)[i_nxt]); crg_prefetch_l2(&crg_half(wb.stC, cur)[i_nxt]);
 				crg_prefetch_l2(&wb.hit[i_nxt]); crg_prefetch_l2(&wb.hitInst[i_nxt]);
 			}
-			const float4 a = wb.stA[cur][i];
-			const float4 b = wb.stB[cur][i];
-			const uint4 c = wb.stC[cur][i];
+			const float4 a = crg_half(wb.stA, cur)[i];
+			const float4 b = crg_half(wb.stB, cur)[i];
+			const uint4 c = crg_half(wb.stC, cur)[i];
 			const float4 hq = wb.hit[i];
 			Hit hit;
 			hit.t = hq.x; hit.u = hq.y; hit.v = hq.z; hit.prim = __float_as_uint(hq.w);
@@ -191,13 +230,23 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 			base = __shfl_sync(0xffffffffu, base, 0);
 			if (alive) {
 				const unsigned k = base + (unsigned)__popc(mask & ((1u << lane) - 1u));
-				wb.stA[nxt][k] = make_float4(p_next.x, p_next.y, p_next.z, d_next.x);
-				wb.stB[nxt][k] = make_float4(d_next.y, d_next.z, wr, wg);
-				wb.stC[nxt][k] = make_uint4(__float_as_uint(wbl), id, (unsigned)(rng & 0xffffffffull), (unsigned)(rng >> 32));
+				crg_half(wb.stA, nxt)[k] = make_float4(p_next.x, p_next.y, p_next.z, d_next.x);
+				crg_half(wb.stB, nxt)[k] = make_float4(d_next.y, d_next.z, wr, wg);
+				crg_half(wb.stC, nxt)[k] = make_uint4(__float_as_uint(wbl), id, (unsigned)(rng & 0xffffffffull), (unsigned)(rng >> 32));
 				if (dirmode) {
-					const unsigned key = cr_dir_bin(sc, p_next, d_next, dirmode);
+					const unsigned key = cr_dir_bin(sc, obox, p_next, d_next, dirmode);
 					wb.dirKey[k] = (unsigned char)key;
 					atomicAdd(&s_dir[key], 1u);
+				}
+			}
+			if (dirmode == 4) {              /* warp-convergent (mask is uniform): min / max of the finite origins written */
+				const bool fin = alive && isfinite(p_next.x) && isfinite(p_next.y) && isfinite(p_next.z);
+				const float pc[3] = { p_next.x, p_next.y, p_next.z };
+#pragma unroll
+				for (int c = 0; c < 3; ++c) {
+					const unsigned lo = __reduce_max_sync(0xffffffffu, fin ? ~crg_ord(pc[c]) : 0u);
+					const unsigned hi = __reduce_max_sync(0xffffffffu, fin ? crg_ord(pc[c]) : 0u);
+					if (lane == 0u && hi) { atomicMax(&s_box[c], lo); atomicMax(&s_box[3 + c], hi); }
 				}
 			}
 		}
@@ -206,6 +255,7 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 	if (dirmode) {
 		__syncthreads();
 		if (s_dir[threadIdx.x]) atomicAdd(&wb.hist[512 + threadIdx.x], s_dir[threadIdx.x]);
+		if (dirmode == 4 && threadIdx.x < 6u && s_box[threadIdx.x]) atomicMax(&box_acc[threadIdx.x], s_box[threadIdx.x]);
 	}
 }
 
@@ -223,9 +273,9 @@ __global__ void __launch_bounds__(128) k_tail(const DevScene *__restrict__ scp, 
 	const unsigned n = wb.counts[cur];
 	if (n == 0u || n > CRG_TAIL_MAX) return;
 	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-		const float4 a = wb.stA[cur][i];
-		const float4 b = wb.stB[cur][i];
-		const uint4 c = wb.stC[cur][i];
+		const float4 a = crg_half(wb.stA, cur)[i];
+		const float4 b = crg_half(wb.stB, cur)[i];
+		const uint4 c = crg_half(wb.stC, cur)[i];
 		v3 o = v3make(a.x, a.y, a.z), d = v3make(a.w, b.x, b.y);
 		float wr = b.z, wg = b.w, wbl = __uint_as_float(c.x);
 		unsigned id = c.y;
@@ -328,7 +378,7 @@ __global__ void k_kat(const DevScene *__restrict__ scp, const int32_t *__restric
 }
 
 void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st) {
-	k_bucket<false><<<grid, 256, 0, st>>>(wb, cur);
+	k_bucket<false><<<grid, 256, 0, st>>>(wb, cur, -1);
 }
 /* X (the last template argument): the scene contains node kinds only the complete interpreter knows (DevScene::has_xnodes, set at
  * upload) — every other scene runs the kernels in which that interpreter is not even linked */
@@ -360,11 +410,11 @@ void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int d
 	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, st);
 	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, st);
 }
-void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int grid, cudaStream_t st) {
-	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt);
+void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st) {
+	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot);
 }
 int crg_dir_mode(void) {
-	static const int mode = [] { const char *e = getenv("CRGPU_TRACE_SORT"); const int v = e ? atoi(e) : 0; return v >= 0 && v <= 3 ? v : 0; }();
+	static const int mode = [] { const char *e = getenv("CRGPU_TRACE_SORT"); const int v = e ? atoi(e) : 0; return v >= 0 && v <= 4 ? v : 0; }();
 	return mode;
 }
 int crg_shade_launches_per_bounce(void) { const char *e = getenv("CRGPU_SHADE_SPLIT"); return (e ? atoi(e) : 1) ? 2 : 1; }

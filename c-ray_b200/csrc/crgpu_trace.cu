@@ -55,14 +55,17 @@ __global__ void __launch_bounds__(256) k_generate(DevScene sc, WaveBuffers wb, T
 #define CRG_NODE_BURST 3
 #define CRG_STAGE_MIN_RAYS 65536u
 #define CRG_DEFER_DEFAULT 0
+/* lanes that must want an instance step before a warp takes one: on hdr.json (1080p, 1000 spp, one H100 80GB HBM3 at 700 W)
+ * 4 renders the frame 0.7% faster than 8 and 12 1.4% slower (tools/k2_order_sweep.py, DESIGN §4) */
+#define CRG_INST_MIN 4
 #define CRG_MAX_STEPS 8000000u   /* > 30x the node count of any scene that fits the 2^23-node address space we support */
 
 template <bool COUNT, int MINB, int DEFER>
 __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb, int cur, int refill, int burst, int sorted, int inst_min) {
 	const unsigned n = wb.counts[cur];
 	const unsigned lane = threadIdx.x & 31u;
-	const float4 *__restrict__ stA = wb.stA[cur];
-	const float4 *__restrict__ stB = wb.stB[cur];
+	const float4 *__restrict__ stA = crg_half(wb.stA, cur);
+	const float4 *__restrict__ stB = crg_half(wb.stB, cur);
 	TraceCounters tc = { 0u, 0u, 0u, 0u };
 	__shared__ unsigned s_hist[256];
 	__shared__ CoopScratch s_coop[DEFER == 2 ? 8 : 1];   /* one per warp (blockDim.x == 256) */
@@ -236,7 +239,7 @@ const TraceKnobs &crg_trace_knobs_env(void) {
 		k.defer = env("CRGPU_TRACE_DEFER", CRG_DEFER_DEFAULT, 0, 2);
 		k.refill = env("CRGPU_TRACE_REFILL", CRG_REFILL, 1, 32);
 		k.burst = env("CRGPU_TRACE_BURST", k.defer ? 4 : CRG_NODE_BURST, 1, 1 << 30);
-		k.inst_min = env("CRGPU_TRACE_INSTMIN", 8, 1, 32);
+		k.inst_min = env("CRGPU_TRACE_INSTMIN", CRG_INST_MIN, 1, 32);
 		return k;
 	}();
 	return kn;

@@ -35,13 +35,22 @@ struct WaveBuffers {
 	float4 *L;
 	unsigned char *hitKey;  /* shading bucket of the hit: 0 = miss, else min(material+1, 255) */
 	unsigned *perm;         /* K4 output: live indices grouped by bucket */
-	unsigned char *dirKey;  /* direction bin of every ray K3 wrote for the next bounce (octant [+ major axis]) */
+	unsigned char *dirKey;  /* direction bin of every ray K3 wrote for the next bounce (crg_dir_mode) */
 	unsigned *perm2;        /* K4b output: the next bounce's rays grouped by direction bin — the order K2 hands them to its lanes */
 	unsigned *hist;         /* [256] bucket sizes (filled by K2), [256..511] K4 cursors, [512..767] direction-bin sizes (filled by K3),
 	                           [768..1023] K4b cursors */
 	unsigned *counts;       /* [0],[1]: live counts of the ping-pong halves; [2]: K2's work counter (next ray to hand out); [3]: tail-kernel block counter; [4]: number of misses of this bounce (K4 -> K3 split) */
+	unsigned *box;          /* [CRG_BOX_SLOTS][12]: bounds of the origins K3 wrote at depth min(d, CRG_BOX_SLOTS - 1), for the origin cell of
+	                           dir mode 4.  [0..5] = this batch (lo x,y,z as ~crg_ord(lo), hi x,y,z as crg_ord(hi); atomicMax, 0 = empty),
+	                           [6..11] = the previous batch of this wave set: K3 keys its rays with those, K4b moves [0..5] there */
 	unsigned long long *stats; /* [0] rays, [1] pairs, [2] tris, [3] spheres, [4] insts */
 };
+
+/* Half h of a ping-pong state array.  Indexing the kernel-parameter array (wb.stA[cur]) with a runtime value makes the compiler
+ * copy the whole WaveBuffers parameter to local memory at kernel entry and reload every wb.* pointer from there; selecting
+ * between the two members keeps the parameter in the constant bank.  ptxas -v, stack frame / spill stores with the copy and
+ * without: k_trace<false,3,0> 768 B / 186 B and 568 B / 110 B; K3's hit kernel (k_shade<2,2,false>) 416 B / 124 B and 304 B / 170 B. */
+template <class T> __device__ __forceinline__ T *crg_half(T *const (&a)[2], int h) { return h ? a[1] : a[0]; }
 
 struct TileDesc {
 	int x0, y0, tw, th;     /* tile origin and size (pixels); y up */
@@ -72,8 +81,12 @@ void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDe
 void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, const TraceKnobs &kn, cudaStream_t st);
 /* per-ray records of K2's write-back (crgpu_trace_rays): t, u, v, instance, poly (-1 for spheres and misses), key */
 void crg_launch_trace_records(const DevScene &sc, const WaveBuffers &wb, unsigned n, void *out, int grid, cudaStream_t st);
-void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int grid, cudaStream_t st);
-int crg_dir_mode(void);   /* 0 = off, 1 = octant (8 bins), 2 = octant x major axis (24 bins), 3 = octant x origin cell (256 bins) */
+#define CRG_BOX_SLOTS 32
+/* box_slot: the depth slot whose bounds K4b moves to the previous-batch half (dir mode 4), or -1 */
+void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st);
+/* 0 = off, 1 = octant (8 bins), 2 = octant x major axis (24 bins), 3 = octant x origin cell in the world box (256 bins),
+ * 4 = octant x 5-bit Morton cell of the origin in the bounds of the previous batch's origins at the same depth (256 bins) */
+int crg_dir_mode(void);
 void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st);
 void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, bool xnodes, cudaStream_t st);
 void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid, cudaStream_t st);
