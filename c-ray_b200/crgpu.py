@@ -61,7 +61,7 @@ RAY_RECORD_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("inst", 
                              ("prim", "<u4"), ("pad", "<u4")])
 assert RAY_RECORD_DTYPE.itemsize == 32
 # the frame path's defaults (crg_trace_knobs_env); burst is 4 when leaves are deferred
-TRACE_DEFAULTS = dict(count=0, minb=3, defer=0, refill=16, burst=3, inst_min=4)
+TRACE_DEFAULTS = dict(count=0, minb=4, defer=0, refill=16, burst=3, inst_min=4)
 
 _lib = None
 

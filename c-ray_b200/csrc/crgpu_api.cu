@@ -138,7 +138,7 @@ extern "C" void crgpu_host_free(void *p) { if (p) cudaFreeHost(p); }
  * crgpu_prepare() does everything about a scene that does not depend on the device: validation, BVH re-layout into pair nodes,
  * triangle packing, shading records.  crgpu_scene_create_prepared() is then one host->device copy of the slab plus two small
  * pointer-carrying tables.  A host that renders many frames of one scene, or one frame on many GPUs, prepares once. */
-enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_SPOLYS, SEC_TOP_PRIMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_NODES, SEC_TEXS, SEC_LUT, SEC_TEXDATA, SEC_COUNT };
+enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_PRIMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_NODES, SEC_TEXS, SEC_LUT, SEC_TEXDATA, SEC_COUNT };
 struct crgpu_prepared {
 	crs_prefs prefs;
 	crs_camera camera;
@@ -148,6 +148,7 @@ struct crgpu_prepared {
 	float world_lo[3], world_inv[3];
 	uint32_t stage_pairs;
 	uint32_t texture_count;
+	size_t key_inst_off;       /* the instance keys follow the prim-slot keys in SEC_KEYS */
 	bool xnodes;               /* some node is of a kind only the complete interpreter (NodeX) evaluates */
 	uint8_t *slab;
 	bool pinned;
@@ -729,14 +730,25 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 			p->world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
 		}
 	}
+	/* shading keys (K4's buckets): min(material + 1, 255) per prim slot from its poly, then per instance for spheres */
+	std::vector<uint8_t> keys((size_t)total_slots + f->instance_count, 0u);
+	{
+		auto key_of = [](uint32_t material) { return (uint8_t)(material + 1u < 255u ? material + 1u : 255u); };
+		host_parallel_for((uint32_t)total_slots, [&](uint32_t lo, uint32_t hi) {
+			for (uint32_t i = lo; i < hi; ++i) keys[i] = key_of(spolys[slot_poly[i]].material);
+		});
+		for (uint32_t i = 0; i < f->instance_count; ++i)
+			if (insts[i].kind == CRS_INST_SPHERE) keys[(size_t)total_slots + i] = key_of(insts[i].material);
+	}
+	p->key_inst_off = (size_t)total_slots;
 	std::vector<float> lut(256);
 	for (int i = 0; i < 256; ++i) { volatile float num = (float)i, den = 255.0f; lut[i] = num / den; }   /* IEEE divss == __fdiv_rn */
 
 	/* lay the sections out in one slab (256-byte aligned each) and copy them in on the host threads */
-	const void *src[SEC_COUNT] = { stage.data(), pairs.data(), tris.data(), slot_poly.data(), spolys.data(), top_prims.data(), bvhs.data(),
+	const void *src[SEC_COUNT] = { stage.data(), pairs.data(), tris.data(), slot_poly.data(), keys.data(), spolys.data(), top_prims.data(), bvhs.data(),
 								   insts.data(), mats.data(), nodes.data(), texs.data(), lut.data(), f->texdata };
 	const size_t len[SEC_COUNT] = { stage.size() * sizeof(PairNode), pairs.size() * sizeof(PairNode), tris.size() * sizeof(PackedTri),
-									slot_poly.size() * sizeof(uint32_t), spolys.size() * sizeof(ShadePoly), top_prims.size() * sizeof(int32_t),
+									slot_poly.size() * sizeof(uint32_t), keys.size(), spolys.size() * sizeof(ShadePoly), top_prims.size() * sizeof(int32_t),
 									bvhs.size() * sizeof(DevBvh), insts.size() * sizeof(DevInstance), mats.size() * sizeof(DevMaterial),
 									nodes.size() * sizeof(crs_node), texs.size() * sizeof(DevTexture), lut.size() * sizeof(float), (size_t)f->texdata_bytes };
 	size_t total = 0;
@@ -824,6 +836,8 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	d.pairs = reinterpret_cast<const PairNode *>(base + p->off[SEC_PAIRS]);
 	d.tris = reinterpret_cast<const PackedTri *>(base + p->off[SEC_TRIS]);
 	d.slot_poly = reinterpret_cast<const uint32_t *>(base + p->off[SEC_SLOT_POLY]);
+	d.slot_key = reinterpret_cast<const uint8_t *>(base + p->off[SEC_KEYS]);
+	d.inst_key = d.slot_key + p->key_inst_off;
 	d.spolys = reinterpret_cast<const ShadePoly *>(base + p->off[SEC_SPOLYS]);
 	d.top_prims = reinterpret_cast<const int32_t *>(base + p->off[SEC_TOP_PRIMS]);
 	d.bvhs = reinterpret_cast<const DevBvh *>(base + p->off[SEC_BVHS]);

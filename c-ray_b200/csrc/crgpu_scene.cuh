@@ -102,6 +102,8 @@ struct DevScene {
 	const PairNode   *pairs;
 	const PackedTri  *tris;
 	const uint32_t   *slot_poly;    /* prim slot -> global poly index */
+	const uint8_t    *slot_key;     /* prim slot -> shading key min(material + 1, 255) of its poly (K2's write-back: one load per hit) */
+	const uint8_t    *inst_key;     /* instance -> shading key of a sphere instance (0 for meshes) */
 	const ShadePoly  *spolys;
 	const int32_t    *top_prims;    /* top-level primIndices (instance indices) */
 	const DevBvh     *bvhs;

@@ -76,13 +76,12 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 	__syncthreads();
 	/* ---- stage the top-of-tree pair nodes into shared memory: one TMA bulk copy (cp.async.bulk, SASS UBLKCP) per
 	 *      block, completion signalled on an mbarrier; skipped for the small tail launches where it cannot pay off */
-	extern __shared__ __align__(128) unsigned char s_dyn[];
 	__shared__ __align__(8) unsigned long long s_mbar;
-	const PairNode *snodes = nullptr;
+	bool staged = false;
 	if (sc.stage_pairs && n >= CRG_STAGE_MIN_RAYS) {
 		const unsigned bytes = sc.stage_pairs * (unsigned)sizeof(PairNode);
 		const unsigned mbar = (unsigned)__cvta_generic_to_shared(&s_mbar);
-		const unsigned dst = (unsigned)__cvta_generic_to_shared(s_dyn);
+		const unsigned dst = (unsigned)__cvta_generic_to_shared(crg_stage_smem);
 		if (threadIdx.x == 0) {
 			asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
 			asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -98,13 +97,11 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 			asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
 						 : "=r"(ok) : "r"(mbar) : "memory");
 		}
-		snodes = reinterpret_cast<const PairNode *>(s_dyn);
+		staged = true;
 	}
-	uint32_t stack[2 * CRG_MAX_STACK + 2];
+	uint32_t ovf[CRG_OVF];           /* the traversal stack below its top CRG_SSTACK entries (those are in shared memory) */
 	Traversal<COUNT> tr;
-	tr.stack = stack;
-	tr.snodes = snodes;
-	tr.begin(sc, v3make(0.f, 0.f, 0.f), v3make(0.f, 0.f, 1.f));   /* every lane holds a VALID (idle) state from the start */
+	tr.begin(sc, v3make(0.f, 0.f, 0.f), v3make(0.f, 0.f, 1.f), staged);   /* every lane holds a VALID (idle) state from the start */
 	bool busy = false;
 	bool exhausted = false;          /* warp-uniform: the work counter ran past n */
 	unsigned ray = 0u;
@@ -125,7 +122,7 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 				const float4 b = stB[i];
 				ray = i;
 				steps = 0u;
-				tr.begin(sc, v3make(a.x, a.y, a.z), v3make(a.w, b.x, b.y));
+				tr.begin(sc, v3make(a.x, a.y, a.z), v3make(a.w, b.x, b.y), staged);
 				busy = true;
 			}
 			active = __ballot_sync(0xffffffffu, busy);
@@ -138,7 +135,7 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 		for (int k = 0; k < burst; ++k) {
 			const bool wn = busy && tr.wants_node();
 			if (!__any_sync(0xffffffffu, wn)) break;
-			if (wn) { tr.template node_step<DEFER != 0>(sc, &tc); ++steps; }
+			if (wn) { tr.template node_step<DEFER != 0>(sc, ovf, &tc); ++steps; }
 		}
 		/* Phase T (DEFER): the triangles of every lane that reached a leaf during the burst, together */
 		if (DEFER == 2) cr_coop_leaves<COUNT>(tr, busy && tr.wants_leaf(), sc, s_coop[threadIdx.x >> 5], lane, &tc);   /* dealt over the warp */
@@ -158,16 +155,11 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 		}
 		/* Phase W: write back finished rays */
 		if (busy && tr.done()) {
-			wb.hit[ray] = make_float4(tr.best.t, tr.best.u, tr.best.v, __uint_as_float(tr.best.prim));
-			wb.hitInst[ray] = tr.best.inst;
-			unsigned key = 0u;                                   /* shading bucket for K4/K3 */
-			if (tr.best.inst >= 0) {
-				const DevInstance *inst = sc.instances + tr.best.inst;
-				unsigned material;
-				if (__ldg(&inst->kind) == CRS_INST_MESH) material = __ldg(&sc.spolys[__ldg(sc.slot_poly + tr.best.prim)].material);
-				else material = __ldg(&inst->material);
-				key = material + 1u < 255u ? material + 1u : 255u;
-			}
+			const Hit best = tr.result();
+			wb.hit[ray] = make_float4(best.t, best.u, best.v, __uint_as_float(best.prim));
+			wb.hitInst[ray] = best.inst;
+			unsigned key = 0u;                                   /* shading bucket for K4/K3: one byte load (DevScene::slot_key) */
+			if (best.inst >= 0) key = (tr.flags & CRG_TF_SPHERE) ? __ldg(sc.inst_key + best.inst) : __ldg(sc.slot_key + best.prim);
 			wb.hitKey[ray] = (unsigned char)key;
 			atomicAdd(&s_hist[key], 1u);
 			busy = false;
@@ -197,9 +189,12 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st) {
 	k_generate<<<grid, 256, 0, st>>>(sc, wb, td);
 }
-/* K2 is persistent: the grid is exactly the number of blocks the device can keep resident.  MINB (blocks per SM
- * the compiler must make room for: 2 -> <=128 registers, 3 -> <=80, 4 -> <=64) trades registers for latency-hiding warps;
- * CRGPU_TRACE_MINB=2|3 overrides the default for experiments. */
+/* K2 is persistent: the grid is exactly the number of blocks the device can keep resident (the occupancy query below also
+ * counts the staged nodes' dynamic shared memory, so CRGPU_TRACE_STAGE=1024 gets fewer blocks).  MINB (blocks per SM the compiler
+ * must make room for: 2 -> <=128 registers, 3 -> <=80, 4 -> <=64) trades registers for latency-hiding warps.  K2 is bound by
+ * latency, and with its cold state and the top of its stack in shared memory it runs at 64 registers with 30 B of spills, so the
+ * default is 4 (32 warps per SM): on hdr.json (1080p, 1000 spp, one H100 80GB HBM3 at 400 W) 4 traces the frame in 854 ms, 3 in
+ * 901 ms (DESIGN §4).  CRGPU_TRACE_MINB=2|3 selects the others. */
 #ifndef CRG_MAX_DEVICES
 #define CRG_MAX_DEVICES 64
 #endif
@@ -235,7 +230,7 @@ const TraceKnobs &crg_trace_knobs_env(void) {
 	static const TraceKnobs kn = [] {
 		auto env = [](const char *name, int dflt, int lo, int hi) { const char *e = getenv(name); const int v = e ? atoi(e) : dflt; return v >= lo && v <= hi ? v : dflt; };
 		TraceKnobs k;
-		k.minb = env("CRGPU_TRACE_MINB", 3, 2, 4);
+		k.minb = env("CRGPU_TRACE_MINB", 4, 2, 4);
 		k.defer = env("CRGPU_TRACE_DEFER", CRG_DEFER_DEFAULT, 0, 2);
 		k.refill = env("CRGPU_TRACE_REFILL", CRG_REFILL, 1, 32);
 		k.burst = env("CRGPU_TRACE_BURST", k.defer ? 4 : CRG_NODE_BURST, 1, 1 << 30);

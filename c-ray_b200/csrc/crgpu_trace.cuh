@@ -61,20 +61,25 @@ CRD void cr_camera_ray(const DevCamera &cam, int x, int y, uint64_t &rng, v3 &o,
 }
 
 /* ---- bvh.c:326-352 -------------------------------------------------------------------------------------------- */
+/* bits of RaySetup::bits (and of the low byte of Traversal::flags, which holds the current level's copy) */
+#define CRG_RS_OX   1u      /* d.x has its sign bit set (bvh.c:369-371) */
+#define CRG_RS_OY   2u
+#define CRG_RS_OZ   4u
+#define CRG_RS_DEG  3       /* bits 3..5: bit 3+a set when -o[a]/d[a] is not finite (1/d[a] is +-inf, or o[a]*(1/d[a]) overflows) — see cr_node_test */
+#define CRG_RS_MASK 0x3fu
+
 struct RaySetup {
 	v3 invDir, scaledStart;
-	bool ox, oy, oz;
-	unsigned deg;      /* bit a set: -o[a]/d[a] is not finite (1/d[a] is +-inf, or o[a]*(1/d[a]) overflows) — see cr_node_test */
+	unsigned bits;     /* CRG_RS_* */
 };
 
 CRD RaySetup cr_ray_setup(v3 o, v3 d) {                                                /* bvh.c:369-376 */
 	RaySetup s;
-	s.ox = (__float_as_uint(d.x) >> 31) != 0u;
-	s.oy = (__float_as_uint(d.y) >> 31) != 0u;
-	s.oz = (__float_as_uint(d.z) >> 31) != 0u;
 	s.invDir = v3make(cr_div(1.0f, d.x), cr_div(1.0f, d.y), cr_div(1.0f, d.z));
 	s.scaledStart = v3scale(v3mul(o, s.invDir), -1.0f);
-	s.deg = (isfinite(s.scaledStart.x) ? 0u : 1u) | (isfinite(s.scaledStart.y) ? 0u : 2u) | (isfinite(s.scaledStart.z) ? 0u : 4u);
+	s.bits = (__float_as_uint(d.x) >> 31) | ((__float_as_uint(d.y) >> 31) << 1) | ((__float_as_uint(d.z) >> 31) << 2) |
+			 ((isfinite(s.scaledStart.x) ? 0u : 1u) << CRG_RS_DEG) | ((isfinite(s.scaledStart.y) ? 0u : 2u) << CRG_RS_DEG) |
+			 ((isfinite(s.scaledStart.z) ? 0u : 4u) << CRG_RS_DEG);
 	return s;
 }
 
@@ -108,18 +113,20 @@ CRD RaySetup cr_ray_setup(v3 o, v3 d) {                                         
  * a superset of the exact one and the Möller–Trumbore test decides every hit on its own, so the closest
  * hit is the same; they could only differ for a ray that grazes a triangle within one ulp of its leaf's
  * bounding box.  All other rays take the verbatim path. */
-CRD bool cr_node_test(const float *b, const RaySetup &r, v3 o, float maxDist, float &tEntry) {
-	float tMinX = CR_SLAB_MAD((r.ox ? b[1] : b[0]), r.invDir.x, r.scaledStart.x);
-	float tMaxX = CR_SLAB_MAD((r.ox ? b[0] : b[1]), r.invDir.x, r.scaledStart.x);
-	float tMinY = CR_SLAB_MAD((r.oy ? b[3] : b[2]), r.invDir.y, r.scaledStart.y);
-	float tMaxY = CR_SLAB_MAD((r.oy ? b[2] : b[3]), r.invDir.y, r.scaledStart.y);
-	float tMinZ = CR_SLAB_MAD((r.oz ? b[5] : b[4]), r.invDir.z, r.scaledStart.z);
-	float tMaxZ = CR_SLAB_MAD((r.oz ? b[4] : b[5]), r.invDir.z, r.scaledStart.z);
-	if (r.deg) {
+CRD bool cr_node_test(const float *b, v3 invDir, v3 scaledStart, unsigned bits, v3 o, float maxDist, float &tEntry) {
+	const bool ox = (bits & CRG_RS_OX) != 0u, oy = (bits & CRG_RS_OY) != 0u, oz = (bits & CRG_RS_OZ) != 0u;
+	float tMinX = CR_SLAB_MAD((ox ? b[1] : b[0]), invDir.x, scaledStart.x);
+	float tMaxX = CR_SLAB_MAD((ox ? b[0] : b[1]), invDir.x, scaledStart.x);
+	float tMinY = CR_SLAB_MAD((oy ? b[3] : b[2]), invDir.y, scaledStart.y);
+	float tMaxY = CR_SLAB_MAD((oy ? b[2] : b[3]), invDir.y, scaledStart.y);
+	float tMinZ = CR_SLAB_MAD((oz ? b[5] : b[4]), invDir.z, scaledStart.z);
+	float tMaxZ = CR_SLAB_MAD((oz ? b[4] : b[5]), invDir.z, scaledStart.z);
+	const unsigned deg = (bits >> CRG_RS_DEG) & 7u;
+	if (deg) {
 		const float inf = __int_as_float(0x7f800000);
-		if (r.deg & 1u) { const bool in = (b[0] <= o.x) && (o.x <= b[1]); tMinX = in ? -inf : inf; tMaxX = in ? inf : -inf; }
-		if (r.deg & 2u) { const bool in = (b[2] <= o.y) && (o.y <= b[3]); tMinY = in ? -inf : inf; tMaxY = in ? inf : -inf; }
-		if (r.deg & 4u) { const bool in = (b[4] <= o.z) && (o.z <= b[5]); tMinZ = in ? -inf : inf; tMaxZ = in ? inf : -inf; }
+		if (deg & 1u) { const bool in = (b[0] <= o.x) && (o.x <= b[1]); tMinX = in ? -inf : inf; tMaxX = in ? inf : -inf; }
+		if (deg & 2u) { const bool in = (b[2] <= o.y) && (o.y <= b[3]); tMinY = in ? -inf : inf; tMaxY = in ? inf : -inf; }
+		if (deg & 4u) { const bool in = (b[4] <= o.z) && (o.z <= b[5]); tMinZ = in ? -inf : inf; tMaxZ = in ? inf : -inf; }
 	}
 	float tMin = tMinX > tMinY ? tMinX : tMinY;
 	float tMax = tMaxX < tMaxY ? tMaxX : tMaxY;
@@ -131,39 +138,14 @@ CRD bool cr_node_test(const float *b, const RaySetup &r, v3 o, float maxDist, fl
 	return tMin <= tMax;
 }
 
-/* rayIntersectsWithPolygon over one leaf (bvh.c:443-462 + poly.c:17-53); tris already offset to the BVH's first slot */
+/* rayIntersectsWithPolygon over two leaves back to back (bvh.c:443-462 + poly.c:17-53): slots [firstA, firstA+nA) then
+ * [firstB, firstB+nB), local to the BVH whose first slot is slot_base.  Only the distance of the closest hit is a register;
+ * its u, v and slot are written to the caller's cold state (shared memory) when a triangle wins. */
 template <bool COUNT>
-CRD bool cr_leaf_tris(const PackedTri *__restrict__ tris, uint32_t slot_base, uint32_t first, uint32_t count,
-					  v3 o, v3 d, Hit &best, TraceCounters *ctr) {
+CRD bool cr_leaf_tris(const DevScene &sc, uint32_t slot_base, uint32_t firstA, uint32_t nA, uint32_t firstB, uint32_t nB,
+					  v3 o, v3 d, float &bestT, float &bestU, float &bestV, uint32_t &bestPrim, TraceCounters *ctr) {
 	bool found = false;
-	for (uint32_t i = 0; i < count; ++i) {
-		const float4 *t4 = reinterpret_cast<const float4 *>(tris + first + i);
-		const float4 a = __ldg(t4 + 0), b = __ldg(t4 + 1), c4 = __ldg(t4 + 2);
-		if (COUNT) ctr->tris++;
-		const v3 v0 = v3make(a.x, a.y, a.z), e1 = v3make(a.w, b.x, b.y), e2 = v3make(b.z, b.w, c4.x);
-		const v3 n = v3make(c4.y, c4.z, c4.w);
-		const v3 c = v3sub(v0, o);
-		const v3 r = v3cross(d, c);
-		const float invDet = cr_div(1.0f, v3dot(n, d));
-		const float u = v3dot(r, e2) * invDet;
-		const float v = v3dot(r, e1) * invDet;
-		if (u >= 0.0f && v >= 0.0f && u + v <= 1.0f) {
-			const float t = v3dot(n, c) * invDet;
-			if (t >= 0.0f && t < best.t) {
-				best.t = t; best.u = u; best.v = v;
-				best.prim = slot_base + first + i;
-				found = true;
-			}
-		}
-	}
-	return found;
-}
-
-/* two leaves back to back: slots [firstA, firstA+nA) then [firstB, firstB+nB) */
-template <bool COUNT>
-CRD bool cr_leaf_tris2(const PackedTri *__restrict__ tris, uint32_t slot_base, uint32_t firstA, uint32_t nA, uint32_t firstB, uint32_t nB,
-					   v3 o, v3 d, Hit &best, TraceCounters *ctr) {
-	bool found = false;
+	const PackedTri *__restrict__ tris = sc.tris + slot_base;
 	const uint32_t total = nA + nB;
 	for (uint32_t k = 0; k < total; ++k) {
 		const uint32_t slot = k < nA ? firstA + k : firstB + (k - nA);
@@ -179,9 +161,9 @@ CRD bool cr_leaf_tris2(const PackedTri *__restrict__ tris, uint32_t slot_base, u
 		const float v = v3dot(r, e1) * invDet;
 		if (u >= 0.0f && v >= 0.0f && u + v <= 1.0f) {
 			const float t = v3dot(n, c) * invDet;
-			if (t >= 0.0f && t < best.t) {
-				best.t = t; best.u = u; best.v = v;
-				best.prim = slot_base + slot;
+			if (t >= 0.0f && t < bestT) {
+				bestT = t; bestU = u; bestV = v;
+				bestPrim = slot_base + slot;
 				found = true;
 			}
 		}
@@ -226,66 +208,141 @@ CRD void cr_object_ray(const float *Ainv, float ray_offset, v3 o, v3 d, v3 &oo, 
  * pushed; instances of a leaf in primIndices order; strict t < distance for triangles, t <= distance
  * for spheres.  The reference's `maxDist` copies always equal isect->distance at the time of a node
  * test (they are refreshed after every leaf that found something), so best.t is used directly. */
+/* Where the traversal state lives.  K2 is bound by latency and pays for every resident warp (DESIGN §4), so a lane keeps only
+ * what the hot loop touches in registers: best.t, the current level's ray and slab setup, node, sp/spBase, the pending-leaf cursors
+ * and one flags word.  The rest is per-thread shared memory, laid out [field][thread] so that a warp's 32 accesses to one field
+ * fall into 32 different banks:
+ *   - the top CRG_SSTACK entries of the traversal stack (deeper entries spill to a thread-local array that is touched only
+ *     when a lane's stack is that deep);
+ *   - cold state: the world ray (read by an instance step and on the way back from a mesh), u, v, prim slot and instance of the
+ *     closest hit (written on a hit, read at write-back), the top-level node to resume after a mesh and the mesh's instance.
+ * Every kernel that runs a Traversal has at most CRG_TRAV_NT threads per block. */
+#define CRG_SSTACK  8
+#define CRG_OVF     (2 * CRG_MAX_STACK + 2)   /* capacity of the whole stack: CRG_MAX_STACK entries per level */
+#define CRG_TRAV_NT 256
+
+struct TravShared {
+	uint32_t stack[CRG_SSTACK][CRG_TRAV_NT];
+	float wo[3][CRG_TRAV_NT], wd[3][CRG_TRAV_NT];   /* world ray */
+	float u[CRG_TRAV_NT], v[CRG_TRAV_NT];           /* closest hit so far */
+	uint32_t prim[CRG_TRAV_NT];                     /* its global prim slot (a triangle) */
+	int inst[CRG_TRAV_NT];                          /* its instance, -1 = miss */
+	uint32_t topNext[CRG_TRAV_NT];                  /* top-level node to resume when the current mesh is exhausted */
+	int curInst[CRG_TRAV_NT];                       /* the mesh instance being traversed */
+};
+
+/* the block's staged top-of-tree pair nodes (K2's dynamic shared memory, DevScene.stage_img); read only where Traversal::flags has CRG_TF_STAGED */
+extern __shared__ __align__(128) unsigned char crg_stage_smem[];
+
+/* bits of Traversal::flags above the current level's CRG_RS_* bits */
+#define CRG_TF_BOTTOM  0x40u    /* in a mesh BVH */
+#define CRG_TF_INSTHIT 0x80u    /* a triangle of the current mesh won */
+#define CRG_TF_STAGED  0x100u   /* the block staged the top of every BVH in crg_stage_smem */
+#define CRG_TF_SPHERE  0x200u   /* the closest hit's instance is a sphere (selects the shading-key table) */
+#define CRG_TF_BUSY    0x400u   /* K2: the lane holds a ray */
+
 template <bool COUNT>
 struct Traversal {
-	Hit best;
-	v3 wo, wd;             /* world ray */
+	float bestT;
 	v3 o, d;               /* ray of the current level */
-	RaySetup rs;
-	const PairNode *__restrict__ base;
-	const PairNode *snodes;        /* shared-memory copy of DevScene.stage_img (NULL: not staged) */
-	uint32_t stageBase, stageCount;/* nodes [0, stageCount) of the current BVH live at snodes[stageBase + node] */
-	const PackedTri *__restrict__ tris;
-	uint32_t slotBase, node, topNext;
+	v3 invDir, scaledStart;/* its slab setup (RaySetup); the sign and degenerate-axis bits are in flags */
+	uint32_t flags;        /* CRG_RS_* | CRG_TF_* */
+	uint32_t pairOff;      /* first pair node of the current BVH in sc.pairs */
+	uint32_t stageBase, stageCount;/* nodes [0, stageCount) of the current BVH live at crg_stage_smem[stageBase + node]; 0 when not staged */
+	uint32_t slotBase, node;
 	uint32_t pendA, cntA, pendB, cntB;     /* pending top-level leaf items: A (left leaf) before B (right leaf) */
 	uint32_t leafA, leafB, leafN;          /* DEFER: bottom-level leaf triangles not yet tested — slots [leafA, +nA) then [leafB, +nB), leafN = nA | nB << 16 */
-	int sp, spBase, curInst;
-	bool bottom, instHit;
-	uint32_t *stack;       /* 2*CRG_MAX_STACK+2 entries of thread-local memory, owned by the caller (keeps the scalars in registers) */
+	int sp, spBase;
 
-	CRD bool done() const { return !bottom && (cntA | cntB) == 0u && node == CRG_END && leafN == 0u; }
+	CRD static TravShared &sh() { __shared__ TravShared s; return s; }
+	CRD static unsigned tid() { return threadIdx.x; }
 
-	CRD void begin(const DevScene &sc, v3 ro, v3 rd) {
-		best.t = CR_FLT_MAX; best.u = 0.0f; best.v = 0.0f; best.inst = -1; best.prim = 0u;
-		wo = ro; wd = rd; o = ro; d = rd;
-		rs = cr_ray_setup(o, d);
-		base = sc.pairs + sc.top.pair_offset;
-		stageBase = sc.top.stage_base; stageCount = snodes ? sc.top.stage_count : 0u;
-		tris = sc.tris;
-		slotBase = 0u; node = 0u; topNext = CRG_END;
+	/* ovf: the caller's thread-local array of CRG_OVF entries, indexed by depth, for the entries at depth >= CRG_SSTACK.  It is
+	 * a local of the calling kernel rather than a member: an array member with a runtime index would keep the whole struct
+	 * in local memory. */
+	CRD void push(uint32_t v, uint32_t *ovf) {
+		if (sp < CRG_SSTACK) sh().stack[sp][tid()] = v;
+		else ovf[sp] = v;
+		++sp;
+	}
+	CRD uint32_t pop(const uint32_t *ovf) {
+		--sp;
+		return sp < CRG_SSTACK ? sh().stack[sp][tid()] : ovf[sp];
+	}
+
+	CRD bool bottom() const { return (flags & CRG_TF_BOTTOM) != 0u; }
+	CRD bool done() const { return !bottom() && (cntA | cntB) == 0u && node == CRG_END && leafN == 0u; }
+
+	CRD void set_ray(v3 ro, v3 rd) {
+		o = ro; d = rd;
+		const RaySetup rs = cr_ray_setup(o, d);
+		invDir = rs.invDir; scaledStart = rs.scaledStart;
+		flags = (flags & ~CRG_RS_MASK) | rs.bits;
+	}
+	CRD void set_top(const DevScene &sc) {
+		pairOff = sc.top.pair_offset;
+		stageBase = sc.top.stage_base; stageCount = (flags & CRG_TF_STAGED) ? sc.top.stage_count : 0u;
+	}
+
+	/* staged: the block holds DevScene.stage_img in crg_stage_smem */
+	CRD void begin(const DevScene &sc, v3 ro, v3 rd, bool staged) {
+		TravShared &s = sh();
+		const unsigned t = tid();
+		bestT = CR_FLT_MAX; s.u[t] = 0.0f; s.v[t] = 0.0f; s.inst[t] = -1; s.prim[t] = 0u;
+		s.wo[0][t] = ro.x; s.wo[1][t] = ro.y; s.wo[2][t] = ro.z;
+		s.wd[0][t] = rd.x; s.wd[1][t] = rd.y; s.wd[2][t] = rd.z;
+		flags = staged ? CRG_TF_STAGED : 0u;
+		set_ray(ro, rd);
+		set_top(sc);
+		slotBase = 0u; node = 0u; s.topNext[t] = CRG_END;
 		pendA = 0u; cntA = 0u; pendB = 0u; cntB = 0u;
-		sp = 0; spBase = 0; curInst = -1;
-		bottom = false; instHit = false;
+		sp = 0; spBase = 0; s.curInst[t] = -1;
 		leafA = 0u; leafB = 0u; leafN = 0u;
 		if (sc.top.node_count < 1) {                                               /* bvh.c:362-365 */
 			node = CRG_END;
 		} else if (sc.top.node_count == 1) {                                       /* bvh.c:382-387 */
 			float te;
 			node = CRG_END;
-			if (cr_node_test(sc.top.root_bounds, rs, o, best.t, te)) { pendA = sc.top.root_first; cntA = sc.top.root_count; }
+			if (cr_node_test(sc.top.root_bounds, invDir, scaledStart, flags, o, bestT, te)) { pendA = sc.top.root_first; cntA = sc.top.root_count; }
 		}
 	}
 
-	CRD bool wants_node() const { return leafN == 0u && (bottom || ((cntA | cntB) == 0u && node != CRG_END)); }
+	CRD bool wants_node() const { return leafN == 0u && (bottom() || ((cntA | cntB) == 0u && node != CRG_END)); }
 	CRD bool wants_leaf() const { return leafN != 0u; }
-	CRD bool wants_instance() const { return !bottom && (cntA | cntB) != 0u; }
+	CRD bool wants_instance() const { return !bottom() && (cntA | cntB) != 0u; }
+
+	/* the closest hit, once done() */
+	CRD Hit result() const {
+		const TravShared &s = sh();
+		const unsigned t = tid();
+		Hit h;
+		h.t = bestT; h.u = s.u[t]; h.v = s.v[t]; h.inst = s.inst[t]; h.prim = s.prim[t];
+		return h;
+	}
 
 	/* one iteration of the flat loop; precondition: !done() */
-	CRD void step(const DevScene &sc, TraceCounters *ctr) {
-		if (bottom || (cntA | cntB) == 0u) node_step(sc, ctr);
+	CRD void step(const DevScene &sc, uint32_t *ovf, TraceCounters *ctr) {
+		if (bottom() || (cntA | cntB) == 0u) node_step(sc, ovf, ctr);
 		else instance_step(sc, ctr);
+	}
+
+	/* triangles of the current mesh: slots [firstA, +nA) then [firstB, +nB) */
+	CRD void leaf_tris(const DevScene &sc, uint32_t firstA, uint32_t nA, uint32_t firstB, uint32_t nB, TraceCounters *ctr) {
+		TravShared &s = sh();
+		const unsigned t = tid();
+		if (cr_leaf_tris<COUNT>(sc, slotBase, firstA, nA, firstB, nB, o, d, bestT, s.u[t], s.v[t], s.prim[t], ctr)) flags |= CRG_TF_INSTHIT;
 	}
 
 	/* the tail of a bottom-level step: once the mesh BVH is exhausted, back to the top level (instance.c:175-184) */
 	CRD void finish_bottom(const DevScene &sc) {
 		if (node == CRG_END) {
-			if (instHit) best.inst = curInst;
-			bottom = false;
-			o = wo; d = wd;
-			rs = cr_ray_setup(o, d);
-			base = sc.pairs + sc.top.pair_offset;
-			stageBase = sc.top.stage_base; stageCount = snodes ? sc.top.stage_count : 0u;
-			node = topNext;
+			TravShared &s = sh();
+			const unsigned t = tid();
+			if (flags & CRG_TF_INSTHIT) { s.inst[t] = s.curInst[t]; flags &= ~CRG_TF_SPHERE; }
+			flags &= ~CRG_TF_BOTTOM;
+			set_ray(v3make(s.wo[0][t], s.wo[1][t], s.wo[2][t]), v3make(s.wd[0][t], s.wd[1][t], s.wd[2][t]));
+			set_top(sc);
+			node = s.topNext[t];
 			spBase = 0;
 		}
 	}
@@ -295,24 +352,24 @@ struct Traversal {
 	 * those of the in-line version; only the warp's interleaving differs: lanes that reached a leaf WAIT, and all waiting lanes of
 	 * the warp test their triangles together after the node burst (K2 warp model, policy "leaves wait"). */
 	CRD void leaf_step(const DevScene &sc, TraceCounters *ctr) {
-		instHit |= cr_leaf_tris2<COUNT>(tris, slotBase, leafA, leafN & 0xffffu, leafB, leafN >> 16, o, d, best, ctr);
+		leaf_tris(sc, leafA, leafN & 0xffffu, leafB, leafN >> 16, ctr);
 		leafN = 0u;
 		finish_bottom(sc);
 	}
 
 	/* precondition: wants_node().  DEFER = true: leaf triangles are left pending for leaf_step() */
 	template <bool DEFER = false>
-	CRD void node_step(const DevScene &sc, TraceCounters *ctr) {
+	CRD void node_step(const DevScene &sc, uint32_t *ovf, TraceCounters *ctr) {
 		{
 			/* ---- one child-pair step (bvh.c:391-439) */
 			float4 q0, q1, q2;
 			uint4 q3;
 			if (node < stageCount) {                     /* top of the tree: staged in shared memory by TMA */
-				const float4 *p4 = reinterpret_cast<const float4 *>(snodes + stageBase + node);
+				const float4 *p4 = reinterpret_cast<const float4 *>(reinterpret_cast<const PairNode *>(crg_stage_smem) + stageBase + node);
 				q0 = p4[0]; q1 = p4[1]; q2 = p4[2];
 				q3 = *reinterpret_cast<const uint4 *>(p4 + 3);
 			} else {
-				const float4 *p4 = reinterpret_cast<const float4 *>(base + node);
+				const float4 *p4 = reinterpret_cast<const float4 *>(sc.pairs + pairOff + node);
 				q0 = __ldg(p4 + 0); q1 = __ldg(p4 + 1); q2 = __ldg(p4 + 2);
 				q3 = __ldg(reinterpret_cast<const uint4 *>(p4 + 3));
 			}
@@ -320,21 +377,21 @@ struct Traversal {
 			const float rb[6] = { q1.z, q1.w, q2.x, q2.y, q2.z, q2.w };
 			if (COUNT) ctr->pairs++;
 			float tL, tR;
-			const bool hitL = cr_node_test(lb, rs, o, best.t, tL);
-			const bool hitR = cr_node_test(rb, rs, o, best.t, tR);
+			const bool hitL = cr_node_test(lb, invDir, scaledStart, flags, o, bestT, tL);
+			const bool hitR = cr_node_test(rb, invDir, scaledStart, flags, o, bestT, tR);
 			const bool leafL = (q3.z & CRG_LEAF_BIT) != 0u, leafR = (q3.w & CRG_LEAF_BIT) != 0u;
 			const bool goL = hitL && !leafL, goR = hitR && !leafR;
 			uint32_t next;
 			if (goL & goR) {
 				const bool swap = tL > tR;                                         /* bvh.c:424-431 */
 				next = swap ? q3.y : q3.x;
-				stack[sp++] = swap ? q3.x : q3.y;
+				push(swap ? q3.x : q3.y, ovf);
 			} else if (goL ^ goR) {
 				next = goL ? q3.x : q3.y;
 			} else {
-				next = (sp == spBase) ? CRG_END : stack[--sp];
+				next = (sp == spBase) ? CRG_END : pop(ovf);
 			}
-			if (bottom) {
+			if (bottom()) {
 				/* left leaf, then right leaf (bvh.c:402-418), as ONE loop so that lanes with a left leaf and lanes with a
 				 * right leaf test their triangles together */
 				const uint32_t nL = (hitL && leafL) ? (q3.z & ~CRG_LEAF_BIT) : 0u;
@@ -343,7 +400,7 @@ struct Traversal {
 				if (DEFER && (nL + nR) != 0u && nL < 65536u && nR < 65536u) {
 					leafA = q3.x; leafB = q3.y; leafN = nL | (nR << 16);               /* tested by leaf_step(), then finish_bottom() */
 				} else {
-					if (nL + nR) instHit |= cr_leaf_tris2<COUNT>(tris, slotBase, q3.x, nL, q3.y, nR, o, d, best, ctr);
+					if (nL + nR) leaf_tris(sc, q3.x, nL, q3.y, nR, ctr);
 					finish_bottom(sc);
 				}
 			} else {
@@ -358,6 +415,8 @@ struct Traversal {
 	CRD void instance_step(const DevScene &sc, TraceCounters *ctr) {
 		{
 			/* ---- one instance of a pending top-level leaf (bvh.c:468-486) */
+			TravShared &s = sh();
+			const unsigned t = tid();
 			uint32_t idx;
 			if (cntA) { idx = pendA++; --cntA; } else { idx = pendB++; --cntB; }
 			const int cur = __ldg(sc.top_prims + sc.top.slot_offset + idx);
@@ -367,38 +426,37 @@ struct Traversal {
 			const float Ainv[12] = { r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w, r2.x, r2.y, r2.z, r2.w };
 			const uint4 meta = __ldg(reinterpret_cast<const uint4 *>(&inst->kind));    /* kind, bvh, ray_offset, radius */
 			v3 oo, od;
-			cr_object_ray(Ainv, __uint_as_float(meta.z), wo, wd, oo, od);
+			cr_object_ray(Ainv, __uint_as_float(meta.z), v3make(s.wo[0][t], s.wo[1][t], s.wo[2][t]), v3make(s.wd[0][t], s.wd[1][t], s.wd[2][t]), oo, od);
 			if (meta.x == CRS_INST_MESH) {                                         /* instance.c:169-175 */
 				if (COUNT) ctr->insts++;
 				const DevBvh *bvh = sc.bvhs + meta.y;
 				const uint32_t nodeCount = __ldg(&bvh->node_count);
 				const uint32_t slotOff = __ldg(&bvh->slot_offset);
 				if (nodeCount < 1u) {
-					best.inst = -1;                                                /* bvh.c:362-365 quirk */
+					s.inst[t] = -1;                                                /* bvh.c:362-365 quirk */
 				} else if (nodeCount == 1u) {                                      /* bvh.c:382-387 */
 					const RaySetup ors = cr_ray_setup(oo, od);
 					float rbnd[6], te;
 					for (int k = 0; k < 6; ++k) rbnd[k] = __ldg(&bvh->root_bounds[k]);
-					if (cr_node_test(rbnd, ors, oo, best.t, te))
-						if (cr_leaf_tris<COUNT>(sc.tris + slotOff, slotOff, __ldg(&bvh->root_first), __ldg(&bvh->root_count), oo, od, best, ctr))
-							best.inst = cur;
+					if (cr_node_test(rbnd, ors.invDir, ors.scaledStart, ors.bits, oo, bestT, te))
+						if (cr_leaf_tris<COUNT>(sc, slotOff, __ldg(&bvh->root_first), __ldg(&bvh->root_count), 0u, 0u, oo, od, bestT, s.u[t], s.v[t], s.prim[t], ctr)) {
+							s.inst[t] = cur;
+							flags &= ~CRG_TF_SPHERE;
+						}
 				} else {
-					bottom = true;
-					topNext = node;
-					o = oo; d = od;
-					rs = cr_ray_setup(o, d);
-					base = sc.pairs + __ldg(&bvh->pair_offset);
-					stageBase = __ldg(&bvh->stage_base); stageCount = snodes ? __ldg(&bvh->stage_count) : 0u;
-					tris = sc.tris + slotOff;
+					flags = (flags | CRG_TF_BOTTOM) & ~CRG_TF_INSTHIT;
+					s.topNext[t] = node;
+					set_ray(oo, od);
+					pairOff = __ldg(&bvh->pair_offset);
+					stageBase = __ldg(&bvh->stage_base); stageCount = (flags & CRG_TF_STAGED) ? __ldg(&bvh->stage_count) : 0u;
 					slotBase = slotOff;
-					curInst = cur;
-					instHit = false;
+					s.curInst[t] = cur;
 					spBase = sp;
 					node = 0u;
 				}
 			} else {                                                               /* instance.c:45-51 */
 				if (COUNT) ctr->spheres++;
-				if (cr_sphere_test(oo, od, __uint_as_float(meta.w), best.t)) best.inst = cur;
+				if (cr_sphere_test(oo, od, __uint_as_float(meta.w), bestT)) { s.inst[t] = cur; flags |= CRG_TF_SPHERE; }
 			}
 		}
 	}
@@ -461,14 +519,16 @@ CRD void cr_coop_leaves(Traversal<COUNT> &tr, bool has, const DevScene &sc, Coop
 		}
 		__syncwarp();
 		if (fits) {
-			float bt = tr.best.t;
+			float bt = tr.bestT;
 			int kb = -1;
 			for (unsigned k = 0u; k < cnt; ++k) { const float x = cs.t[excl + k]; if (x < bt) { bt = x; kb = (int)k; } }
 			if (kb >= 0) {
 				const unsigned k = (unsigned)kb;
-				tr.best.t = bt; tr.best.u = cs.u[excl + k]; tr.best.v = cs.v[excl + k];
-				tr.best.prim = tr.slotBase + (k < nA ? tr.leafA + k : tr.leafB + (k - nA));
-				tr.instHit = true;
+				TravShared &ts = tr.sh();
+				const unsigned t = tr.tid();
+				tr.bestT = bt; ts.u[t] = cs.u[excl + k]; ts.v[t] = cs.v[excl + k];
+				ts.prim[t] = tr.slotBase + (k < nA ? tr.leafA + k : tr.leafB + (k - nA));
+				tr.flags |= CRG_TF_INSTHIT;
 			}
 			tr.leafN = 0u;
 			tr.finish_bottom(sc);
@@ -481,11 +541,9 @@ CRD void cr_coop_leaves(Traversal<COUNT> &tr, bool has, const DevScene &sc, Coop
 
 template <bool COUNT>
 CRD Hit cr_closest_hit(const DevScene &sc, v3 wo, v3 wd, TraceCounters *ctr) {
-	uint32_t stack[2 * CRG_MAX_STACK + 2];
+	uint32_t ovf[CRG_OVF];
 	Traversal<COUNT> tr;
-	tr.stack = stack;
-	tr.snodes = nullptr;
-	tr.begin(sc, wo, wd);
-	while (!tr.done()) tr.step(sc, ctr);
-	return tr.best;
+	tr.begin(sc, wo, wd, false);
+	while (!tr.done()) tr.step(sc, ovf, ctr);
+	return tr.result();
 }
