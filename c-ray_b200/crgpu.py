@@ -63,6 +63,22 @@ assert RAY_RECORD_DTYPE.itemsize == 32
 # the frame path's defaults (crg_trace_knobs_env); burst is 4 when leaves are deferred
 TRACE_DEFAULTS = dict(count=0, minb=4, defer=0, refill=16, burst=3, inst_min=4)
 
+# struct crgpu_path_state / crgpu_shade_result (crgpu_shade_rays); the path state is struct cro_path_state of the oracle
+PATH_STATE_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("weight", "<f4", 3), ("has_l", "<u4"), ("rng", "<u8"),
+                             ("L", "<f4", 3), ("pad", "<u4")])
+assert PATH_STATE_DTYPE.itemsize == 64
+SHADE_RESULT_DTYPE = np.dtype([("rec", RAY_RECORD_DTYPE), ("alive", "<i4"), ("slot", "<u4"), ("dir_key", "<u4"), ("pad", "<u4"),
+                               ("next", PATH_STATE_DTYPE)])
+assert SHADE_RESULT_DTYPE.itemsize == 112
+# the frame path's K3 defaults (crg_shade_knobs_env)
+SHADE_DEFAULTS = dict(minb=2, split=1, prefetch=0, dirmode=0, complete_interpreter=0, tail=0)
+LIBM = ["sin", "cos", "tan", "log", "log10", "atan2", "acos", "asin", "pow", "pow5", "sincos_sin", "sincos_cos"]
+
+
+class ShadeOpts(C.Structure):
+    """struct crgpu_shade_opts"""
+    _fields_ = [(n, C.c_int32) for n in ("minb", "split", "prefetch", "dirmode", "complete_interpreter", "tail", "depth", "max_depth")]
+
 _lib = None
 
 
@@ -92,6 +108,8 @@ def lib():
         L.crgpu_framebuffer_device_ptr.argtypes = [P, C.POINTER(P), C.POINTER(C.c_size_t)]
         L.crgpu_trace_kat.argtypes = [P, P, C.c_int, P]
         L.crgpu_trace_rays.argtypes = [P, P, C.c_uint32, C.POINTER(TraceOpts), P, P, C.POINTER(C.c_uint32), C.POINTER(Stats)]
+        L.crgpu_shade_rays.argtypes = [P, P, C.c_uint32, C.POINTER(ShadeOpts), P, P, C.POINTER(C.c_uint32), P]
+        L.crgpu_libm_eval.argtypes = [C.c_int, C.c_int, P, P, P, C.c_uint32]
         L.crgpu_scene_create_prepared.argtypes = [P, C.c_int, C.POINTER(P)]
         L.crgpu_scene_info.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.crgpu_device_trim.argtypes = [C.c_int]
@@ -101,6 +119,7 @@ def lib():
         for f in ("crgpu_device_count", "crgpu_scene_create", "crgpu_scene_destroy", "crgpu_set_max_paths_in_flight",
                   "crgpu_render_tile", "crgpu_render_tiles", "crgpu_set_stream", "crgpu_use_own_stream", "crgpu_get_stats", "crgpu_framebuffer_clear", "crgpu_framebuffer_read", "crgpu_framebuffer_write",
                   "crgpu_framebuffer_to_srgb8", "crgpu_framebuffer_device_ptr", "crgpu_trace_kat", "crgpu_trace_rays", "crscene_load",
+                  "crgpu_shade_rays", "crgpu_libm_eval",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
                   "crscene_set_config"):
             getattr(L, f).restype = C.c_int
@@ -260,6 +279,23 @@ class GpuScene:
                                       C.byref(misses), C.byref(st)), "crgpu_trace_rays")
         return rec, perm, misses.value, st.as_dict()
 
+    def shade_rays(self, states, depth, max_depth, **opts):
+        """One bounce of path states (PATH_STATE_DTYPE) through the frame's K2 -> K4 -> K3 (-> K4b), or the tail kernel (tail=1).
+        opts: minb, split, prefetch, dirmode, complete_interpreter, tail (SHADE_DEFAULTS).
+        Returns (results (SHADE_RESULT_DTYPE, one per state), perm2 of the survivors, survivors, origin-box slot (12 x u32))."""
+        states = np.ascontiguousarray(states, dtype=PATH_STATE_DTYPE)
+        n = len(states)
+        k = dict(SHADE_DEFAULTS)
+        k.update(opts)
+        o = ShadeOpts(depth=int(depth), max_depth=int(max_depth), **{f: int(k[f]) for f in SHADE_DEFAULTS})
+        res = np.zeros(n, dtype=SHADE_RESULT_DTYPE)
+        perm2 = np.zeros(n, dtype=np.uint32)
+        box = np.zeros(12, dtype=np.uint32)
+        surv = C.c_uint32(0)
+        _check(lib().crgpu_shade_rays(self.handle, states.ctypes.data, n, C.byref(o), res.ctypes.data, perm2.ctypes.data,
+                                      C.byref(surv), box.ctypes.data), "crgpu_shade_rays")
+        return res, perm2[:surv.value], surv.value, box
+
     def set_max_paths(self, n):
         _check(lib().crgpu_set_max_paths_in_flight(self.handle, int(n)), "crgpu_set_max_paths_in_flight")
 
@@ -273,6 +309,15 @@ class GpuScene:
             self.close()
         except Exception:
             pass
+
+
+def libm_eval(fn, x, y=None, device=0):
+    """The device's fp64 libm stand-in `fn` (a name of LIBM) over float32 arrays x (and y: atan2's x, pow's exponent)."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    y = np.zeros_like(x) if y is None else np.ascontiguousarray(y, dtype=np.float32)
+    out = np.zeros_like(x)
+    _check(lib().crgpu_libm_eval(device, LIBM.index(fn), x.ctypes.data, y.ctypes.data, out.ctypes.data, len(x)), "crgpu_libm_eval")
+    return out
 
 
 class RankGather:

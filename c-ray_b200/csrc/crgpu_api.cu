@@ -974,6 +974,7 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	const int grid = s->sm_count * 8;
 	const int dirmode = crg_dir_mode();
 	const TraceKnobs &knobs = crg_trace_knobs_env();
+	const ShadeKnobs &sknobs = crg_shade_knobs_env();
 	uint64_t launches = 0;
 	float trace_ms = 0.f, shade_ms = 0.f;
 	if (timing) CU(cudaEventRecord(s->ev[0], s->stream));
@@ -1003,13 +1004,13 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
 			crg_launch_bucket(wb, cur, grid, st);
 			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
-			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, grid, st);
+			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, grid, sknobs, st);
 			if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
 				crg_launch_dirsort(wb, cur ^ 1, dirmode == 4 ? (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1) : -1, grid, st);
 				++launches;
 			}
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
-			launches += 2 + (uint64_t)crg_shade_launches_per_bounce();
+			launches += 2 + (uint64_t)crg_shade_launches_per_bounce(sknobs);
 			cur ^= 1;
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
@@ -1276,5 +1277,139 @@ extern "C" int crgpu_trace_kat(crgpu_scene *s, const int32_t *xyp, int count, vo
 	if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
 	cudaFree(dx); cudaFree(dk);
 	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "trace_kat: %s", cudaGetErrorString(e));
+	return CRGPU_OK;
+}
+
+/* One bounce of a batch of path states through the kernels of a frame's bounce, launched by the frame's own launch functions: K2 ->
+ * K4 -> K3 (and K4b when a sort mode is set and another bounce follows), or the tail kernel.  The states go into the current half
+ * of the wave buffers with id = their index (| CRG_ID_HAS_L where has_l is set) and L as given; the other half is poisoned.  Each
+ * result is found by the id K3 compacted it with. */
+#define CRG_ID_HAS_L_HOST 0x80000000u
+extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *states, uint32_t n, const struct crgpu_shade_opts *opts,
+								struct crgpu_shade_result *results, uint32_t *perm2_out, uint32_t *survivors_out, uint32_t *box_out) {
+	if (!s || !opts || (n && (!states || !results || !perm2_out)) || !survivors_out || n > (1u << 30)) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad argument");
+	ShadeKnobs kn;
+	kn.minb = opts->minb; kn.split = opts->split; kn.prefetch = opts->prefetch;
+	if (kn.minb < 2 || kn.minb > 4 || kn.split < 0 || kn.split > 1 || kn.prefetch < 0 || kn.prefetch > 1 || opts->dirmode < 0 || opts->dirmode > 4 ||
+		opts->depth < 0 || opts->max_depth < 1 || opts->depth >= opts->max_depth)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "shade options out of range");
+	CU(cudaSetDevice(s->device));
+	int rc = crgpu_get_stats(s, nullptr);
+	if (rc) return rc;
+	rc = alloc_wave(s, n ? n : 1, 1);
+	if (rc) return rc;
+	const WaveBuffers &wb = s->wb;
+	cudaStream_t st = s->stream;
+	const int grid = s->sm_count * 8;
+	const bool xnodes = s->xnodes || opts->complete_interpreter;
+	std::vector<float4> a(n), b(n), L(n);
+	std::vector<uint4> c(n);
+	for (uint32_t i = 0; i < n; ++i) {
+		const crgpu_path_state &p = states[i];
+		a[i] = make_float4(p.o[0], p.o[1], p.o[2], p.d[0]);
+		b[i] = make_float4(p.d[1], p.d[2], p.weight[0], p.weight[1]);
+		uint32_t wb32;
+		memcpy(&wb32, &p.weight[2], 4);
+		c[i] = make_uint4(wb32, i | (p.has_l ? CRG_ID_HAS_L_HOST : 0u), (uint32_t)(p.rng & 0xffffffffull), (uint32_t)(p.rng >> 32));
+		L[i] = make_float4(p.L[0], p.L[1], p.L[2], 0.0f);
+	}
+	const unsigned counts[5] = { n, 0u, 0u, 0u, 0u };
+	const size_t n4 = (size_t)n * sizeof(float4);
+	if (n) {
+		CU(cudaMemcpyAsync(wb.stA[0], a.data(), n4, cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(wb.stB[0], b.data(), n4, cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(wb.stC[0], c.data(), n4, cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(wb.L, L.data(), n4, cudaMemcpyHostToDevice, st));
+		CU(cudaMemsetAsync(wb.stA[1], 0xA5, n4, st));
+		CU(cudaMemsetAsync(wb.stB[1], 0xA5, n4, st));
+		CU(cudaMemsetAsync(wb.stC[1], 0xA5, n4, st));
+		CU(cudaMemsetAsync(wb.hit, 0xA5, n4, st));
+		CU(cudaMemsetAsync(wb.hitInst, 0xA5, (size_t)n * sizeof(int), st));
+		CU(cudaMemsetAsync(wb.dirKey, 0xA5, (size_t)n, st));
+		CU(cudaMemsetAsync(wb.perm2, 0xFF, (size_t)n * sizeof(unsigned), st));
+	}
+	CU(cudaMemcpyAsync(wb.counts, counts, sizeof counts, cudaMemcpyHostToDevice, st));
+	CU(cudaMemsetAsync(wb.hist, 0, 1024 * sizeof(unsigned), st));
+	const int depth = opts->depth, maxDepth = opts->max_depth;
+	const int box_slot = depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1;
+	unsigned box[12];
+	CU(cudaMemcpyAsync(box, wb.box + 12 * box_slot, sizeof box, cudaMemcpyDeviceToHost, st));
+	if (opts->tail) {
+		crg_launch_tail(s->dev_copy, wb, 0, depth, maxDepth, xnodes, st);
+	} else {
+		crg_launch_trace(s->dev, wb, 0, false, false, crg_trace_knobs_env(), st);
+		crg_launch_bucket(wb, 0, grid, st);
+		const bool sort_next = opts->dirmode != 0 && depth + 1 < maxDepth;
+		crg_launch_shade(s->dev_copy, wb, 0, depth, maxDepth, sort_next ? opts->dirmode : 0, xnodes, grid, kn, st);
+		if (sort_next) crg_launch_dirsort(wb, 1, opts->dirmode == 4 ? box_slot : -1, grid, st);
+	}
+	CU(cudaGetLastError());
+	void *drec = nullptr;
+	if (n && !opts->tail) {
+		CU(cudaMalloc(&drec, (size_t)n * sizeof(struct crgpu_ray_record)));
+		crg_launch_trace_records(s->dev, wb, n, drec, grid, st);
+	}
+	std::vector<crgpu_ray_record> rec(n);
+	std::vector<float4> a2(n), b2(n), L2(n);
+	std::vector<uint4> c2(n);
+	std::vector<uint8_t> dk(n);
+	unsigned cnt[5];
+	cudaError_t e = cudaGetLastError();
+	if (e == cudaSuccess && drec) e = cudaMemcpyAsync(rec.data(), drec, (size_t)n * sizeof(struct crgpu_ray_record), cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, wb.counts, sizeof cnt, cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+	const uint32_t surv = opts->tail ? cnt[0] : cnt[1];
+	if (e == cudaSuccess && surv > n) { if (drec) cudaFree(drec); return fail(CRGPU_ERR_CUDA, "shade_rays: %u survivors of %u paths", surv, n); }
+	const int half = opts->tail ? 0 : 1;
+	if (e == cudaSuccess && surv) {
+		e = cudaMemcpyAsync(a2.data(), half ? wb.stA[1] : wb.stA[0], (size_t)surv * sizeof(float4), cudaMemcpyDeviceToHost, st);
+		if (e == cudaSuccess) e = cudaMemcpyAsync(b2.data(), half ? wb.stB[1] : wb.stB[0], (size_t)surv * sizeof(float4), cudaMemcpyDeviceToHost, st);
+		if (e == cudaSuccess) e = cudaMemcpyAsync(c2.data(), half ? wb.stC[1] : wb.stC[0], (size_t)surv * sizeof(uint4), cudaMemcpyDeviceToHost, st);
+		if (e == cudaSuccess) e = cudaMemcpyAsync(dk.data(), wb.dirKey, surv, cudaMemcpyDeviceToHost, st);
+		if (e == cudaSuccess) e = cudaMemcpyAsync(perm2_out, wb.perm2, (size_t)surv * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+	}
+	if (e == cudaSuccess && n) e = cudaMemcpyAsync(L2.data(), wb.L, n4, cudaMemcpyDeviceToHost, st);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+	if (drec) cudaFree(drec);
+	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "shade_rays: %s", cudaGetErrorString(e));
+	for (uint32_t i = 0; i < n; ++i) {
+		crgpu_shade_result &r = results[i];
+		memset(&r, 0, sizeof r);
+		if (!opts->tail) r.rec = rec[i];
+		else { r.rec.inst = -2; r.rec.poly = -2; }
+		r.slot = 0xffffffffu;
+		r.dir_key = 0xffffffffu;
+		memcpy(r.next.L, &L2[i], 12);
+	}
+	for (uint32_t k = 0; k < surv; ++k) {
+		const uint32_t id = c2[k].y & ~CRG_ID_HAS_L_HOST;
+		if (id >= n || results[id].alive) return fail(CRGPU_ERR_CUDA, "shade_rays: survivor %u carries id %u (duplicate or out of range)", k, c2[k].y);
+		crgpu_shade_result &r = results[id];
+		r.alive = 1;
+		r.slot = k;
+		r.dir_key = dk[k];
+		r.next.o[0] = a2[k].x; r.next.o[1] = a2[k].y; r.next.o[2] = a2[k].z; r.next.d[0] = a2[k].w;
+		r.next.d[1] = b2[k].x; r.next.d[2] = b2[k].y; r.next.weight[0] = b2[k].z; r.next.weight[1] = b2[k].w;
+		memcpy(&r.next.weight[2], &c2[k].x, 4);
+		r.next.has_l = (c2[k].y & CRG_ID_HAS_L_HOST) ? 1u : 0u;
+		r.next.rng = (uint64_t)c2[k].z | ((uint64_t)c2[k].w << 32);
+	}
+	*survivors_out = surv;
+	if (box_out) memcpy(box_out, box, sizeof box);
+	return crgpu_get_stats(s, nullptr);
+}
+
+extern "C" int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *out, uint32_t n) {
+	if (fn < 0 || fn >= CRGPU_LIBM_COUNT || (n && (!x || !y || !out))) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad argument");
+	if (n == 0) return CRGPU_OK;
+	CU(cudaSetDevice(device));
+	float *d = nullptr;
+	CU(cudaMalloc((void **)&d, (size_t)n * 3 * sizeof(float)));
+	cudaError_t e = cudaMemcpy(d, x, (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
+	if (e == cudaSuccess) e = cudaMemcpy(d + n, y, (size_t)n * sizeof(float), cudaMemcpyHostToDevice);
+	if (e == cudaSuccess) { crg_launch_libm(fn, d, d + n, d + 2 * (size_t)n, n, 0); e = cudaGetLastError(); }
+	if (e == cudaSuccess) e = cudaMemcpy(out, d + 2 * (size_t)n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
+	cudaFree(d);
+	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "libm_eval: %s", cudaGetErrorString(e));
 	return CRGPU_OK;
 }

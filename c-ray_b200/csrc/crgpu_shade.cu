@@ -90,7 +90,9 @@ CRD bool cr_shade_one(const DevScene &sc, float4 *__restrict__ Lbuf, v3 o, v3 d,
 	Rec rec;
 	const int material = cr_reconstruct_hit(sc, o, d, hit, rec, false);
 	const DevMaterial mat = sc.materials[material];
-	if (mat.flags & 2u)                                                               /* pathtrace.c:44 (x + w*0 == x) */
+	/* pathtrace.c:44.  Without emission (flag 2) the add is x + w*0 == x, skipped, unless w is not finite: then the reference's
+	 * sum becomes NaN and so must L (DESIGN.md §2, deviation 4) */
+	if ((mat.flags & 2u) || !(isfinite(wr) && isfinite(wg) && isfinite(wbl)))
 		cr_add_radiance(Lbuf, id, wr * mat.emission[0], wg * mat.emission[1], wbl * mat.emission[2]);
 	if (depth + 1 < maxDepth) {                                                       /* else: the loop ends, the sample is unused */
 		const BsdfSample s = cr_sample_bsdf<X>(sc, mat.bsdf, rng, rec);              /* pathtrace.c:46-48 */
@@ -390,11 +392,23 @@ void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int de
  * miss kernel at 4 blocks per SM), CRGPU_SHADE_PREFETCH = 0|1 — read once; the defaults are what measured best.  On an H100 80GB HBM3
  * at a 400 W limit (hdr.json, 1080p, 1000 spp) the shading step takes 720 ms per frame with the hit kernel at 2 blocks per SM, 883 ms at 3 and 1068 ms at 4.
  * ptxas reports 784 B of spill stores for the hit kernel at 80 registers and 124 B at 128. */
+const ShadeKnobs &crg_shade_knobs_env(void) {
+	static const ShadeKnobs kn = [] {
+		ShadeKnobs k;
+		const char *e = getenv("CRGPU_SHADE_MINB");
+		const int v = e ? atoi(e) : 2;
+		k.minb = v >= 2 && v <= 4 ? v : 2;
+		e = getenv("CRGPU_SHADE_SPLIT");
+		k.split = e ? atoi(e) : 1;
+		e = getenv("CRGPU_SHADE_PREFETCH");
+		k.prefetch = e ? atoi(e) : 0;
+		return k;
+	}();
+	return kn;
+}
 template <bool X>
-static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, cudaStream_t st) {
-	static const int minb = [] { const char *e = getenv("CRGPU_SHADE_MINB"); const int v = e ? atoi(e) : 2; return v >= 2 && v <= 4 ? v : 2; }();
-	static const int split = [] { const char *e = getenv("CRGPU_SHADE_SPLIT"); return e ? atoi(e) : 1; }();
-	static const int prefetch = [] { const char *e = getenv("CRGPU_SHADE_PREFETCH"); return e ? atoi(e) : 0; }();
+static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, const ShadeKnobs &kn, cudaStream_t st) {
+	const int minb = kn.minb, split = kn.split, prefetch = kn.prefetch;
 	if (split) {
 		k_shade<4, 1, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		if (minb == 3) k_shade<3, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
@@ -406,9 +420,10 @@ static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, in
 	else if (minb == 4) k_shade<4, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	else k_shade<2, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 }
-void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid, cudaStream_t st) {
-	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, st);
-	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, st);
+void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid,
+                      const ShadeKnobs &kn, cudaStream_t st) {
+	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, st);
+	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, st);
 }
 void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st) {
 	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot);
@@ -417,7 +432,33 @@ int crg_dir_mode(void) {
 	static const int mode = [] { const char *e = getenv("CRGPU_TRACE_SORT"); const int v = e ? atoi(e) : 0; return v >= 0 && v <= 4 ? v : 0; }();
 	return mode;
 }
-int crg_shade_launches_per_bounce(void) { const char *e = getenv("CRGPU_SHADE_SPLIT"); return (e ? atoi(e) : 1) ? 2 : 1; }
+int crg_shade_launches_per_bounce(const ShadeKnobs &kn) { return kn.split ? 2 : 1; }
+
+/* ---- the libm stand-ins one by one (test entry crgpu_libm_eval; the order of include/crgpu.h CRGPU_LIBM_*) -------------------- */
+__global__ void k_libm(int fn, const float *__restrict__ x, const float *__restrict__ y, float *__restrict__ out, unsigned n) {
+	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const float a = x[i], b = y[i];
+		float r, s, c;
+		switch (fn) {
+		case 0: r = cr_sinf(a); break;
+		case 1: r = cr_cosf(a); break;
+		case 2: r = cr_tanf(a); break;
+		case 3: r = cr_logf(a); break;
+		case 4: r = cr_log10f(a); break;
+		case 5: r = cr_atan2f(a, b); break;
+		case 6: r = cr_acosf(a); break;
+		case 7: r = cr_asinf(a); break;
+		case 8: r = cr_powf(a, b); break;
+		case 9: r = cr_pow5f(a); break;
+		case 10: cr_sincosf(a, &s, &c); r = s; break;
+		default: cr_sincosf(a, &s, &c); r = c; break;
+		}
+		out[i] = r;
+	}
+}
+void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st) {
+	k_libm<<<256, 256, 0, st>>>(fn, x, y, out, n);
+}
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st) {
 	k_accumulate<<<grid, 256, 0, st>>>(fb, L, td, W, H);
 }

@@ -55,7 +55,8 @@ CRD col4 cr_texel(const DevScene &sc, const DevTexture &t, uint64_t x64, uint64_
 		o.a = t.has_alpha ? __ldg(f + idx + 3) : 1.0f;
 	} else if (t.channels == 4) {
 		const uchar4 px = __ldg(reinterpret_cast<const uchar4 *>(t.data + idx));
-		o.r = __ldg(lut + px.x); o.g = __ldg(lut + px.y); o.b = __ldg(lut + px.z); o.a = __ldg(lut + px.w);
+		o.r = __ldg(lut + px.x); o.g = __ldg(lut + px.y); o.b = __ldg(lut + px.z);
+		o.a = t.has_alpha ? __ldg(lut + px.w) : 1.0f;                 /* like every other branch: alpha only where the texture has one */
 	} else {
 		o.r = __ldg(lut + __ldg(t.data + idx));
 		o.g = __ldg(lut + __ldg(t.data + idx + 1));

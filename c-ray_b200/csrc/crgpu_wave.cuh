@@ -89,8 +89,18 @@ void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, 
 int crg_dir_mode(void);
 void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st);
 void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, bool xnodes, cudaStream_t st);
-void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid, cudaStream_t st);
-int crg_shade_launches_per_bounce(void);
+/* Launch variant of K3.  Every variant computes the same path states.
+ *   minb      blocks per SM of the hit kernel (or of the one kernel when not split): 2, 3 or 4
+ *   split     1 = a separate miss kernel (PART 1) ahead of the hit kernel (PART 2); 0 = one kernel for every ray (PART 0)
+ *   prefetch  1 = read perm two iterations ahead and prefetch the records it points to into L2
+ * The frame path reads them once from CRGPU_SHADE_MINB / _SPLIT / _PREFETCH (crg_shade_knobs_env); crgpu_shade_rays passes its own. */
+struct ShadeKnobs { int minb, split, prefetch; };
+const ShadeKnobs &crg_shade_knobs_env(void);
+void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid,
+                      const ShadeKnobs &kn, cudaStream_t st);
+int crg_shade_launches_per_bounce(const ShadeKnobs &kn);
+/* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */
+void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st);
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st);
 void crg_launch_kat(const DevScene *dsc, const int32_t *xyp, int count, void *out, cudaStream_t st);

@@ -160,6 +160,48 @@ struct crgpu_ray_record {
 int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, const struct crgpu_trace_opts *opts,
                      struct crgpu_ray_record *records_out, uint32_t *perm_out, uint32_t *misses_out, struct crgpu_stats *stats_out);
 
+/* Test entry point of the shading step that renders frames: one bounce of `n` path states through the kernels and launch functions
+ * of a frame's bounce — K2 (trace, the frame's trace knobs), K4 (bucket sort), K3 (shade + compaction, in the variant `opts` names)
+ * and K4b (direction sort, when `dirmode` is set and depth + 1 < max_depth) — or through the tail kernel, which runs every path to
+ * its end (and does nothing when more than 16,384 paths are given).  State i is loaded as path id i with its L; the other half of
+ * the wave buffers is poisoned.  Returns per state: K2's record (tail: inst = poly = -2), whether the path continues and its next
+ * state (found by the id it was compacted with), L (the L buffer after the step; for a live path meaningful only with has_l),
+ * its slot and K3's direction key; `perm2_out` receives K4b's order of the survivors, `*survivors_out` the live count the step left
+ * (tail: the live count of the current half) and `box_out` (12 values, may be NULL) dir mode 4's origin-box slot of this depth
+ * as it was before the step. */
+struct crgpu_path_state {          /* 64 bytes, the layout of struct cro_path_state (oracle/cray_oracle.h) */
+	float o[3], d[3];
+	float weight[3];
+	uint32_t has_l;                /* CRG_ID_HAS_L: L holds radiance */
+	uint64_t rng;                  /* PCG state */
+	float L[3];
+	uint32_t pad;
+};
+struct crgpu_shade_opts {
+	int32_t minb;                  /* K3 hit kernel blocks per SM: 2, 3 or 4 */
+	int32_t split;                 /* 1: separate miss kernel */
+	int32_t prefetch;              /* 1: perm read ahead + L2 prefetch */
+	int32_t dirmode;               /* 0..4: the direction sort of the next bounce (CRGPU_TRACE_SORT) */
+	int32_t complete_interpreter;  /* 1: the complete node interpreter even when the scene does not need it */
+	int32_t tail;                  /* 1: the tail kernel instead of K2 -> K4 -> K3 */
+	int32_t depth, max_depth;      /* the bounce and the scene's bounce limit */
+};
+struct crgpu_shade_result {
+	struct crgpu_ray_record rec;
+	int32_t alive;
+	uint32_t slot;                 /* compacted index of a live path, else 0xffffffff */
+	uint32_t dir_key;              /* K3's direction key of a live path (dirmode != 0), else 0xffffffff */
+	uint32_t pad;
+	struct crgpu_path_state next;
+};
+int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *states, uint32_t n, const struct crgpu_shade_opts *opts,
+                     struct crgpu_shade_result *results, uint32_t *perm2_out, uint32_t *survivors_out, uint32_t *box_out);
+
+/* The fp64 libm stand-ins of the shading kernels (crgpu_math.cuh) one by one on device `device`: out[i] = f(x[i]) or f(x[i], y[i]). */
+enum { CRGPU_LIBM_SIN, CRGPU_LIBM_COS, CRGPU_LIBM_TAN, CRGPU_LIBM_LOG, CRGPU_LIBM_LOG10, CRGPU_LIBM_ATAN2, CRGPU_LIBM_ACOS,
+       CRGPU_LIBM_ASIN, CRGPU_LIBM_POW, CRGPU_LIBM_POW5, CRGPU_LIBM_SINCOS_SIN, CRGPU_LIBM_SINCOS_COS, CRGPU_LIBM_COUNT };
+int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *out, uint32_t n);
+
 /* SURVEY §8(f1): the reference's binned-SAH BVH build (reference src/accelerators/bvh.c:96-296: partitionPrimitives,
  * buildBvhRecursive, buildBvhGeneric) on device `device`, level-synchronous (c-ray_b200/csrc/crgpu_bvh_build.cu).  Produces the
  * SAME tree as the reference and as the host builder (crloader_build_bvh): node order, leaf ranges, primitive order, bounds.

@@ -22,6 +22,62 @@ typedef struct { float r, g, b, a; } col;
 #define MIN_(a, b) (((a) < (b)) ? (a) : (b))
 #define MAX_(a, b) (((a) > (b)) ? (a) : (b))
 
+/* ---- libm semantics ----------------------------------------------------------------------------------
+ * Every libm call of the hot loop goes through lm_*().  Semantics 0 is the reference: glibc's fp32 routine.  Semantics 1 is the
+ * device (crgpu_math.cuh): the fp64 function rounded once to fp32, powf as exp(y*log x) on its fast branch, and powf(x, 5) of
+ * schlick() as fp64 products.  The device's fp64 routines are not glibc's (CUDA documents up to 2 ulp, glibc up to 1), so an fp64
+ * result that lies within a few fp64 ulps of an fp32 rounding boundary may round the other way on the device: such an evaluation
+ * sets the thread's near-tie flag (lm_tie), which the callers report per path.  The mode and the flag are per thread: every
+ * worker sets lm_sem from its job and clears lm_tie per path. */
+static _Thread_local int lm_sem;
+static _Thread_local int lm_tie;
+#define LM_TIE_ULPS 4.0   /* CUDA's error bound + glibc's, with a margin */
+
+/* flags r when an fp32 rounding boundary (the midpoint between two adjacent floats; for subnormal results the absolute grid) lies
+ * within LM_TIE_ULPS * scale fp64 ulps of it */
+static void lm_check(double r, double scale) {
+	if (!isfinite(r)) return;
+	const double a = fabs(r);
+	const float f = (float)r;
+	double lo, hi;                                       /* the boundaries either side of f */
+	const double top = (double)FLT_MAX + ldexp(1.0, 103);   /* FLT_MAX and +inf round apart here */
+	if (isinf(f)) { lo = hi = signbit(f) ? -top : top; }
+	else {
+		const float fd = nextafterf(f, -INFINITY), fu = nextafterf(f, INFINITY);
+		lo = isinf(fd) ? -top : ((double)f + (double)fd) * 0.5;
+		hi = isinf(fu) ? top : ((double)f + (double)fu) * 0.5;
+	}
+	const double ulp = nextafter(a, INFINITY) - a;
+	const double tol = LM_TIE_ULPS * scale * ulp;
+	if (fabs(r - lo) <= tol || fabs(r - hi) <= tol) lm_tie = 1;
+}
+static inline float lm_round(double r, double scale) { lm_check(r, scale); return (float)r; }
+
+static float lm_sinf(float x) { return lm_sem ? lm_round(sin((double)x), 1.0) : sinf(x); }
+static float lm_cosf(float x) { return lm_sem ? lm_round(cos((double)x), 1.0) : cosf(x); }
+static float lm_tanf(float x) { return lm_sem ? lm_round(tan((double)x), 1.0) : tanf(x); }
+static float lm_logf(float x) { return lm_sem ? lm_round(log((double)x), 1.0) : logf(x); }
+static float lm_log10f(float x) { return lm_sem ? lm_round(log10((double)x), 1.0) : log10f(x); }
+static float lm_atan2f(float y, float x) { return lm_sem ? lm_round(atan2((double)y, (double)x), 1.0) : atan2f(y, x); }
+static float lm_acosf(float x) { return lm_sem ? lm_round(acos((double)x), 1.0) : acosf(x); }
+static float lm_asinf(float x) { return lm_sem ? lm_round(asin((double)x), 1.0) : asinf(x); }
+/* cr_powf: exp(y*log x) on 0 < x < FLT_MAX, finite y, |y| < 1e6, where an error of the fp64 log is magnified |y ln x| times;
+ * the full pow() special-case logic everywhere else */
+static float lm_powf(float x, float y) {
+	if (!lm_sem) return powf(x, y);
+	if (x > 0.0f && x < FLT_MAX && y == y && fabsf(y) < 1.0e6f) {
+		const double e = (double)y * log((double)x);
+		return lm_round(exp(e), 1.0 + fabs(e));
+	}
+	return lm_round(pow((double)x, (double)y), 1.0);
+}
+/* powf(x, 5.0f) of schlick(); cr_pow5f is four exact-order fp64 products, which this restates operation for operation */
+static float lm_pow5f(float x) {
+	if (!lm_sem) return powf(x, 5.0f);
+	const double a = (double)x, a2 = a * a;
+	return (float)(a2 * a2 * a);
+}
+
 /* ---- vector.h ------------------------------------------------------------------------------------ */
 static inline v3 v3add(v3 a, v3 b) { return (v3){ a.x + b.x, a.y + b.y, a.z + b.z }; }          /* :65 */
 static inline v3 v3sub(v3 a, v3 b) { return (v3){ a.x - b.x, a.y - b.y, a.z - b.z }; }          /* :76 */
@@ -46,14 +102,14 @@ static inline col ccoef(float k, col c) { return (col){ c.r * k, c.g * k, c.b * 
 static inline col cmix(col a, col b, float t) { return cadd(ccoef(1.0f - t, a), ccoef(t, b)); }        /* :54 */
 static inline float srgb_to_linear(float c) {                                                           /* :68 */
 	if (c <= 0.04045f) return c / 12.92f;
-	return powf(((c + 0.055f) / 1.055f), 2.4f);
+	return lm_powf(((c + 0.055f) / 1.055f), 2.4f);
 }
 static inline float linear_to_srgb(float c) {                                                           /* :60 */
 	if (c <= 0.0031308f) return 12.92f * c;
-	return (1.055f * powf(c, 0.4166666667f)) - 0.055f;
+	return (1.055f * lm_powf(c, 0.4166666667f)) - 0.055f;
 }
 static inline col to_grayscale(col c) {                                                                 /* :43 — note the double constants */
-	float b = sqrtf(0.299f * powf(c.r, 2) + 0.587 * powf(c.g, 2) + 0.114 * powf(c.b, 2));
+	float b = sqrtf(0.299f * lm_powf(c.r, 2) + 0.587 * lm_powf(c.g, 2) + 0.114 * lm_powf(c.b, 2));
 	return (col){ b, b, b, c.a };
 }
 static col color_for_kelvin(float kelvin) {                                                             /* color.c:28-70 */
@@ -64,18 +120,18 @@ static col color_for_kelvin(float kelvin) {                                     
 		ret.r = 255.0f;
 	} else {
 		ret.r = temp - 60.0f;
-		ret.r = 329.698727446f * powf(ret.r, -0.1332047592f);
+		ret.r = 329.698727446f * lm_powf(ret.r, -0.1332047592f);
 		ret.r = ret.r < 0.0f ? 0.0f : ret.r;
 		ret.r = ret.r > 255.0f ? 255.0f : ret.r;
 	}
 	if (temp <= 66.0f) {
 		ret.g = temp;
-		ret.g = 99.4708025861f * logf(ret.g) - 161.1195681661f;
+		ret.g = 99.4708025861f * lm_logf(ret.g) - 161.1195681661f;
 		ret.g = ret.g < 0.0f ? 0.0f : ret.g;
 		ret.g = ret.g > 255.0f ? 255.0f : ret.g;
 	} else {
 		ret.g = temp - 60.0f;
-		ret.g = 288.1221695283f * powf(ret.g, -0.0755148492f);
+		ret.g = 288.1221695283f * lm_powf(ret.g, -0.0755148492f);
 		ret.g = ret.g < 0.0f ? 0.0f : ret.g;
 		ret.g = ret.g > 255.0f ? 255.0f : ret.g;
 	}
@@ -86,7 +142,7 @@ static col color_for_kelvin(float kelvin) {                                     
 			ret.b = 0.0f;
 		} else {
 			ret.b = temp - 10.0f;
-			ret.b = 138.5177312231f * logf(ret.b) - 305.0447927307f;
+			ret.b = 138.5177312231f * lm_logf(ret.b) - 305.0447927307f;
 			ret.b = ret.b < 0.0f ? 0.0f : ret.b;
 			ret.b = ret.b > 255.0f ? 255.0f : ret.b;
 		}
@@ -128,7 +184,7 @@ static inline v3 random_on_unit_sphere(struct rng *r) {                         
 	const float sy = draw(r);
 	const float a = sx * (2.0f * PI);
 	const float s = 2.0f * sqrtf(MAX_(0.0f, sy * (1.0f - sy)));
-	return (v3){ cosf(a) * s, sinf(a) * s, 1.0f - 2.0f * sy };
+	return (v3){ lm_cosf(a) * s, lm_sinf(a) * s, 1.0f - 2.0f * sy };
 }
 
 /* ---- transforms.c:76-116 ----------------------------------------------------------------------------- */
@@ -187,7 +243,7 @@ static struct ray camera_ray(const struct crs_camera *cam, int x, int y, struct 
 		v3 focus = v3add(ray.o, v3scale(ray.d, ft));
 		float rr = sqrtf(draw(r));                           /* randomCoordOnUnitDisc, vector.h:194-198 */
 		float theta = ((draw(r)) * (2.0f * PI - 0.0f)) + 0.0f; /* rndFloatRange(0, 2π) */
-		v2 lens = { (rr * cosf(theta)) * cam->aperture, (rr * sinf(theta)) * cam->aperture };
+		v2 lens = { (rr * lm_cosf(theta)) * cam->aperture, (rr * lm_sinf(theta)) * cam->aperture };
 		ray.o = v3add(ray.o, v3add(v3scale(right, lens.x), v3scale(up, lens.y)));
 		ray.d = v3norm(v3sub(focus, ray.o));
 	}
@@ -333,8 +389,8 @@ static bool traverse(const struct trav_ctx *c, uint32_t bvhIdx, int meshIdx /* -
 					 const struct ray *ray, struct hit *isect);
 
 static v2 texmap_sphere(v3 ud) {                                                              /* instance.c:33-43 */
-	float phi = atan2f(ud.z, ud.x);
-	float theta = asinf(ud.y);
+	float phi = lm_atan2f(ud.z, ud.x);
+	float theta = lm_asinf(ud.y);
 	float v = (theta + PI / 2.0f) / PI;
 	float u = 1.0f - (phi + PI) / (PI * 2.0f);
 	u = wrapMinMax(u, 0.0f, 1.0f);
@@ -569,8 +625,8 @@ static col eval_color(const struct crs_scene *s, int node, const struct hit *rec
 	case CRS_COLOR_CHECKER: {                                                         /* checker.c:31-54 */
 		const float coef = eval_value(s, n->in[2], rec);
 		float sines;
-		if (rec->uv.x >= 0) sines = sinf(coef * rec->uv.x) * sinf(coef * rec->uv.y);
-		else sines = sinf(coef * rec->p.x) * sinf(coef * rec->p.y) * sinf(coef * rec->p.z);
+		if (rec->uv.x >= 0) sines = lm_sinf(coef * rec->uv.x) * lm_sinf(coef * rec->uv.y);
+		else sines = lm_sinf(coef * rec->p.x) * lm_sinf(coef * rec->p.y) * lm_sinf(coef * rec->p.z);
 		return sines < 0.0f ? eval_color(s, n->in[0], rec) : eval_color(s, n->in[1], rec);
 	}
 	case CRS_COLOR_GRADIENT: {                                                        /* gradient.c:40-45 */
@@ -614,15 +670,15 @@ static float eval_value(const struct crs_scene *s, int node, const struct hit *r
 		case CRS_MATH_SUBTRACT: return a - b;
 		case CRS_MATH_MULTIPLY: return a * b;
 		case CRS_MATH_DIVIDE: return a / b;
-		case CRS_MATH_POWER: return powf(a, b);
-		case CRS_MATH_LOG: return log10f(a);
+		case CRS_MATH_POWER: return lm_powf(a, b);
+		case CRS_MATH_LOG: return lm_log10f(a);
 		case CRS_MATH_SQRT: return sqrtf(a);
 		case CRS_MATH_ABS: return fabsf(a);
 		case CRS_MATH_MIN: return MIN_(a, b);
 		case CRS_MATH_MAX: return MAX_(a, b);
-		case CRS_MATH_SINE: return sinf(a);
-		case CRS_MATH_COSINE: return cosf(a);
-		case CRS_MATH_TANGENT: return tanf(a);
+		case CRS_MATH_SINE: return lm_sinf(a);
+		case CRS_MATH_COSINE: return lm_cosf(a);
+		case CRS_MATH_TANGENT: return lm_tanf(a);
 		case CRS_MATH_TO_RADIANS: return (a * PI) / 180.0f;                             /* transforms.c:18-20 */
 		case CRS_MATH_TO_DEGREES: return a * (180.0f / PI);                             /* transforms.c:22-24 */
 		default: return 0.0f;
@@ -660,7 +716,7 @@ static bool refract_(v3 in, v3 normal, float niOverNt, v3 *refracted) {         
 static inline float schlick(float cosine, float IOR) {                                  /* vector.h:268-272 */
 	float r0 = (1.0f - IOR) / (1.0f + IOR);
 	r0 = r0 * r0;
-	return r0 + (1.0f - r0) * powf((1.0f - cosine), 5.0f);
+	return r0 + (1.0f - r0) * lm_pow5f((1.0f - cosine));
 }
 
 static struct bsdf_sample sample_bsdf(const struct crs_scene *s, int node, struct rng *r, struct hit *rec) {
@@ -754,8 +810,8 @@ static struct bsdf_sample sample_bsdf(const struct crs_scene *s, int node, struc
 	case CRS_BSDF_BACKGROUND: {                                                       /* background.c:39-66 */
 		v3 ud = v3norm(rec->incident.d);
 		float rr = 1.0f;
-		float phi = (atan2f(ud.z, ud.x) / 4.0f) + eval_value(s, n->in[2], rec);
-		float theta = acosf((-ud.y / rr));
+		float phi = (lm_atan2f(ud.z, ud.x) / 4.0f) + eval_value(s, n->in[2], rec);
+		float theta = lm_acosf((-ud.y / rr));
 		float u = theta / PI;
 		float v = (phi / (PI / 2.0f));
 		u = wrapMinMax(u, 0.0f, 1.0f);
@@ -784,42 +840,68 @@ static struct hit closest_isect(const struct trav_ctx *c, const struct ray *ray)
 	return isect;
 }
 
-static col path_trace(const struct trav_ctx *c, struct ray ray, int maxDepth, struct rng *r) {
+/* One pass through pathTrace's loop body (pathtrace.c:37-57) at `depth`: returns false where the loop breaks.  `final` is only
+ * read once `*has_final` is set (it is treated as (0, 0, 0, 1), pathtrace.c:34, before), which is how a path state that has not
+ * received any radiance yet is handed between calls (cro_path_step); path_trace starts with it set.  `hit_out` (may be NULL)
+ * receives the closest-hit record of the step's ray. */
+static bool path_step(const struct trav_ctx *c, struct ray *ray, col *weight, col *final, int *has_final, int depth,
+					  struct rng *r, struct cro_ray_record *hit_out) {
 	const struct crs_scene *s = c->s;
+	size_t hdr = 0;
+	const size_t HDR = 36;
+	int have_hdr = 0;
+	if (c->tr && c->tr->len + HDR <= c->tr->cap) {           /* record header: x, y, pass, depth (u16), event count (u32), o, d (6 x f32) */
+		hdr = c->tr->len;
+		have_hdr = 1;
+		const uint16_t h[4] = { c->tr->x, c->tr->y, c->tr->pass, (uint16_t)depth };
+		const float od[6] = { ray->o.x, ray->o.y, ray->o.z, ray->d.x, ray->d.y, ray->d.z };
+		memcpy(c->tr->buf + hdr, h, 8);
+		memcpy(c->tr->buf + hdr + 12, od, 24);
+		c->tr->len += HDR;
+	}
+	struct hit isect = closest_isect(c, ray);
+	if (have_hdr) { const uint32_t n = (uint32_t)(c->tr->len - hdr - HDR); memcpy(c->tr->buf + hdr + 8, &n, 4); }
+	if (c->ctr && (uint64_t)(depth + 1) > c->ctr->max_depth) c->ctr->max_depth = (uint64_t)(depth + 1);
+	if (hit_out) {
+		hit_out->t = isect.dist; hit_out->u = isect.bary.x; hit_out->v = isect.bary.y;
+		hit_out->inst = isect.inst; hit_out->poly = -1; hit_out->material = -1;
+		if (isect.inst >= 0) {
+			hit_out->poly = s->instances[isect.inst].kind == CRS_INST_MESH ? isect.poly : -1;
+			hit_out->material = isect.material;
+		}
+	}
+	if (!*has_final) *final = (col){ 0, 0, 0, 1 };
+	if (isect.inst < 0) {
+		*final = cadd(*final, cmul(*weight, sample_bsdf(s, s->background, r, &isect).color));
+		*has_final = 1;
+		return false;
+	}
+	const struct crs_material *m = &s->materials[isect.material];
+	/* The device adds emission only where it can change `final` (cr_shade_one: DevMaterial flag 2, or a weight that is not finite):
+	 * x + w*0 == x for finite w and every x but -0, which a sum that starts at +0 never is.  `*has_final` follows that rule in
+	 * both semantics, so a state without radiance always holds +0 (DESIGN.md §2, deviation 4); semantics 1 also skips the add. */
+	const col e = { m->emission[0], m->emission[1], m->emission[2], m->emission[3] };
+	const bool adds = !(e.r == 0.0f && e.g == 0.0f && e.b == 0.0f) || !(isfinite(weight->r) && isfinite(weight->g) && isfinite(weight->b));
+	if (adds) *has_final = 1;
+	if (adds || !c->dev) *final = cadd(*final, cmul(*weight, e));
+	const struct bsdf_sample smp = sample_bsdf(s, m->bsdf, r, &isect);
+	*ray = (struct ray){ isect.p, smp.out };
+	const col att = smp.color;
+	float probability = 1.0f;
+	if (depth >= 4) {
+		probability = MAX_(att.r, MAX_(att.g, att.b));
+		if (draw(r) > probability) return false;
+	}
+	*weight = ccoef(1.0f / probability, cmul(att, *weight));
+	return true;
+}
+
+static col path_trace(const struct trav_ctx *c, struct ray ray, int maxDepth, struct rng *r) {
 	col weight = { 1, 1, 1, 1 };
 	col final = { 0, 0, 0, 1 };
-	for (int depth = 0; depth < maxDepth; ++depth) {
-		size_t hdr = 0;
-		const size_t HDR = 36;
-		int have_hdr = 0;
-		if (c->tr && c->tr->len + HDR <= c->tr->cap) {           /* record header: x, y, pass, depth (u16), event count (u32), o, d (6 x f32) */
-			hdr = c->tr->len;
-			have_hdr = 1;
-			const uint16_t h[4] = { c->tr->x, c->tr->y, c->tr->pass, (uint16_t)depth };
-			const float od[6] = { ray.o.x, ray.o.y, ray.o.z, ray.d.x, ray.d.y, ray.d.z };
-			memcpy(c->tr->buf + hdr, h, 8);
-			memcpy(c->tr->buf + hdr + 12, od, 24);
-			c->tr->len += HDR;
-		}
-		struct hit isect = closest_isect(c, &ray);
-		if (have_hdr) { const uint32_t n = (uint32_t)(c->tr->len - hdr - HDR); memcpy(c->tr->buf + hdr + 8, &n, 4); }
-		if (c->ctr && (uint64_t)(depth + 1) > c->ctr->max_depth) c->ctr->max_depth = (uint64_t)(depth + 1);
-		if (isect.inst < 0) {
-			final = cadd(final, cmul(weight, sample_bsdf(s, s->background, r, &isect).color));
-			break;
-		}
-		const struct crs_material *m = &s->materials[isect.material];
-		final = cadd(final, cmul(weight, (col){ m->emission[0], m->emission[1], m->emission[2], m->emission[3] }));
-		const struct bsdf_sample smp = sample_bsdf(s, m->bsdf, r, &isect);
-		ray = (struct ray){ isect.p, smp.out };
-		const col att = smp.color;
-		float probability = 1.0f;
-		if (depth >= 4) {
-			probability = MAX_(att.r, MAX_(att.g, att.b));
-			if (draw(r) > probability) break;
-		}
-		weight = ccoef(1.0f / probability, cmul(att, weight));
-	}
+	int has_final = 1;
+	for (int depth = 0; depth < maxDepth; ++depth)
+		if (!path_step(c, &ray, &weight, &final, &has_final, depth, r, NULL)) break;
 	return final;
 }
 
@@ -830,12 +912,15 @@ struct job {
 	float *rgb;
 	struct cro_counters ctr;
 	bool count;
+	int sem;                 /* libm and slab-test semantics (cro_render_sem) */
+	uint32_t *flagged;       /* per framebuffer pixel: samples with a near-tie libm evaluation, or NULL */
 };
 
 static void *render_rows(void *arg) {
 	struct job *j = arg;
 	const struct crs_scene *s = j->s;
-	struct trav_ctx c = { s, j->count ? &j->ctr : NULL, NULL, 0 };
+	struct trav_ctx c = { s, j->count ? &j->ctr : NULL, NULL, j->sem };
+	lm_sem = j->sem;
 	const int W = (int)s->prefs.image_width, H = (int)s->prefs.image_height;
 	const int maxPasses = (int)s->prefs.sample_count, bounces = (int)s->prefs.bounces;
 	for (int y = j->yend - 1; y > j->ybegin - 1; --y) {
@@ -846,9 +931,11 @@ static void *render_rows(void *arg) {
 				struct rng r = { 0, c.ctr };
 				rng_init(&r, pixIdx, pass, maxPasses);
 				col out = { px[0], px[1], px[2], 1.0f };
+				lm_tie = 0;
 				struct ray ray = camera_ray(&s->camera, x, y, &r);
 				if (c.ctr) c.ctr->paths++;
 				col smp = path_trace(&c, ray, bounces, &r);
+				if (lm_tie && j->flagged) j->flagged[(size_t)x + (size_t)(H - (y + 1)) * (size_t)W]++;
 				const int completed = pass + 1;
 				out = ccoef((float)(completed - 1), out);
 				out = cadd(out, smp);
@@ -891,6 +978,12 @@ size_t cro_trace_region(const struct crs_scene *s, int x0, int y0, int x1, int y
 
 int cro_render(const struct crs_scene *s, int x0, int y0, int x1, int y1, int pass_begin, int pass_count,
 			   float *rgb, int threads, struct cro_counters *counters) {
+	return cro_render_sem(s, x0, y0, x1, y1, pass_begin, pass_count, rgb, threads, 0, NULL, counters);
+}
+
+int cro_render_sem(const struct crs_scene *s, int x0, int y0, int x1, int y1, int pass_begin, int pass_count,
+				   float *rgb, int threads, int semantics, uint32_t *flagged, struct cro_counters *counters) {
+	if (semantics != 0 && semantics != 1) return -1;
 	if (threads < 1) threads = 1;
 	int rows = y1 - y0;
 	if (rows < 1 || x1 <= x0) return 0;
@@ -902,7 +995,7 @@ int cro_render(const struct crs_scene *s, int x0, int y0, int x1, int y1, int pa
 	for (int i = 0; i < chunks; ++i) {
 		jobs[i] = (struct job){ .s = s, .x0 = x0, .x1 = x1, .ybegin = y0 + (int)((int64_t)rows * i / chunks),
 			.yend = y0 + (int)((int64_t)rows * (i + 1) / chunks), .pass_begin = pass_begin, .pass_count = pass_count,
-			.rgb = rgb, .count = counters != NULL };
+			.rgb = rgb, .count = counters != NULL, .sem = semantics, .flagged = flagged };
 	}
 	/* simple static round-robin over threads: each thread runs chunks t, t+threads, ... */
 	pthread_t *tids = calloc((size_t)threads, sizeof *tids);
@@ -971,6 +1064,7 @@ struct ray_job { const struct crs_scene *s; const float *rays; struct cro_ray_re
 static void *closest_hit_rows(void *arg) {
 	struct ray_job *j = arg;
 	struct trav_ctx c = { j->s, j->count ? &j->ctr : NULL, NULL, j->dev };
+	lm_sem = j->dev;
 	for (size_t i = j->lo; i < j->hi; ++i) {
 		const float *r = j->rays + 6 * i;
 		const struct ray ray = { { r[0], r[1], r[2] }, { r[3], r[4], r[5] } };
@@ -1022,4 +1116,120 @@ void cro_to_srgb8(const float *rgb, uint8_t *out, size_t pixels) {
 		float c = linear_to_srgb(rgb[i]);
 		out[i] = (unsigned char)MIN_(c * 255.0f, 255.0f);
 	}
+}
+
+/* ---- path states: pathTrace's loop body one step at a time (the device's per-bounce kernels) ------------------------------------ */
+static inline struct rng rng_of(uint64_t state) { struct rng r = { state, NULL }; return r; }
+
+void cro_camera_states(const struct crs_scene *s, int x0, int y0, int x1, int y1, int pass_begin, int pass_count, int semantics,
+					   struct cro_path_state *out) {
+	const int W = (int)s->prefs.image_width;
+	const int maxPasses = (int)s->prefs.sample_count;
+	size_t k = 0;
+	lm_sem = semantics;
+	for (int y = y0; y < y1; ++y)
+		for (int x = x0; x < x1; ++x)
+			for (int pass = pass_begin; pass < pass_begin + pass_count; ++pass, ++k) {
+				struct rng r = { 0, NULL };
+				rng_init(&r, (uint32_t)(y * W + x), pass, maxPasses);
+				lm_tie = 0;
+				const struct ray ray = camera_ray(&s->camera, x, y, &r);
+				struct cro_path_state *p = &out[k];
+				memset(p, 0, sizeof *p);
+				p->pad = (uint32_t)lm_tie;
+				p->o[0] = ray.o.x; p->o[1] = ray.o.y; p->o[2] = ray.o.z;
+				p->d[0] = ray.d.x; p->d[1] = ray.d.y; p->d[2] = ray.d.z;
+				p->weight[0] = p->weight[1] = p->weight[2] = 1.0f;
+				p->rng = r.state;
+			}
+	lm_sem = 0;
+}
+
+struct step_job {
+	const struct crs_scene *s;
+	const struct cro_path_state *in;
+	struct cro_step_result *out;
+	size_t lo, hi;
+	int depth, maxDepth, bounces, sem;
+};
+
+static void *step_rows(void *arg) {
+	struct step_job *j = arg;
+	struct trav_ctx c = { j->s, NULL, NULL, j->sem };
+	lm_sem = j->sem;
+	for (size_t i = j->lo; i < j->hi; ++i) {
+		const struct cro_path_state *p = &j->in[i];
+		struct cro_step_result *o = &j->out[i];
+		memset(o, 0, sizeof *o);
+		struct ray ray = { { p->o[0], p->o[1], p->o[2] }, { p->d[0], p->d[1], p->d[2] } };
+		col weight = { p->weight[0], p->weight[1], p->weight[2], 1.0f };
+		col final = { p->L[0], p->L[1], p->L[2], 1.0f };
+		int has = p->has_l ? 1 : 0;
+		struct rng r = rng_of(p->rng);
+		lm_tie = 0;
+		bool alive = true;
+		o->rec.inst = -1; o->rec.poly = -1; o->rec.material = -1;
+		for (int depth = j->depth, k = 0; k < j->bounces; ++depth, ++k) {
+			if (depth >= j->maxDepth) { alive = false; break; }
+			alive = path_step(&c, &ray, &weight, &final, &has, depth, &r, k == 0 ? &o->rec : NULL)
+					&& depth + 1 < j->maxDepth;
+			if (!alive) break;
+		}
+		if (!alive && !has) final = (col){ 0, 0, 0, 1 };
+		o->alive = alive;
+		o->flag = (uint32_t)lm_tie;
+		o->next.o[0] = ray.o.x; o->next.o[1] = ray.o.y; o->next.o[2] = ray.o.z;
+		o->next.d[0] = ray.d.x; o->next.d[1] = ray.d.y; o->next.d[2] = ray.d.z;
+		o->next.weight[0] = weight.r; o->next.weight[1] = weight.g; o->next.weight[2] = weight.b;
+		o->next.has_l = (uint32_t)has;
+		o->next.rng = r.state;
+		o->next.L[0] = has ? final.r : p->L[0]; o->next.L[1] = has ? final.g : p->L[1]; o->next.L[2] = has ? final.b : p->L[2];
+		if (!alive) { o->next.L[0] = final.r; o->next.L[1] = final.g; o->next.L[2] = final.b; }
+	}
+	return NULL;
+}
+
+int cro_path_step(const struct crs_scene *s, size_t n, const struct cro_path_state *states, int depth, int maxDepth, int bounces,
+				  int semantics, int threads, struct cro_step_result *out) {
+	if ((semantics != 0 && semantics != 1) || depth < 0 || bounces < 1) return -1;
+	if (n == 0) return 0;
+	if (threads < 1) threads = 1;
+	if ((size_t)threads > n) threads = (int)n;
+	struct step_job *jobs = calloc((size_t)threads, sizeof *jobs);
+	pthread_t *tids = calloc((size_t)threads, sizeof *tids);
+	if (!jobs || !tids) { free(jobs); free(tids); return -1; }
+	for (int t = 0; t < threads; ++t) {
+		jobs[t] = (struct step_job){ .s = s, .in = states, .out = out, .lo = n * (size_t)t / (size_t)threads,
+			.hi = n * (size_t)(t + 1) / (size_t)threads, .depth = depth, .maxDepth = maxDepth, .bounces = bounces, .sem = semantics };
+		pthread_create(&tids[t], NULL, step_rows, &jobs[t]);
+	}
+	for (int t = 0; t < threads; ++t) pthread_join(tids[t], NULL);
+	free(tids); free(jobs);
+	return 0;
+}
+
+/* ---- the libm stand-ins one by one (test sweeps) ------------------------------------------------------------------------------- */
+int cro_libm(int fn, int semantics, size_t n, const float *x, const float *y, float *out, uint8_t *flag) {
+	if ((semantics != 0 && semantics != 1) || fn < 0 || fn >= CRO_LIBM_COUNT) return -1;
+	lm_sem = semantics;
+	for (size_t i = 0; i < n; ++i) {
+		lm_tie = 0;
+		float r;
+		switch (fn) {
+		case CRO_LIBM_SIN: r = lm_sinf(x[i]); break;
+		case CRO_LIBM_COS: r = lm_cosf(x[i]); break;
+		case CRO_LIBM_TAN: r = lm_tanf(x[i]); break;
+		case CRO_LIBM_LOG: r = lm_logf(x[i]); break;
+		case CRO_LIBM_LOG10: r = lm_log10f(x[i]); break;
+		case CRO_LIBM_ATAN2: r = lm_atan2f(x[i], y[i]); break;
+		case CRO_LIBM_ACOS: r = lm_acosf(x[i]); break;
+		case CRO_LIBM_ASIN: r = lm_asinf(x[i]); break;
+		case CRO_LIBM_POW: r = lm_powf(x[i], y[i]); break;
+		default: r = lm_pow5f(x[i]); break;
+		}
+		out[i] = r;
+		if (flag) flag[i] = (uint8_t)lm_tie;
+	}
+	lm_sem = 0;
+	return 0;
 }

@@ -92,6 +92,13 @@ assert HIT_KAT_DTYPE.itemsize == 160
 RAY_RECORD_DTYPE = np.dtype([("t", "<f4"), ("u", "<f4"), ("v", "<f4"), ("inst", "<i4"), ("poly", "<i4"), ("material", "<i4")])
 assert RAY_RECORD_DTYPE.itemsize == 24
 SEM_REFERENCE, SEM_DEVICE = 0, 1
+# struct cro_path_state / cro_step_result (cro_path_step)
+PATH_STATE_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("weight", "<f4", 3), ("has_l", "<u4"), ("rng", "<u8"),
+                             ("L", "<f4", 3), ("pad", "<u4")])
+assert PATH_STATE_DTYPE.itemsize == 64
+STEP_RESULT_DTYPE = np.dtype([("rec", RAY_RECORD_DTYPE), ("alive", "<i4"), ("flag", "<u4"), ("next", PATH_STATE_DTYPE)])
+assert STEP_RESULT_DTYPE.itemsize == 96
+LIBM = ["sin", "cos", "tan", "log", "log10", "atan2", "acos", "asin", "pow", "pow5"]
 
 _lib = None
 
@@ -116,6 +123,13 @@ def lib():
         L.cro_closest_hit.restype = C.c_int
         L.cro_trace_region.argtypes = [C.POINTER(Scene)] + [C.c_int] * 6 + [C.c_void_p, C.c_size_t]
         L.cro_trace_region.restype = C.c_size_t
+        L.cro_render_sem.argtypes = [C.POINTER(Scene)] + [C.c_int] * 6 + [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(Counters)]
+        L.cro_render_sem.restype = C.c_int
+        L.cro_camera_states.argtypes = [C.POINTER(Scene)] + [C.c_int] * 7 + [C.c_void_p]
+        L.cro_path_step.argtypes = [C.POINTER(Scene), C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+        L.cro_path_step.restype = C.c_int
+        L.cro_libm.argtypes = [C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.cro_libm.restype = C.c_int
         _lib = L
     return _lib
 
@@ -169,8 +183,49 @@ class OracleScene:
             pos += 36 + ev
         return np.array(rays, dtype=np.float32).reshape(-1, 6)
 
+    def render_sem(self, semantics, threads=None, tile=None, passes=None):
+        """Full frame (or a tile / pass range) in the given semantics: (fp32 (H,W,3) frame, per-pixel count of flagged samples)."""
+        rgb = np.zeros((self.H, self.W, 3), dtype=np.float32)
+        flagged = np.zeros((self.H, self.W), dtype=np.uint32)
+        x0, y0, x1, y1 = tile if tile else (0, 0, self.W, self.H)
+        pb, pc = passes if passes else (0, self.s.prefs.sample_count)
+        rc = lib().cro_render_sem(C.byref(self.s), x0, y0, x1, y1, pb, pc, rgb.ctypes.data, threads or os.cpu_count() or 1,
+                                  semantics, flagged.ctypes.data, None)
+        if rc != 0:
+            raise RuntimeError(f"cro_render_sem failed ({rc})")
+        return rgb, flagged
+
+    def camera_states(self, x0, y0, x1, y1, passes=None, semantics=SEM_DEVICE):
+        """Path states of the camera rays of a region: pixels row-major (y up), passes innermost (pad = near-tie flag)."""
+        pb, pc = passes if passes else (0, self.s.prefs.sample_count)
+        out = np.zeros((y1 - y0) * (x1 - x0) * pc, dtype=PATH_STATE_DTYPE)
+        lib().cro_camera_states(C.byref(self.s), x0, y0, x1, y1, pb, pc, semantics, out.ctypes.data)
+        return out
+
+    def path_step(self, states, depth, max_depth=None, bounces=1, semantics=SEM_DEVICE, threads=None):
+        """`bounces` passes of pathTrace's loop body from bounce `depth` (STEP_RESULT_DTYPE per state)."""
+        states = np.ascontiguousarray(states, dtype=PATH_STATE_DTYPE)
+        out = np.zeros(len(states), dtype=STEP_RESULT_DTYPE)
+        md = self.s.prefs.bounces if max_depth is None else max_depth
+        rc = lib().cro_path_step(C.byref(self.s), len(states), states.ctypes.data, depth, md, bounces, semantics,
+                                 threads or os.cpu_count() or 1, out.ctypes.data)
+        if rc != 0:
+            raise RuntimeError(f"cro_path_step failed ({rc})")
+        return out
+
     def close(self):
         lib().crscene_free(C.byref(self.s))
+
+
+def libm(fn, semantics, x, y=None):
+    """An oracle libm call over float32 arrays: (results, near-tie flags)."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    y = np.zeros_like(x) if y is None else np.ascontiguousarray(y, dtype=np.float32)
+    out = np.zeros_like(x)
+    flag = np.zeros(len(x), dtype=np.uint8)
+    rc = lib().cro_libm(LIBM.index(fn), semantics, len(x), x.ctypes.data, y.ctypes.data, out.ctypes.data, flag.ctypes.data)
+    assert rc == 0
+    return out, flag.astype(bool)
 
 
 def sampler_kat(pix, p, maxp, n):

@@ -220,3 +220,156 @@ def test_zero_bounces_is_black():
     img = sc.render(threads=2)
     assert not img.any()
     sc.close()
+
+
+# ------------------------------------------------------------------------------------------------ path steps and libm semantics
+def chain_frame(o, semantics):
+    """The frame of cro_render, rebuilt from cro_path_step one bounce at a time from the camera states, and the running average
+    of renderer.c:288-291 in numpy fp32.  Returns (frame, per-pixel count of flagged samples)."""
+    W, H, spp, B = o.W, o.H, o.s.prefs.sample_count, o.s.prefs.bounces
+    cur = o.camera_states(0, 0, W, H, semantics=semantics)
+    n = len(cur)
+    L = np.zeros((n, 3), np.float32)
+    flag = cur["pad"] != 0
+    idx = np.arange(n)
+    for depth in range(B):
+        if len(cur) == 0:
+            break
+        r = o.path_step(cur, depth, semantics=semantics)
+        flag[idx] |= r["flag"] != 0
+        dead = r["alive"] == 0
+        L[idx[dead]] = r["next"]["L"][dead]
+        idx, cur = idx[~dead], r["next"][~dead]
+    assert len(cur) == 0 or B == 0
+    Ls = L.reshape(H, W, spp, 3)
+    out = np.zeros((H, W, 3), np.float32)
+    for p in range(spp):
+        out = (out * np.float32(p)) + Ls[:, :, p]
+        out = out * (np.float32(1) / np.float32(p + 1))
+    return out[::-1], flag.reshape(H, W, spp).sum(axis=2)[::-1]
+
+
+def _synthetic_flat(tmp_path):
+    from test_gpu_trace import _write_synthetic, _flatten
+    d = str(tmp_path)
+    return {n: _flatten(p, os.path.join(d, n + ".crscene")) for n, p in _write_synthetic(os.path.join(d, "syn")).items()}
+
+
+def test_path_step_chain_is_the_render(tmp_path):
+    """cro_path_step is pathTrace's loop body: chained one bounce at a time from the camera states, it reproduces cro_render's
+    framebuffer bit for bit (semantics 0) on every golden and synthetic scene, and cro_render_sem's (semantics 1)."""
+    scenes = {n: os.path.join(GOLDEN, n + ".crscene") for n in GOLDEN_FLAT}
+    scenes.update(_synthetic_flat(tmp_path))
+    for name, path in scenes.items():
+        o = O.OracleScene(path)
+        ref = o.render(threads=os.cpu_count())
+        img, _ = chain_frame(o, O.SEM_REFERENCE)
+        assert np.array_equal(img.view(np.uint32), ref.view(np.uint32)), name
+        ref1, fl1 = o.render_sem(O.SEM_DEVICE)
+        img1, fl = chain_frame(o, O.SEM_DEVICE)
+        assert np.array_equal(img1.view(np.uint32), ref1.view(np.uint32)), name
+        assert np.array_equal(fl, fl1), name
+        r0, f0 = o.render_sem(O.SEM_REFERENCE)
+        assert np.array_equal(r0.view(np.uint32), ref.view(np.uint32)) and not f0.any(), name
+        o.close()
+
+
+def test_non_finite_weight_reaches_radiance():
+    """A weight that is not finite makes the reference's finalColor NaN at every hit, emissive or not (pathtrace.c:44): both
+    semantics must say so, with the radiance flag set, although semantics 1 skips the add of zero emission for finite weights."""
+    o = O.OracleScene(os.path.join(GOLDEN, "g_single.crscene"))
+    st = o.camera_states(0, 0, o.W, o.H, passes=(0, 1))
+    r = o.path_step(st, 0, semantics=O.SEM_REFERENCE)
+    hit = r["rec"]["inst"] >= 0
+    assert hit.any()
+    st = st[hit]
+    for w in (np.inf, -np.inf, np.nan):
+        st["weight"] = w
+        for sem in (O.SEM_REFERENCE, O.SEM_DEVICE):
+            r = o.path_step(st, 1, semantics=sem)
+            assert (r["next"]["has_l"] == 1).all() and np.isnan(r["next"]["L"]).any(axis=1).all(), (w, sem)
+    o.close()
+
+
+_F32 = np.finfo(np.float32)
+
+
+def _sweeps():
+    """(function, x, y) sweeps over the inputs where fp32 libm results go wrong"""
+    rng = np.random.default_rng(5)
+    f = np.float32
+    specials = np.array([0.0, -0.0, np.inf, -np.inf, np.nan, 1e-45, -1e-45, _F32.tiny, -_F32.tiny, _F32.max, -_F32.max, 1.0, -1.0], f)
+
+    def around(c, k=64):                      # floats within k ulps of c
+        c = f(c)
+        up, dn = [c], [c]
+        for _ in range(k):
+            up.append(np.nextafter(up[-1], f(np.inf)))
+            dn.append(np.nextafter(dn[-1], f(-np.inf)))
+        return np.array(up + dn, f)
+
+    out = []
+    trig = [specials, rng.uniform(-10, 10, 20000).astype(f), (rng.uniform(-1, 1, 5000) * f(1e30)).astype(f),
+            (10.0 ** rng.uniform(3, 38, 5000)).astype(f) * np.where(rng.integers(0, 2, 5000) == 1, f(1), f(-1))]
+    trig += [around(k * np.pi / 2) for k in range(-8, 9)]
+    trig = np.concatenate(trig)
+    out += [("sin", trig, None), ("cos", trig, None)]
+    out.append(("tan", np.concatenate([specials, rng.uniform(-10, 10, 20000).astype(f)] + [around(k * np.pi / 2, 256) for k in (-3, -1, 1, 3)]), None))
+    vals = np.concatenate([specials, (np.array([0, 1, 2, 4, 8, -0.5], f)[:, None] * np.ones(1, f)).ravel(), rng.normal(size=4000).astype(f),
+                           (10.0 ** rng.uniform(-40, 38, 4000)).astype(f) * np.where(rng.integers(0, 2, 4000) == 1, f(1), f(-1))])
+    X, Y = np.meshgrid(vals[:60], vals[:60])
+    out.append(("atan2", np.concatenate([X.ravel(), vals]), np.concatenate([Y.ravel(), vals[::-1]])))
+    unit = np.concatenate([specials, around(1.0, 256), around(-1.0, 256), around(0.0, 64), rng.uniform(-1, 1, 20000).astype(f),
+                           np.array([1.0000001, -1.0000001, 2.0, -2.0], f)])
+    out += [("acos", unit, None), ("asin", unit, None)]
+    logs = np.concatenate([specials, np.array([2 ** -149, 2 ** -140, 2 ** -127, 2 ** -126, 1e-40], f), around(1.0, 256),
+                           (10.0 ** rng.uniform(-45, 38.5, 20000)).astype(f), -np.abs(rng.normal(size=100)).astype(f)])
+    out += [("log", logs, None), ("log10", logs, None)]
+    px = np.concatenate([specials, around(1.0, 32), np.array([-2.0, -0.5, -1.0, -3.0, 0.5, 2.0, 10.0], f),
+                         (10.0 ** rng.uniform(-45, 38, 3000)).astype(f), rng.uniform(0, 1, 3000).astype(f)])
+    py = np.concatenate([specials, np.array([2.0, 3.0, -2.0, 0.5, 2.4, 0.4166666667, -0.1332047592, -0.0755148492, 5.0, 1e6, -1e6,
+                                             999999.94, -999999.94, 1000000.06, 3e7, -3e7], f), around(1e6, 8), rng.normal(size=200).astype(f) * 40])
+    X, Y = np.meshgrid(px, py)
+    out.append(("pow", X.ravel(), Y.ravel()))
+    near1 = around(1.0, 2048)
+    big = np.concatenate([rng.uniform(-1e6, 1e6, 2048), np.array([1e5, -1e5, 4e5, -7e5])]).astype(f)
+    out.append(("pow", np.resize(near1, len(near1) * 8), np.resize(big, len(near1) * 8)))
+    return out
+
+
+def _exact(fn, x, y):
+    """the correctly rounded fp32 result, from numpy.longdouble (x87 80-bit) evaluation"""
+    X = x.astype(np.longdouble)
+    with np.errstate(all="ignore"):
+        if fn == "atan2":
+            r = np.arctan2(X, y.astype(np.longdouble))
+        elif fn == "pow":
+            r = np.power(X, y.astype(np.longdouble))
+        else:
+            r = {"sin": np.sin, "cos": np.cos, "tan": np.tan, "log": np.log, "log10": np.log10, "acos": np.arccos, "asin": np.arcsin}[fn](X)
+        return r.astype(np.float32)
+
+
+def same_bits(a, b):
+    """bit-identical fp32, except that any NaN equals any NaN"""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    return (a.view(np.uint32) == b.view(np.uint32)) | (np.isnan(a) & np.isnan(b))
+
+
+def test_device_libm_semantics_are_correctly_rounded_unless_flagged():
+    """Semantics 1's stand-ins (the device's fp64-then-round evaluation) give the correctly rounded fp32 result of the same
+    function, from an 80-bit evaluation, everywhere they do not raise the near-tie flag; and they raise it rarely."""
+    assert np.finfo(np.longdouble).nmant >= 63, "needs x87 long double"
+    total = flagged = 0
+    for fn, x, y in _sweeps():
+        got, flag = O.libm(fn, O.SEM_DEVICE, x, y)
+        ok = same_bits(got, _exact(fn, x, y))
+        bad = np.nonzero(~ok & ~flag)[0]
+        assert len(bad) == 0, (fn, x[bad[:5]], None if y is None else y[bad[:5]], got[bad[:5]], _exact(fn, x, y)[bad[:5]])
+        total += len(x)
+        flagged += int(flag.sum())
+    print(f"libm sweeps: {flagged} of {total} evaluations flagged")
+    assert flagged <= total * 1e-3
+    # exact results far from any boundary are not flagged
+    v, fl = O.libm("pow", O.SEM_DEVICE, np.array([1.5, 4.0], np.float32), np.array([1.0, 0.5], np.float32))
+    assert not fl.any() and v[0] == 1.5 and v[1] == 2.0
