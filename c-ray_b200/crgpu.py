@@ -71,13 +71,14 @@ SHADE_RESULT_DTYPE = np.dtype([("rec", RAY_RECORD_DTYPE), ("alive", "<i4"), ("sl
                                ("next", PATH_STATE_DTYPE)])
 assert SHADE_RESULT_DTYPE.itemsize == 112
 # the frame path's K3 defaults (crg_shade_knobs_env)
-SHADE_DEFAULTS = dict(minb=2, split=1, prefetch=0, dirmode=0, complete_interpreter=0, tail=0)
+SHADE_DEFAULTS = dict(minb=2, split=1, prefetch=0, dirmode=0, complete_interpreter=0, tail=0, generic_only=0)
 LIBM = ["sin", "cos", "tan", "log", "log10", "atan2", "acos", "asin", "pow", "pow5", "sincos_sin", "sincos_cos"]
 
 
 class ShadeOpts(C.Structure):
     """struct crgpu_shade_opts"""
-    _fields_ = [(n, C.c_int32) for n in ("minb", "split", "prefetch", "dirmode", "complete_interpreter", "tail", "depth", "max_depth")]
+    _fields_ = [(n, C.c_int32) for n in ("minb", "split", "prefetch", "dirmode", "complete_interpreter", "tail", "depth", "max_depth",
+                                         "generic_only")]
 
 _lib = None
 
@@ -281,7 +282,7 @@ class GpuScene:
 
     def shade_rays(self, states, depth, max_depth, **opts):
         """One bounce of path states (PATH_STATE_DTYPE) through the frame's K2 -> K4 -> K3 (-> K4b), or the tail kernel (tail=1).
-        opts: minb, split, prefetch, dirmode, complete_interpreter, tail (SHADE_DEFAULTS).
+        opts: minb, split, prefetch, dirmode, complete_interpreter, tail, generic_only (SHADE_DEFAULTS).
         Returns (results (SHADE_RESULT_DTYPE, one per state), perm2 of the survivors, survivors, origin-box slot (12 x u32))."""
         states = np.ascontiguousarray(states, dtype=PATH_STATE_DTYPE)
         n = len(states)

@@ -138,7 +138,8 @@ extern "C" void crgpu_host_free(void *p) { if (p) cudaFreeHost(p); }
  * crgpu_prepare() does everything about a scene that does not depend on the device: validation, BVH re-layout into pair nodes,
  * triangle packing, shading records.  crgpu_scene_create_prepared() is then one host->device copy of the slab plus two small
  * pointer-carrying tables.  A host that renders many frames of one scene, or one frame on many GPUs, prepares once. */
-enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_PRIMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_NODES, SEC_TEXS, SEC_LUT, SEC_TEXDATA, SEC_COUNT };
+enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_PRIMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_FLAT, SEC_ORDER, SEC_NODES, SEC_TEXS, SEC_LUT,
+       SEC_TEXDATA, SEC_COUNT };
 struct crgpu_prepared {
 	crs_prefs prefs;
 	crs_camera camera;
@@ -149,6 +150,8 @@ struct crgpu_prepared {
 	uint32_t stage_pairs;
 	uint32_t texture_count;
 	size_t key_inst_off;       /* the instance keys follow the prim-slot keys in SEC_KEYS */
+	uint32_t material_count;
+	uint32_t flat_keys;        /* DevScene::flat_keys */
 	bool xnodes;               /* some node is of a kind only the complete interpreter (NodeX) evaluates */
 	uint8_t *slab;
 	bool pinned;
@@ -316,6 +319,77 @@ static int check_bsdf(const crs_scene *f, int idx, int add_level, int guard, boo
 	}
 }
 
+/* ---- flat materials (DevFlat): the fixed-form graphs the flat K3 launch samples without the node interpreter -------------
+ * A leaf (diffuse, metal, glass, emissive, or plastic over a diffuse) whose colour is a constant or one image node and whose values
+ * are constants, alone or under the loader's legacy wrapper Mix(Transparent(constant c0), leaf, Alpha(constant or image colour))
+ * (host/loader/cr_nodes.c crl_assign_bsdf).  Folding copies the bits the interpreter would read — f[0..3] of a constant colour, f[0]
+ * of a value, f[3] of an alpha's constant, tex / options of an image — and computes nothing.  Anything else stays generic. */
+static bool flat_color(const crs_scene *f, int idx, float col[4], int32_t &tex, uint32_t &opt, bool &img) {
+	if (!node_ok(f, idx)) return false;
+	const crs_node &n = f->nodes[idx];
+	if (n.kind == CRS_COLOR_CONSTANT) { memcpy(col, n.f, 4 * sizeof(float)); img = false; return true; }
+	if (n.kind == CRS_COLOR_IMAGE) { tex = n.tex; opt = n.options; img = true; return true; }
+	return false;
+}
+static bool flat_value(const crs_scene *f, int idx, float &v) {
+	if (!node_ok(f, idx) || f->nodes[idx].kind != CRS_VALUE_CONSTANT) return false;
+	memcpy(&v, &f->nodes[idx].f[0], sizeof v);
+	return true;
+}
+static bool flat_leaf(const crs_scene *f, int idx, DevFlat &d) {
+	if (!node_ok(f, idx)) return false;
+	const crs_node &n = f->nodes[idx];
+	int color = n.in[0];
+	switch (n.kind) {
+	case CRS_BSDF_DIFFUSE: d.kind = CRG_FLAT_DIFFUSE; break;
+	case CRS_BSDF_METAL: d.kind = CRG_FLAT_METAL; if (!flat_value(f, n.in[1], d.rough)) return false; break;
+	case CRS_BSDF_GLASS:
+		d.kind = CRG_FLAT_GLASS;
+		if (!flat_value(f, n.in[1], d.rough) || !flat_value(f, n.in[2], d.ior)) return false;
+		break;
+	case CRS_BSDF_EMISSIVE: d.kind = CRG_FLAT_EMISSIVE; if (!flat_value(f, n.in[1], d.strength)) return false; break;
+	case CRS_BSDF_PLASTIC: {                          /* roughness = color(in[1]).r; in[0] is never read (plastic.c:42-87) */
+		d.kind = CRG_FLAT_PLASTIC;
+		if (!node_ok(f, n.in[1]) || f->nodes[n.in[1]].kind != CRS_COLOR_CONSTANT) return false;
+		memcpy(&d.rough, &f->nodes[n.in[1]].f[0], sizeof d.rough);
+		if (!node_ok(f, n.in[2]) || f->nodes[n.in[2]].kind != CRS_BSDF_DIFFUSE) return false;
+		color = f->nodes[n.in[2]].in[0];
+		break;
+	}
+	default: return false;
+	}
+	bool img = false;
+	if (!flat_color(f, color, d.col, d.col_tex, d.col_opt, img)) return false;
+	if (img) d.flags |= CRG_FLAT_COL_IMG;
+	return true;
+}
+static DevFlat fold_flat(const crs_scene *f, int root) {
+	DevFlat d;
+	memset(&d, 0, sizeof d);
+	int leaf = root;
+	const crs_node &r = f->nodes[root];
+	if (r.kind == CRS_BSDF_MIX) {                     /* only the wrapper's shape: MIX(TRANSPARENT(constant), leaf, ALPHA(colour)) */
+		bool ok = node_ok(f, r.in[0]) && node_ok(f, r.in[2]);
+		if (ok) {
+			const crs_node &t = f->nodes[r.in[0]], &a = f->nodes[r.in[2]];
+			ok = t.kind == CRS_BSDF_TRANSPARENT && node_ok(f, t.in[0]) && f->nodes[t.in[0]].kind == CRS_COLOR_CONSTANT && a.kind == CRS_VALUE_ALPHA;
+			float ac[4];
+			bool img = false;
+			if (ok) ok = flat_color(f, a.in[0], ac, d.alpha_tex, d.alpha_opt, img);
+			if (ok) {
+				memcpy(d.c0, f->nodes[t.in[0]].f, sizeof d.c0);
+				if (img) d.flags |= CRG_FLAT_ALPHA_IMG;
+				else memcpy(&d.alpha, &ac[3], sizeof d.alpha);
+				d.flags |= CRG_FLAT_WRAPPED;
+			}
+		}
+		if (!ok) { memset(&d, 0, sizeof d); return d; }
+		leaf = r.in[1];
+	}
+	if (!flat_leaf(f, leaf, d)) memset(&d, 0, sizeof d);
+	return d;
+}
+
 /* ---- BVH re-layout: reference nodes (bvh.c:37-42) -> BFS-ordered PairNodes ---------------------------------------- */
 /* errors raised on worker threads (fail() writes a thread-local buffer): first one wins, reported by the caller */
 struct HostError {
@@ -476,6 +550,14 @@ extern "C" int crgpu_prepared_update_config(crgpu_prepared *p, const struct crs_
 	return CRGPU_OK;
 }
 
+extern "C" int crgpu_prepared_materials(const crgpu_prepared *p, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count) {
+	if (!p || (count && (!kinds || !flags))) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	const DevFlat *fl = reinterpret_cast<const DevFlat *>(p->slab + p->off[SEC_FLAT]);
+	for (uint32_t i = 0; i < count && i < p->material_count; ++i) { kinds[i] = fl[i].kind; flags[i] = fl[i].flags; }
+	if (material_count) *material_count = p->material_count;
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_prepared_slab(const crgpu_prepared *p, const void **slab, size_t *bytes) {
 	if (!p) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (slab) *slab = p->slab;
@@ -505,6 +587,7 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 
 	/* materials + graph validation */
 	std::vector<DevMaterial> mats(f->material_count);
+	std::vector<DevFlat> flat(f->material_count);
 	{
 		bool uv = false;
 		PFAIL(check_bsdf(f, f->background, 0, 0, &uv));
@@ -521,6 +604,7 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 		const bool emits = !(m.emission[0] == 0.0f && m.emission[1] == 0.0f && m.emission[2] == 0.0f);
 		d.flags = (uv ? 1u : 0u) | (emits ? 2u : 0u);
 		mats[i] = d;
+		flat[i] = fold_flat(f, m.bsdf);
 	}
 
 	/* BVHs → pair nodes; triangles in leaf order; per-poly shading records.  The three products are independent once the
@@ -741,16 +825,27 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 			if (insts[i].kind == CRS_INST_SPHERE) keys[(size_t)total_slots + i] = key_of(insts[i].material);
 	}
 	p->key_inst_off = (size_t)total_slots;
+	/* K4's bucket order for the flat launch: the misses, the keys of flat materials (1..254, one material each), then the rest —
+	 * the generic keys and the overflow key 255, which materials 254 and up share */
+	std::vector<uint8_t> order;
+	{
+		auto is_flat = [&](uint32_t k) { return k < 255u && k - 1u < f->material_count && flat[k - 1u].kind != CRG_FLAT_NONE; };
+		order.push_back(0);
+		for (uint32_t k = 1; k < 256; ++k) if (is_flat(k)) order.push_back((uint8_t)k);
+		p->flat_keys = (uint32_t)order.size() - 1u;
+		for (uint32_t k = 1; k < 256; ++k) if (!is_flat(k)) order.push_back((uint8_t)k);
+	}
+	p->material_count = f->material_count;
 	std::vector<float> lut(256);
 	for (int i = 0; i < 256; ++i) { volatile float num = (float)i, den = 255.0f; lut[i] = num / den; }   /* IEEE divss == __fdiv_rn */
 
 	/* lay the sections out in one slab (256-byte aligned each) and copy them in on the host threads */
 	const void *src[SEC_COUNT] = { stage.data(), pairs.data(), tris.data(), slot_poly.data(), keys.data(), spolys.data(), top_prims.data(), bvhs.data(),
-								   insts.data(), mats.data(), nodes.data(), texs.data(), lut.data(), f->texdata };
+								   insts.data(), mats.data(), flat.data(), order.data(), nodes.data(), texs.data(), lut.data(), f->texdata };
 	const size_t len[SEC_COUNT] = { stage.size() * sizeof(PairNode), pairs.size() * sizeof(PairNode), tris.size() * sizeof(PackedTri),
 									slot_poly.size() * sizeof(uint32_t), keys.size(), spolys.size() * sizeof(ShadePoly), top_prims.size() * sizeof(int32_t),
 									bvhs.size() * sizeof(DevBvh), insts.size() * sizeof(DevInstance), mats.size() * sizeof(DevMaterial),
-									nodes.size() * sizeof(crs_node), texs.size() * sizeof(DevTexture), lut.size() * sizeof(float), (size_t)f->texdata_bytes };
+									flat.size() * sizeof(DevFlat), order.size(), nodes.size() * sizeof(crs_node), texs.size() * sizeof(DevTexture), lut.size() * sizeof(float), (size_t)f->texdata_bytes };
 	size_t total = 0;
 	for (int k = 0; k < SEC_COUNT; ++k) { p->off[k] = total; p->len[k] = len[k]; total += (len[k] + 255u) & ~(size_t)255u; }
 	total += 512;                                                  /* room for the DevScene descriptor behind the arrays */
@@ -843,6 +938,9 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	d.bvhs = reinterpret_cast<const DevBvh *>(base + p->off[SEC_BVHS]);
 	d.instances = reinterpret_cast<const DevInstance *>(base + p->off[SEC_INSTS]);
 	d.materials = reinterpret_cast<const DevMaterial *>(base + p->off[SEC_MATS]);
+	d.flat = reinterpret_cast<const DevFlat *>(base + p->off[SEC_FLAT]);
+	d.key_order = base + p->off[SEC_ORDER];
+	d.flat_keys = p->flat_keys;
 	d.nodes = reinterpret_cast<const crs_node *>(base + p->off[SEC_NODES]);
 	d.textures = reinterpret_cast<const DevTexture *>(base + p->off[SEC_TEXS]);
 	d.u8_to_unit = reinterpret_cast<const float *>(base + p->off[SEC_LUT]);
@@ -1002,7 +1100,8 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
 			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, knobs, st);
 			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
-			crg_launch_bucket(wb, cur, grid, st);
+			if (crg_shade_flat_order(sknobs)) crg_launch_bucket(wb, cur, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
+			else crg_launch_bucket(wb, cur, grid, nullptr, 0, st);
 			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
 			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, grid, sknobs, st);
 			if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
@@ -1243,7 +1342,7 @@ extern "C" int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, c
 	CU(cudaMemsetAsync(wb.hitKey, 0xA5, (size_t)n, st));
 	CU(cudaMemsetAsync(wb.perm, 0xFF, (size_t)n * sizeof(unsigned), st));
 	crg_launch_trace(s->dev, wb, 0, opts->count != 0, opts->order != nullptr, kn, st);
-	crg_launch_bucket(wb, 0, grid, st);
+	crg_launch_bucket(wb, 0, grid, nullptr, 0, st);      /* buckets in key order */
 	CU(cudaGetLastError());
 	void *drec = nullptr;
 	if (n) {
@@ -1290,7 +1389,9 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 	if (!s || !opts || (n && (!states || !results || !perm2_out)) || !survivors_out || n > (1u << 30)) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad argument");
 	ShadeKnobs kn;
 	kn.minb = opts->minb; kn.split = opts->split; kn.prefetch = opts->prefetch;
+	kn.generic_only = opts->generic_only; kn.flat_minb = opts->minb;      /* both hit kernels at the bound the caller names */
 	if (kn.minb < 2 || kn.minb > 4 || kn.split < 0 || kn.split > 1 || kn.prefetch < 0 || kn.prefetch > 1 || opts->dirmode < 0 || opts->dirmode > 4 ||
+		kn.generic_only < 0 || kn.generic_only > 1 ||
 		opts->depth < 0 || opts->max_depth < 1 || opts->depth >= opts->max_depth)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "shade options out of range");
 	CU(cudaSetDevice(s->device));
@@ -1338,7 +1439,8 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 		crg_launch_tail(s->dev_copy, wb, 0, depth, maxDepth, xnodes, st);
 	} else {
 		crg_launch_trace(s->dev, wb, 0, false, false, crg_trace_knobs_env(), st);
-		crg_launch_bucket(wb, 0, grid, st);
+		if (crg_shade_flat_order(kn)) crg_launch_bucket(wb, 0, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
+		else crg_launch_bucket(wb, 0, grid, nullptr, 0, st);
 		const bool sort_next = opts->dirmode != 0 && depth + 1 < maxDepth;
 		crg_launch_shade(s->dev_copy, wb, 0, depth, maxDepth, sort_next ? opts->dirmode : 0, xnodes, grid, kn, st);
 		if (sort_next) crg_launch_dirsort(wb, 1, opts->dirmode == 4 ? box_slot : -1, grid, st);

@@ -78,6 +78,28 @@ struct DevMaterial {
 	uint32_t pad[2];
 };
 
+/* A "flat" material, folded at upload (crgpu_api.cu fold_flat): a leaf bsdf whose inputs are constants or one image node,
+ * optionally under the loader's legacy wrapper MIX(TRANSPARENT(c0), leaf, ALPHA(c)).  The flat hit launch of K3 samples it with
+ * a call-free switch instead of the node interpreter; the fields are bit copies of what the interpreter would read. */
+#define CRG_FLAT_NONE     0u        /* generic: the interpreter shades it */
+#define CRG_FLAT_DIFFUSE  1u
+#define CRG_FLAT_METAL    2u
+#define CRG_FLAT_GLASS    3u
+#define CRG_FLAT_EMISSIVE 4u
+#define CRG_FLAT_PLASTIC  5u        /* over a diffuse: col is the diffuse's colour, rough the plastic's in[1].r */
+#define CRG_FLAT_WRAPPED  1u        /* flags: the legacy alpha wrapper */
+#define CRG_FLAT_ALPHA_IMG 2u       /* flags: the wrapper's alpha is an image node (else the constant alpha) */
+#define CRG_FLAT_COL_IMG  4u        /* flags: the leaf colour is an image node (else col) */
+struct __align__(16) DevFlat {
+	uint32_t kind, flags;
+	int32_t  col_tex;  uint32_t col_opt;       /* image colour: crs_node.tex / .options */
+	int32_t  alpha_tex; uint32_t alpha_opt;    /* image alpha */
+	float    col[4];                           /* constant leaf colour (f[0..3]) */
+	float    c0[4];                            /* the wrapper's transparent colour */
+	float    alpha;                            /* constant alpha (f[3] of the wrapper's alpha colour) */
+	float    rough, ior, strength;             /* value inputs (f[0]); plastic: rough = f[0] of its roughness colour */
+};
+
 struct DevTexture {
 	uint32_t width, height, channels, is_float, has_alpha;
 	uint32_t wmask, hmask;          /* width-1 / height-1 when that dimension is a power of two, else 0 (x % W == x & (W-1), also for the
@@ -109,6 +131,9 @@ struct DevScene {
 	const DevBvh     *bvhs;
 	const DevInstance*instances;
 	const DevMaterial*materials;
+	const DevFlat    *flat;         /* [material] folded flat record (kind CRG_FLAT_NONE: generic) */
+	const uint8_t    *key_order;    /* [256] K4's bucket order: the miss key, the keys of flat materials, then the generic keys */
+	uint32_t          flat_keys;    /* number of flat keys (they take ranks 1..flat_keys of key_order) */
 	const crs_node   *nodes;
 	const DevTexture *textures;
 	const PairNode   *stage_img;    /* top-of-tree pair nodes of every BVH, contiguous: K2 copies it into shared memory with one

@@ -18,8 +18,9 @@
  *              hist[512..767], cursors hist[768..1023], output perm2): K2 hands rays to its lanes in perm2 order, so the 32 rays
  *              of a warp point into the same octant and walk the BVH in the same child order — fewer divergent steps. */
 template <bool DIR>
-__global__ void __launch_bounds__(256) k_bucket(WaveBuffers wb, int cur, int box_slot) {
+__global__ void __launch_bounds__(256) k_bucket(WaveBuffers wb, int cur, int box_slot, const uint8_t *__restrict__ order, int nflat) {
 	__shared__ unsigned s_base[256], s_cnt[256], s_off[256];
+	__shared__ unsigned char s_ord[256];
 	const unsigned n = wb.counts[cur];
 	const unsigned t = threadIdx.x;
 	if (DIR && box_slot >= 0 && blockIdx.x == 0u && t < 6u) {   /* K3 is done with this depth's bounds: they key the next batch */
@@ -32,10 +33,20 @@ __global__ void __launch_bounds__(256) k_bucket(WaveBuffers wb, int cur, int box
 	const unsigned char *__restrict__ keys = DIR ? wb.dirKey : wb.hitKey;
 	unsigned *__restrict__ out = DIR ? wb.perm2 : wb.perm;
 	s_cnt[t] = sizes[t];
+	s_ord[t] = order ? order[t] : (unsigned char)t;
 	__syncthreads();
-	if (t == 0u) { unsigned acc = 0u; for (int k = 0; k < 256; ++k) { s_base[k] = acc; acc += s_cnt[k]; } }
+	if (t == 0u) {
+		unsigned acc = 0u, flat_end = 0u;
+		for (int r = 0; r < 256; ++r) {
+			if (r == nflat + 1) flat_end = acc;
+			const unsigned k = s_ord[r];
+			s_base[k] = acc;
+			acc += s_cnt[k];
+		}
+		/* perm[0 .. counts[4]) are the misses (bucket 0 is always first), perm[counts[4] .. counts[5]) the hits on flat materials */
+		if (!DIR && blockIdx.x == 0u) { wb.counts[4] = s_cnt[0]; wb.counts[5] = flat_end; }
+	}
 	__syncthreads();
-	if (!DIR && blockIdx.x == 0u && t == 0u) wb.counts[4] = s_base[1];      /* = bucket 0's size: perm[0 .. counts[4]) are the misses (K3 split) */
 	const unsigned chunk = 256u * CRG_BUCKET_ITEMS;
 	for (unsigned c0 = blockIdx.x * chunk; c0 < n; c0 += gridDim.x * chunk) {
 		s_cnt[t] = 0u;
@@ -79,7 +90,7 @@ CRD void cr_finish_path(float4 *__restrict__ Lbuf, unsigned id) {
 }
 
 /* returns true when the path continues with (p_next, d_next) and the updated weight / rng / id */
-template <bool X, bool MAYBE_MISS = true>
+template <bool X, bool MAYBE_MISS = true, bool FLAT = false>
 CRD bool cr_shade_one(const DevScene &sc, float4 *__restrict__ Lbuf, v3 o, v3 d, const Hit &hit, float &wr, float &wg, float &wbl,
 					  unsigned &id, uint64_t &rng, int depth, int maxDepth, v3 &p_next, v3 &d_next) {
 	if (MAYBE_MISS && hit.inst < 0) {                                                               /* pathtrace.c:39-42 */
@@ -95,7 +106,9 @@ CRD bool cr_shade_one(const DevScene &sc, float4 *__restrict__ Lbuf, v3 o, v3 d,
 	if ((mat.flags & 2u) || !(isfinite(wr) && isfinite(wg) && isfinite(wbl)))
 		cr_add_radiance(Lbuf, id, wr * mat.emission[0], wg * mat.emission[1], wbl * mat.emission[2]);
 	if (depth + 1 < maxDepth) {                                                       /* else: the loop ends, the sample is unused */
-		const BsdfSample s = cr_sample_bsdf<X>(sc, mat.bsdf, rng, rec);              /* pathtrace.c:46-48 */
+		BsdfSample s;                                                                 /* pathtrace.c:46-48 */
+		if constexpr (FLAT) s = cr_sample_flat(sc, sc.flat[material], rng, rec);
+		else s = cr_sample_bsdf<X>(sc, mat.bsdf, rng, rec);
 		float probability = 1.0f;
 		bool cont = true;
 		if (depth >= 4) {                                                             /* pathtrace.c:50-55 */
@@ -160,13 +173,14 @@ CRD unsigned cr_dir_bin(const DevScene &sc, const OriginBox &box, v3 o, v3 d, in
 }
 
 /* ---- K3 (+ compaction) ----------------------------------------------------------------------------------------------
- * PART 0: every ray of the queue.  PART 1 / 2: the two halves of a split launch — 1 = the misses (bucket 0 = perm[0 .. counts[4]):
- * background lookup + radiance, the path always ends, nothing to compact), 2 = the hits (perm[counts[4] .. n)).  The miss half
- * needs a third of the registers of the hit half, so it runs at twice the occupancy; on hdr.json 40% of all rays are misses. */
+ * PART 0: every ray of the queue.  PART 1 / 3 / 2: the parts of a split launch — 1 = the misses (bucket 0 = perm[0 .. counts[4]):
+ * background lookup + radiance, the path always ends, nothing to compact), 3 = the hits on flat materials (perm[counts[4] ..
+ * counts[5]): cr_sample_flat, no node interpreter), 2 = the other hits (perm[counts[5] .. n)).  The miss half needs a third of the
+ * registers of the hit half, so it runs at twice the occupancy; on hdr.json 40% of all rays are misses and every hit is flat. */
 template <int MINB, int PART, bool X>
 __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict__ scp, WaveBuffers wb, int cur, int depth, int maxDepth, int dirmode, int prefetch) {
 	const DevScene &sc = *scp;
-	const unsigned n = wb.counts[cur];
+	unsigned n = wb.counts[cur];
 	const int nxt = cur ^ 1;
 	const unsigned stride = gridDim.x * blockDim.x;
 	if (PART == 1) {
@@ -182,6 +196,7 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 		}
 		return;
 	}
+	static_assert(PART != 3 || !X, "the flat launch does not use the node interpreter");
 	__shared__ unsigned s_dir[256];                               /* direction-bin sizes of the rays this block writes (blockDim.x == 256) */
 	__shared__ unsigned s_box[6];                                 /* dir mode 4: bounds of the origins this block writes (WaveBuffers::box) */
 	s_dir[threadIdx.x] = 0u;
@@ -189,11 +204,14 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 	unsigned *box_acc = wb.box + 12 * (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1);
 	const OriginBox obox = dirmode == 4 ? crg_origin_box(box_acc + 6) : OriginBox{};
 	__syncthreads();
-	if (blockIdx.x == 0 && threadIdx.x == 0) wb.counts[2] = 0u;   /* K2's work counter, for the next bounce */
-	if (blockIdx.x == 0) { wb.hist[threadIdx.x] = 0u; wb.hist[256 + threadIdx.x] = 0u; }   /* K2/K4 histogram + cursors (blockDim.x == 256) */
+	if (PART != 3) {                                              /* the flat launch runs first: the last one resets */
+		if (blockIdx.x == 0 && threadIdx.x == 0) wb.counts[2] = 0u;   /* K2's work counter, for the next bounce */
+		if (blockIdx.x == 0) { wb.hist[threadIdx.x] = 0u; wb.hist[256 + threadIdx.x] = 0u; }   /* K2/K4 histogram + cursors (blockDim.x == 256) */
+	}
 	const unsigned lane = threadIdx.x & 31u;
-	/* whole warps iterate together so the ballot below is convergent */
-	const unsigned first = PART == 2 ? wb.counts[4] : 0u;
+	/* whole warps iterate together so the ballot below is convergent; this launch walks perm[first .. n) */
+	const unsigned first = PART == 2 ? wb.counts[5] : (PART == 3 ? wb.counts[4] : 0u);
+	if (PART == 3) n = wb.counts[5];
 	const unsigned nround = first + ((n - first + 31u) & ~31u);
 	/* perm is read two iterations ahead and the records it points to one iteration ahead (crg_prefetch_l2): the five 16-B gathers
 	 * through perm are the DRAM-latency loads of this loop (the scene itself is L2-resident), so they are L2 hits when needed */
@@ -222,7 +240,7 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 			wr = b.z; wg = b.w; wbl = __uint_as_float(c.x);
 			id = c.y;
 			rng = (uint64_t)c.z | ((uint64_t)c.w << 32);
-			alive = cr_shade_one<X, PART != 2>(sc, wb.L, v3make(a.x, a.y, a.z), v3make(a.w, b.x, b.y), hit, wr, wg, wbl, id, rng, depth, maxDepth, p_next, d_next);
+			alive = cr_shade_one<X, PART == 0, PART == 3>(sc, wb.L, v3make(a.x, a.y, a.z), v3make(a.w, b.x, b.y), hit, wr, wg, wbl, id, rng, depth, maxDepth, p_next, d_next);
 		}
 		/* order-preserving warp compaction, one atomic per warp */
 		const unsigned mask = __ballot_sync(0xffffffffu, alive);
@@ -379,8 +397,8 @@ __global__ void k_kat(const DevScene *__restrict__ scp, const int32_t *__restric
 	outv[i] = k;
 }
 
-void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st) {
-	k_bucket<false><<<grid, 256, 0, st>>>(wb, cur, -1);
+void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, const uint8_t *order, int nflat, cudaStream_t st) {
+	k_bucket<false><<<grid, 256, 0, st>>>(wb, cur, -1, order, nflat);
 }
 /* X (the last template argument): the scene contains node kinds only the complete interpreter knows (DevScene::has_xnodes, set at
  * upload) — every other scene runs the kernels in which that interpreter is not even linked */
@@ -391,7 +409,10 @@ void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int de
 /* CRGPU_SHADE_MINB = 2|3|4 (blocks per SM of the hit/all kernel: 128 / 80 / 64 registers), CRGPU_SHADE_SPLIT = 0|1 (separate
  * miss kernel at 4 blocks per SM), CRGPU_SHADE_PREFETCH = 0|1 — read once; the defaults are what measured best.  On an H100 80GB HBM3
  * at a 400 W limit (hdr.json, 1080p, 1000 spp) the shading step takes 720 ms per frame with the hit kernel at 2 blocks per SM, 883 ms at 3 and 1068 ms at 4.
- * ptxas reports 784 B of spill stores for the hit kernel at 80 registers and 124 B at 128. */
+ * ptxas reports 784 B of spill stores for the hit kernel at 80 registers and 124 B at 128.
+ * CRGPU_SHADE_GENERIC_ONLY = 0|1 (1: no flat launch), CRGPU_SHADE_FLAT_MINB = 2|3|4: the flat hit kernel needs no call and no spill at
+ * 80 registers, and on an H100 80GB HBM3 at 700 W its shading step takes 481 ms per frame at 3 blocks per SM, 499 ms at 2, 502 ms at 4
+ * (616 ms with every hit through the interpreter). */
 const ShadeKnobs &crg_shade_knobs_env(void) {
 	static const ShadeKnobs kn = [] {
 		ShadeKnobs k;
@@ -402,6 +423,11 @@ const ShadeKnobs &crg_shade_knobs_env(void) {
 		k.split = e ? atoi(e) : 1;
 		e = getenv("CRGPU_SHADE_PREFETCH");
 		k.prefetch = e ? atoi(e) : 0;
+		e = getenv("CRGPU_SHADE_GENERIC_ONLY");
+		k.generic_only = e ? atoi(e) != 0 : 0;
+		e = getenv("CRGPU_SHADE_FLAT_MINB");
+		const int f = e ? atoi(e) : 3;
+		k.flat_minb = f >= 2 && f <= 4 ? f : 3;
 		return k;
 	}();
 	return kn;
@@ -411,6 +437,11 @@ static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, in
 	const int minb = kn.minb, split = kn.split, prefetch = kn.prefetch;
 	if (split) {
 		k_shade<4, 1, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		if (!kn.generic_only) {                                      /* perm[counts[4] .. counts[5]): the flat materials */
+			if (kn.flat_minb == 3) k_shade<3, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+			else if (kn.flat_minb == 4) k_shade<4, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+			else k_shade<2, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		}
 		if (minb == 3) k_shade<3, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		else if (minb == 4) k_shade<4, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		else k_shade<2, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
@@ -426,13 +457,14 @@ void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int d
 	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, st);
 }
 void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st) {
-	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot);
+	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot, nullptr, 0);
 }
 int crg_dir_mode(void) {
 	static const int mode = [] { const char *e = getenv("CRGPU_TRACE_SORT"); const int v = e ? atoi(e) : 0; return v >= 0 && v <= 4 ? v : 0; }();
 	return mode;
 }
-int crg_shade_launches_per_bounce(const ShadeKnobs &kn) { return kn.split ? 2 : 1; }
+int crg_shade_launches_per_bounce(const ShadeKnobs &kn) { return kn.split ? (kn.generic_only ? 2 : 3) : 1; }
+bool crg_shade_flat_order(const ShadeKnobs &kn) { return kn.split && !kn.generic_only; }
 
 /* ---- the libm stand-ins one by one (test entry crgpu_libm_eval; the order of include/crgpu.h CRGPU_LIBM_*) -------------------- */
 __global__ void k_libm(int fn, const float *__restrict__ x, const float *__restrict__ y, float *__restrict__ out, unsigned n) {

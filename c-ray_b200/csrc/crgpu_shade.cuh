@@ -125,29 +125,32 @@ template <int D, bool X> struct NodeEval {
 	static __device__ __noinline__ float alpha(const DevScene &sc, int node, const Rec &rec);
 };
 
-static __device__ __noinline__ col4 cr_image_color(const DevScene &sc, const crs_node &n, const Rec &rec) {            /* image.c:31-48 */
-	if (n.tex < 0) return c4make(1.0f, 0.0f, 0.5f, 1.0f);
-	const DevTexture t = sc.textures[n.tex];
+/* image.c:31-48, by value (tex / options of the image node, uv of the hit): the flat hit launch inlines these, the interpreter calls
+ * them through cr_image_color / cr_image_alpha */
+CRD col4 cr_image_color_at(const DevScene &sc, int32_t tex, uint32_t options, v2 uv) {
+	if (tex < 0) return c4make(1.0f, 0.0f, 0.5f, 1.0f);
+	const DevTexture t = sc.textures[tex];
 	col4 out;
-	if (n.options & CRS_IMG_NO_BILINEAR) {
-		const float x = rec.uv.x * (float)t.width;
-		const float y = rec.uv.y * (float)t.height;
+	if (options & CRS_IMG_NO_BILINEAR) {
+		const float x = uv.x * (float)t.width;
+		const float y = uv.y * (float)t.height;
 		out = cr_texture_get(sc, t, x, y, false);
 	} else {
-		out = cr_texture_get(sc, t, rec.uv.x, rec.uv.y, true);
+		out = cr_texture_get(sc, t, uv.x, uv.y, true);
 	}
-	if (n.options & CRS_IMG_SRGB_TRANSFORM)
+	if (options & CRS_IMG_SRGB_TRANSFORM)
 		out = c4make(cr_srgb_to_linear(out.r), cr_srgb_to_linear(out.g), cr_srgb_to_linear(out.b), out.a);
 	return out;
 }
-
-static __device__ __noinline__ float cr_image_alpha(const DevScene &sc, const crs_node &n, const Rec &rec) {
-	if (n.tex < 0) return 1.0f;
-	const DevTexture t = sc.textures[n.tex];
-	if (n.options & CRS_IMG_NO_BILINEAR)
-		return cr_texture_get_alpha(sc, t, rec.uv.x * (float)t.width, rec.uv.y * (float)t.height, false);
-	return cr_texture_get_alpha(sc, t, rec.uv.x, rec.uv.y, true);
+CRD float cr_image_alpha_at(const DevScene &sc, int32_t tex, uint32_t options, v2 uv) {
+	if (tex < 0) return 1.0f;
+	const DevTexture t = sc.textures[tex];
+	if (options & CRS_IMG_NO_BILINEAR)
+		return cr_texture_get_alpha(sc, t, uv.x * (float)t.width, uv.y * (float)t.height, false);
+	return cr_texture_get_alpha(sc, t, uv.x, uv.y, true);
 }
+static __device__ __noinline__ col4 cr_image_color(const DevScene &sc, const crs_node &n, const Rec &rec) { return cr_image_color_at(sc, n.tex, n.options, rec.uv); }
+static __device__ __noinline__ float cr_image_alpha(const DevScene &sc, const crs_node &n, const Rec &rec) { return cr_image_alpha_at(sc, n.tex, n.options, rec.uv); }
 
 CRD col4 cr_gradient(const crs_node &n, const Rec &rec) {                                   /* gradient.c:40-45 */
 	const v3 unit = v3norm(rec.inc_d);
@@ -508,6 +511,61 @@ CRD BsdfSample cr_sample_bsdf(const DevScene &sc, int root, uint64_t &rng, const
 		if (nt == 0) return vals[0];
 		node = todo[--nt];
 	}
+}
+
+/* cr_sample_bsdf for a flat material (DevFlat, folded at upload): the wrapper's MIX step, then the leaf of cr_sample_leaf or the
+ * PLASTIC step, with the same device functions in the same draw order and every node input read from the record.  No call, so
+ * rec stays in registers. */
+CRD BsdfSample cr_sample_flat(const DevScene &sc, const DevFlat &m, uint64_t &rng, const Rec &rec) {
+	BsdfSample s;
+	if (m.flags & CRG_FLAT_WRAPPED) {                                                         /* mix.c:42-50: Mix(Transparent(c0), leaf, Alpha(c)) */
+		const float lerp = (m.flags & CRG_FLAT_ALPHA_IMG) ? cr_image_alpha_at(sc, m.alpha_tex, m.alpha_opt, rec.uv) : m.alpha;
+		if (cr_draw(rng) > lerp) {                                                            /* transparent.c:40-44 */
+			s.out = rec.inc_d;
+			s.color = c4make(m.c0[0], m.c0[1], m.c0[2], m.c0[3]);
+			return s;
+		}
+	}
+	switch (m.kind) {
+	case CRG_FLAT_METAL: {                                                                    /* metal.c:40-55 */
+		const v3 nd = v3norm(rec.inc_d);
+		v3 reflected = v3reflect(nd, rec.n);
+		if (m.rough > 0.0f) reflected = v3add(reflected, v3scale(cr_random_on_unit_sphere(rng), m.rough));
+		s.out = reflected;
+		break;
+	}
+	case CRG_FLAT_GLASS: {                                                                    /* glass.c:41-87, as cr_sample_leaf */
+		v3 reflected = v3reflect(rec.inc_d, rec.n);
+		v3 refracted = reflected;
+		const float prob = cr_fresnel_probability(rec, m.ior, refracted);
+		if (m.rough > 0.0f) {
+			const v3 fuzz = v3scale(cr_random_on_unit_sphere(rng), m.rough);
+			reflected = v3add(reflected, fuzz);
+			refracted = v3add(refracted, fuzz);
+		}
+		s.out = cr_draw(rng) < prob ? reflected : refracted;
+		break;
+	}
+	case CRG_FLAT_PLASTIC: {                                                                  /* plastic.c:42-87 */
+		v3 refracted;
+		const float prob = cr_fresnel_probability(rec, rec.IOR, refracted);
+		if (cr_draw(rng) < prob) {
+			v3 reflected = v3reflect(rec.inc_d, rec.n);
+			if (m.rough > 0.0f) reflected = v3add(reflected, v3scale(cr_random_on_unit_sphere(rng), m.rough));
+			s.out = reflected;
+			s.color = c4make(1.0f, 1.0f, 1.0f, 1.0f);
+			return s;
+		}
+		s.out = v3norm(v3add(rec.n, cr_random_on_unit_sphere(rng)));                         /* the diffuse below: diffuse.c:40-47 */
+		break;
+	}
+	default:                                                                                  /* diffuse.c:40-47, emission.c:42-49 */
+		s.out = v3norm(v3add(rec.n, cr_random_on_unit_sphere(rng)));
+		break;
+	}
+	const col4 col = (m.flags & CRG_FLAT_COL_IMG) ? cr_image_color_at(sc, m.col_tex, m.col_opt, rec.uv) : c4make(m.col[0], m.col[1], m.col[2], m.col[3]);
+	s.color = m.kind == CRG_FLAT_EMISSIVE ? c4coef(m.strength, col) : col;
+	return s;
 }
 
 /* scene->background->sample(...) — background.c:39-66 (pathtrace.c:40) */

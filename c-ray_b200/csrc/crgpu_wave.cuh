@@ -39,7 +39,7 @@ struct WaveBuffers {
 	unsigned *perm2;        /* K4b output: the next bounce's rays grouped by direction bin — the order K2 hands them to its lanes */
 	unsigned *hist;         /* [256] bucket sizes (filled by K2), [256..511] K4 cursors, [512..767] direction-bin sizes (filled by K3),
 	                           [768..1023] K4b cursors */
-	unsigned *counts;       /* [0],[1]: live counts of the ping-pong halves; [2]: K2's work counter (next ray to hand out); [3]: tail-kernel block counter; [4]: number of misses of this bounce (K4 -> K3 split) */
+	unsigned *counts;       /* [0],[1]: live counts of the ping-pong halves; [2]: K2's work counter (next ray to hand out); [3]: tail-kernel block counter; [4]: number of misses of this bounce (K4 -> K3 split); [5]: end of the flat materials' range of perm (K4 -> K3 flat launch) */
 	unsigned *box;          /* [CRG_BOX_SLOTS][12]: bounds of the origins K3 wrote at depth min(d, CRG_BOX_SLOTS - 1), for the origin cell of
 	                           dir mode 4.  [0..5] = this batch (lo x,y,z as ~crg_ord(lo), hi x,y,z as crg_ord(hi); atomicMax, 0 = empty),
 	                           [6..11] = the previous batch of this wave set: K3 keys its rays with those, K4b moves [0..5] there */
@@ -87,18 +87,25 @@ void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, 
 /* 0 = off, 1 = octant (8 bins), 2 = octant x major axis (24 bins), 3 = octant x origin cell in the world box (256 bins),
  * 4 = octant x 5-bit Morton cell of the origin in the bounds of the previous batch's origins at the same depth (256 bins) */
 int crg_dir_mode(void);
-void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, cudaStream_t st);
+/* K4.  order: NULL (buckets in key order) or DevScene::key_order with nflat = DevScene::flat_keys (the flat materials' buckets
+ * right behind the misses, for the flat K3 launch); it also writes counts[4] (misses) and counts[5] (end of the flat range) */
+void crg_launch_bucket(const WaveBuffers &wb, int cur, int grid, const uint8_t *order, int nflat, cudaStream_t st);
 void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, bool xnodes, cudaStream_t st);
 /* Launch variant of K3.  Every variant computes the same path states.
- *   minb      blocks per SM of the hit kernel (or of the one kernel when not split): 2, 3 or 4
- *   split     1 = a separate miss kernel (PART 1) ahead of the hit kernel (PART 2); 0 = one kernel for every ray (PART 0)
- *   prefetch  1 = read perm two iterations ahead and prefetch the records it points to into L2
- * The frame path reads them once from CRGPU_SHADE_MINB / _SPLIT / _PREFETCH (crg_shade_knobs_env); crgpu_shade_rays passes its own. */
-struct ShadeKnobs { int minb, split, prefetch; };
+ *   minb          blocks per SM of the generic hit kernel (or of the one kernel when not split): 2, 3 or 4
+ *   split         1 = a separate miss kernel (PART 1) ahead of the hit kernels (PART 3, PART 2); 0 = one kernel for every ray (PART 0)
+ *   prefetch      1 = read perm two iterations ahead and prefetch the records it points to into L2
+ *   generic_only  1 = no flat launch: every hit goes through the node interpreter (PART 2), K4 keeps the buckets in key order
+ *   flat_minb     blocks per SM of the flat hit kernel (PART 3): 2, 3 or 4
+ * The frame path reads them once from CRGPU_SHADE_MINB / _SPLIT / _PREFETCH / _GENERIC_ONLY / _FLAT_MINB (crg_shade_knobs_env);
+ * crgpu_shade_rays passes its own. */
+struct ShadeKnobs { int minb, split, prefetch, generic_only, flat_minb; };
 const ShadeKnobs &crg_shade_knobs_env(void);
 void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid,
                       const ShadeKnobs &kn, cudaStream_t st);
 int crg_shade_launches_per_bounce(const ShadeKnobs &kn);
+/* whether K4 must order the buckets for the flat launch (crg_launch_bucket's order) */
+bool crg_shade_flat_order(const ShadeKnobs &kn);
 /* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st);

@@ -81,6 +81,10 @@ int  crgpu_prepare(const struct crs_scene *flat, crgpu_prepared **out);
 int  crgpu_prepared_update_config(crgpu_prepared *p, const struct crs_scene *flat);
 int  crgpu_prepared_slab(const crgpu_prepared *p, const void **slab, size_t *bytes);
 void crgpu_prepared_free(crgpu_prepared *p);
+/* How the shading kernels will sample each material: kinds[i] = 0 for a generic material (the node interpreter), else the flat
+ * leaf (1 diffuse, 2 metal, 3 glass, 4 emissive, 5 plastic over a diffuse) with flags[i] bit 0 = under the alpha wrapper, bit 1 =
+ * the wrapper's alpha is an image, bit 2 = the leaf colour is an image.  Fills min(count, material count) entries. */
+int  crgpu_prepared_materials(const crgpu_prepared *p, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count);
 int  crgpu_scene_create_prepared(const crgpu_prepared *p, int device, crgpu_scene **out);
 
 /* Device memory released by crgpu_scene_destroy is kept in a per-device cache for the next scene (a frame's 35 GB of
@@ -185,6 +189,8 @@ struct crgpu_shade_opts {
 	int32_t complete_interpreter;  /* 1: the complete node interpreter even when the scene does not need it */
 	int32_t tail;                  /* 1: the tail kernel instead of K2 -> K4 -> K3 */
 	int32_t depth, max_depth;      /* the bounce and the scene's bounce limit */
+	int32_t generic_only;          /* 1: every hit through the node interpreter; 0: hits on flat materials through the flat launch
+	                                  (when split; it then runs at `minb` too) */
 };
 struct crgpu_shade_result {
 	struct crgpu_ray_record rec;
