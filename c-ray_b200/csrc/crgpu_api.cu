@@ -153,6 +153,7 @@ struct crgpu_prepared {
 	uint32_t material_count;
 	uint32_t flat_keys;        /* DevScene::flat_keys */
 	bool xnodes;               /* some node is of a kind only the complete interpreter (NodeX) evaluates */
+	DevFlatBg bg;              /* DevScene::bg */
 	uint8_t *slab;
 	bool pinned;
 	size_t slab_bytes;
@@ -390,6 +391,25 @@ static DevFlat fold_flat(const crs_scene *f, int root) {
 	return d;
 }
 
+/* ---- the folded background (DevFlatBg): BACKGROUND(constant | image | gradient colour, constant strength, constant offset) ---------
+ * host/loader/cr_sceneload.c builds every JSON scene's background in this form (crl_background).  Folding copies the node fields
+ * cr_sample_background reads and computes nothing; any other graph stays with the interpreter (kind CRG_BG_NONE). */
+static DevFlatBg fold_background(const crs_scene *f, int root) {
+	DevFlatBg b;
+	memset(&b, 0, sizeof b);
+	const crs_node &r = f->nodes[root];
+	if (!flat_value(f, r.in[1], b.strength) || !flat_value(f, r.in[2], b.offset) || !node_ok(f, r.in[0])) { memset(&b, 0, sizeof b); return b; }
+	const crs_node &c = f->nodes[r.in[0]];
+	switch (c.kind) {
+	case CRS_COLOR_CONSTANT: b.kind = CRG_BG_CONSTANT; break;
+	case CRS_COLOR_IMAGE: b.kind = CRG_BG_IMAGE; b.tex = c.tex; b.opt = c.options; break;
+	case CRS_COLOR_GRADIENT: b.kind = CRG_BG_GRADIENT; break;
+	default: memset(&b, 0, sizeof b); return b;
+	}
+	memcpy(b.f, c.f, sizeof b.f);
+	return b;
+}
+
 /* ---- BVH re-layout: reference nodes (bvh.c:37-42) -> BFS-ordered PairNodes ---------------------------------------- */
 /* errors raised on worker threads (fail() writes a thread-local buffer): first one wins, reported by the caller */
 struct HostError {
@@ -558,6 +578,12 @@ extern "C" int crgpu_prepared_materials(const crgpu_prepared *p, uint32_t *kinds
 	return CRGPU_OK;
 }
 
+extern "C" int crgpu_prepared_background(const crgpu_prepared *p, uint32_t *kind) {
+	if (!p || !kind) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	*kind = p->bg.kind;
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_prepared_slab(const crgpu_prepared *p, const void **slab, size_t *bytes) {
 	if (!p) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (slab) *slab = p->slab;
@@ -582,6 +608,7 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 		if (k == CRS_COLOR_VECTOCOLOR || k == CRS_COLOR_COMBINE_VALUE || k == CRS_COLOR_COMBINE_RGB || k == CRS_VALUE_MATH || k == CRS_VALUE_FRESNEL ||
 			k == CRS_VALUE_RAYLENGTH || k == CRS_VECTOR_CONSTANT || k == CRS_VECTOR_NORMAL || k == CRS_VECTOR_VECMATH) p->xnodes = true;
 	}
+	p->bg = fold_background(f, f->background);
 	p->texture_count = f->texture_count;
 #define PFAIL(x) do { int rc_ = (x); if (rc_) return pfail(p, rc_); } while (0)
 
@@ -941,6 +968,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	d.flat = reinterpret_cast<const DevFlat *>(base + p->off[SEC_FLAT]);
 	d.key_order = base + p->off[SEC_ORDER];
 	d.flat_keys = p->flat_keys;
+	d.bg = p->bg;
 	d.nodes = reinterpret_cast<const crs_node *>(base + p->off[SEC_NODES]);
 	d.textures = reinterpret_cast<const DevTexture *>(base + p->off[SEC_TEXS]);
 	d.u8_to_unit = reinterpret_cast<const float *>(base + p->off[SEC_LUT]);
@@ -1076,7 +1104,11 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	uint64_t launches = 0;
 	float trace_ms = 0.f, shade_ms = 0.f;
 	if (timing) CU(cudaEventRecord(s->ev[0], s->stream));
-	std::vector<cudaEvent_t> tev;   /* per-kernel events when timing */
+	/* per-kernel events when timing: per batch K1's start and end (gev); per bounce CRG_TEV events (tev): before K2, after K2, after
+	 * K4, after each of K3's miss / flat / generic launches, after the K4b sort */
+	enum { CRG_TEV = 7 };
+	std::vector<cudaEvent_t> tev, gev;
+	auto mark = [&](std::vector<cudaEvent_t> &v, cudaStream_t on) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, on); v.push_back(e); };
 	if (sets == 2) {                /* fork: the second stream starts behind whatever is queued on the first */
 		CU(cudaEventRecord(s->evFork, s->stream));
 		CU(cudaStreamWaitEvent(s->stream2, s->evFork, 0));
@@ -1090,25 +1122,33 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 		td.npix = (unsigned)tile_pixels;
 		td.pass_begin = pb;
 		td.pass_count = (pass_begin + pass_count - pb) < (int)batch ? (pass_begin + pass_count - pb) : (int)batch;
+		if (timing) mark(gev, st);
 		crg_launch_generate(s->dev, wb, td, grid, st); ++launches;
+		if (timing) mark(gev, st);
 		/* bounces == 0: pathTrace's loop never runs and every sample is black (pathtrace.c:34-36,59).  L is write-once by
 		 * design (cr_add_radiance / cr_finish_path), so with no bounce nothing would write it: clear it here instead */
 		if (maxDepth == 0) CU(cudaMemsetAsync(wb.L, 0, (size_t)tile_pixels * (size_t)td.pass_count * sizeof(float4), st));
 		int cur = 0;
 		for (int depth = 0; depth < maxDepth; ++depth) {
 			if (depth >= CRG_TAIL_FROM && !count) { crg_launch_tail(s->dev_copy, wb, cur, depth, maxDepth, s->xnodes, st); ++launches; }
-			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
+			if (timing) mark(tev, st);
 			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, knobs, st);
-			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
+			if (timing) mark(tev, st);
 			if (crg_shade_flat_order(sknobs)) crg_launch_bucket(wb, cur, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
 			else crg_launch_bucket(wb, cur, grid, nullptr, 0, st);
+			cudaEvent_t k3ev[3] = { nullptr, nullptr, nullptr };
+			if (timing) {
+				mark(tev, st);
+				for (cudaEvent_t &e : k3ev) { cudaEventCreate(&e); tev.push_back(e); }
+			}
 			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
-			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, grid, sknobs, st);
+			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, s->dev.bg.kind != CRG_BG_NONE, grid, sknobs, st,
+			                 timing ? k3ev : nullptr);
 			if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
 				crg_launch_dirsort(wb, cur ^ 1, dirmode == 4 ? (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1) : -1, grid, st);
 				++launches;
 			}
-			if (timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); }
+			if (timing) mark(tev, st);
 			launches += 2 + (uint64_t)crg_shade_launches_per_bounce(sknobs);
 			cur ^= 1;
 		}
@@ -1129,15 +1169,27 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 		CU(cudaStreamSynchronize(st));
 		float total_ms = 0.f;
 		cudaEventElapsedTime(&total_ms, s->ev[0], s->ev[1]);
-		for (size_t i = 0; i + 3 <= tev.size(); i += 3) {
-			float a = 0.f, b = 0.f;
-			cudaEventElapsedTime(&a, tev[i], tev[i + 1]);
-			cudaEventElapsedTime(&b, tev[i + 1], tev[i + 2]);
+		const char *dump = getenv("CRGPU_DUMP_TIMES");
+		const int dump_level = dump ? atoi(dump) : 0;
+		/* CRGPU_DUMP_TIMES=2: K1 per batch, and per bounce K2 (trace), K4 + K3 (shade) and shade's parts: K4, K3's miss / flat / generic
+		 * launches (an unsplit K3 counts as miss), the rest (the K4b sort) */
+		for (size_t i = 0; dump_level > 1 && i + 2 <= gev.size(); i += 2) {
+			float g = 0.f;
+			cudaEventElapsedTime(&g, gev[i], gev[i + 1]);
+			fprintf(stderr, "crgpu: batch %zu k1 %.3f ms\n", i / 2, g);
+		}
+		for (size_t i = 0; i + CRG_TEV <= tev.size(); i += CRG_TEV) {
+			float t[CRG_TEV - 1] = {};
+			for (int k = 0; k + 1 < CRG_TEV; ++k) cudaEventElapsedTime(&t[k], tev[i + (size_t)k], tev[i + (size_t)k + 1]);
+			const float a = t[0], b = t[1] + t[2] + t[3] + t[4] + t[5];
 			trace_ms += a; shade_ms += b;
-			if (getenv("CRGPU_DUMP_TIMES") && (a > 5.f || b > 8.f || atoi(getenv("CRGPU_DUMP_TIMES")) > 1))
-				fprintf(stderr, "crgpu: batch %zu depth %zu trace %.3f ms shade %.3f ms\n", (i / 3) / (size_t)maxDepth, (i / 3) % (size_t)maxDepth, a, b);
+			const size_t bounce = i / CRG_TEV;
+			if (dump && (a > 5.f || b > 8.f || dump_level > 1))
+				fprintf(stderr, "crgpu: batch %zu depth %zu trace %.3f ms shade %.3f ms k4 %.3f miss %.3f flat %.3f generic %.3f sort %.3f\n",
+				        bounce / (size_t)maxDepth, bounce % (size_t)maxDepth, a, b, t[1], t[2], t[3], t[4], t[5]);
 		}
 		for (cudaEvent_t e : tev) cudaEventDestroy(e);
+		for (cudaEvent_t e : gev) cudaEventDestroy(e);
 		s->pend_trace_ms += trace_ms; s->pend_shade_ms += shade_ms; s->pend_total_ms += total_ms;
 	}
 	if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
@@ -1442,7 +1494,7 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 		if (crg_shade_flat_order(kn)) crg_launch_bucket(wb, 0, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
 		else crg_launch_bucket(wb, 0, grid, nullptr, 0, st);
 		const bool sort_next = opts->dirmode != 0 && depth + 1 < maxDepth;
-		crg_launch_shade(s->dev_copy, wb, 0, depth, maxDepth, sort_next ? opts->dirmode : 0, xnodes, grid, kn, st);
+		crg_launch_shade(s->dev_copy, wb, 0, depth, maxDepth, sort_next ? opts->dirmode : 0, xnodes, s->dev.bg.kind != CRG_BG_NONE, grid, kn, st);
 		if (sort_next) crg_launch_dirsort(wb, 1, opts->dirmode == 4 ? box_slot : -1, grid, st);
 	}
 	CU(cudaGetLastError());

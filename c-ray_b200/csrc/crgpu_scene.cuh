@@ -100,6 +100,21 @@ struct __align__(16) DevFlat {
 	float    rough, ior, strength;             /* value inputs (f[0]); plastic: rough = f[0] of its roughness colour */
 };
 
+/* A folded background (crgpu_api.cu fold_background): BACKGROUND(colour, strength, offset) whose colour is a constant, an image
+ * or a gradient and whose strength and offset are value constants — every background the JSON loader builds.  The miss launch
+ * of K3 samples it inline (cr_sample_flat_bg) instead of calling the node interpreter; the fields are bit copies of the node
+ * fields cr_sample_background reads. */
+#define CRG_BG_NONE     0u          /* generic: the interpreter samples it */
+#define CRG_BG_CONSTANT 1u
+#define CRG_BG_IMAGE    2u
+#define CRG_BG_GRADIENT 3u
+struct DevFlatBg {
+	uint32_t kind;
+	int32_t  tex;  uint32_t opt;               /* image colour: crs_node.tex / .options */
+	float    strength, offset;                 /* f[0] of the value constants */
+	float    f[8];                             /* the colour node's f: constant f[0..3], gradient down f[0..3] / up f[4..7] */
+};
+
 struct DevTexture {
 	uint32_t width, height, channels, is_float, has_alpha;
 	uint32_t wmask, hmask;          /* width-1 / height-1 when that dimension is a power of two, else 0 (x % W == x & (W-1), also for the
@@ -134,6 +149,7 @@ struct DevScene {
 	const DevFlat    *flat;         /* [material] folded flat record (kind CRG_FLAT_NONE: generic) */
 	const uint8_t    *key_order;    /* [256] K4's bucket order: the miss key, the keys of flat materials, then the generic keys */
 	uint32_t          flat_keys;    /* number of flat keys (they take ranks 1..flat_keys of key_order) */
+	DevFlatBg         bg;           /* folded background (kind CRG_BG_NONE: the interpreter samples nodes[background]) */
 	const crs_node   *nodes;
 	const DevTexture *textures;
 	const PairNode   *stage_img;    /* top-of-tree pair nodes of every BVH, contiguous: K2 copies it into shared memory with one

@@ -176,8 +176,9 @@ CRD unsigned cr_dir_bin(const DevScene &sc, const OriginBox &box, v3 o, v3 d, in
  * PART 0: every ray of the queue.  PART 1 / 3 / 2: the parts of a split launch — 1 = the misses (bucket 0 = perm[0 .. counts[4]):
  * background lookup + radiance, the path always ends, nothing to compact), 3 = the hits on flat materials (perm[counts[4] ..
  * counts[5]): cr_sample_flat, no node interpreter), 2 = the other hits (perm[counts[5] .. n)).  The miss half needs a third of the
- * registers of the hit half, so it runs at twice the occupancy; on hdr.json 40% of all rays are misses and every hit is flat. */
-template <int MINB, int PART, bool X>
+ * registers of the hit half, so it runs at twice the occupancy; on hdr.json 40% of all rays are misses and every hit is flat.
+ * FLATBG (miss launch only): the scene's background is folded (DevScene::bg) and sampled inline by cr_sample_flat_bg. */
+template <int MINB, int PART, bool X, bool FLATBG = false>
 __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict__ scp, WaveBuffers wb, int cur, int depth, int maxDepth, int dirmode, int prefetch) {
 	const DevScene &sc = *scp;
 	unsigned n = wb.counts[cur];
@@ -191,7 +192,8 @@ __global__ void __launch_bounds__(256, MINB) k_shade(const DevScene *__restrict_
 			const float4 b = crg_half(wb.stB, cur)[i];
 			const uint4 c = crg_half(wb.stC, cur)[i];
 			unsigned id = c.y;
-			const col4 bg = cr_sample_background<X>(sc, v3make(a.w, b.x, b.y));                 /* pathtrace.c:39-42 */
+			const v3 d = v3make(a.w, b.x, b.y);
+			const col4 bg = FLATBG ? cr_sample_flat_bg(sc, sc.bg, d) : cr_sample_background<X>(sc, d);               /* pathtrace.c:39-42 */
 			cr_add_radiance(wb.L, id, b.z * bg.r, b.w * bg.g, __uint_as_float(c.x) * bg.b);
 		}
 		return;
@@ -433,28 +435,34 @@ const ShadeKnobs &crg_shade_knobs_env(void) {
 	return kn;
 }
 template <bool X>
-static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, const ShadeKnobs &kn, cudaStream_t st) {
+static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, const ShadeKnobs &kn,
+                         bool flat_bg, cudaStream_t st, cudaEvent_t *ev) {
 	const int minb = kn.minb, split = kn.split, prefetch = kn.prefetch;
 	if (split) {
-		k_shade<4, 1, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		if (flat_bg) k_shade<4, 1, X, true><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		else k_shade<4, 1, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		if (ev) cudaEventRecord(ev[0], st);
 		if (!kn.generic_only) {                                      /* perm[counts[4] .. counts[5]): the flat materials */
 			if (kn.flat_minb == 3) k_shade<3, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 			else if (kn.flat_minb == 4) k_shade<4, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 			else k_shade<2, 3, false><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		}
+		if (ev) cudaEventRecord(ev[1], st);
 		if (minb == 3) k_shade<3, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		else if (minb == 4) k_shade<4, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		else k_shade<2, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+		if (ev) cudaEventRecord(ev[2], st);
 		return;
 	}
 	if (minb == 3) k_shade<3, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	else if (minb == 4) k_shade<4, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	else k_shade<2, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
+	if (ev) for (int k = 0; k < 3; ++k) cudaEventRecord(ev[k], st);   /* one launch: it is all in the "miss" share */
 }
-void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, int grid,
-                      const ShadeKnobs &kn, cudaStream_t st) {
-	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, st);
-	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, st);
+void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, bool flat_bg, int grid,
+                      const ShadeKnobs &kn, cudaStream_t st, cudaEvent_t *ev) {
+	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
+	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
 }
 void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st) {
 	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot, nullptr, 0);

@@ -152,11 +152,12 @@ CRD float cr_image_alpha_at(const DevScene &sc, int32_t tex, uint32_t options, v
 static __device__ __noinline__ col4 cr_image_color(const DevScene &sc, const crs_node &n, const Rec &rec) { return cr_image_color_at(sc, n.tex, n.options, rec.uv); }
 static __device__ __noinline__ float cr_image_alpha(const DevScene &sc, const crs_node &n, const Rec &rec) { return cr_image_alpha_at(sc, n.tex, n.options, rec.uv); }
 
-CRD col4 cr_gradient(const crs_node &n, const Rec &rec) {                                   /* gradient.c:40-45 */
-	const v3 unit = v3norm(rec.inc_d);
+CRD col4 cr_gradient_at(const float (&f)[8], v3 inc_d) {                                     /* gradient.c:40-45 */
+	const v3 unit = v3norm(inc_d);
 	const float t = 0.5f * (unit.y + 1.0f);
-	return c4add(c4coef(1.0f - t, c4make(n.f[0], n.f[1], n.f[2], n.f[3])), c4coef(t, c4make(n.f[4], n.f[5], n.f[6], n.f[7])));
+	return c4add(c4coef(1.0f - t, c4make(f[0], f[1], f[2], f[3])), c4coef(t, c4make(f[4], f[5], f[6], f[7])));
 }
+CRD col4 cr_gradient(const crs_node &n, const Rec &rec) { return cr_gradient_at(n.f, rec.inc_d); }
 
 template <int D, bool X>
 __device__ __noinline__ col4 NodeEval<D, X>::color(const DevScene &sc, int node, const Rec &rec) {
@@ -589,6 +590,30 @@ static __device__ __noinline__ col4 cr_sample_background(const DevScene &sc, v3 
 	rec.uv.x = v; rec.uv.y = u;
 	const float strength = NodesT<X>::value(sc, n.in[1], rec);
 	return c4coef(strength, NodesT<X>::color(sc, n.in[0], rec));
+}
+
+/* cr_sample_background for a folded background (DevFlatBg): the same operations in the same order, every node input read from the
+ * record and no call, so the miss launch keeps everything in registers.  A constant or gradient colour does not read the uv the
+ * interpreter computes first; those operations have no other effect and are skipped. */
+CRD col4 cr_sample_flat_bg(const DevScene &sc, const DevFlatBg &bg, v3 dir) {
+	col4 c;
+	if (bg.kind == CRG_BG_IMAGE) {
+		const v3 ud = v3norm(dir);
+		const float phi = cr_div(cr_atan2f(ud.z, ud.x), 4.0f) + bg.offset;
+		const float theta = cr_acosf(cr_div(-ud.y, 1.0f));
+		float u = cr_div(theta, CR_PI);
+		float v = cr_div(phi, CR_PI / 2.0f);
+		u = cr_wrapMinMax(u, 0.0f, 1.0f);
+		v = cr_wrapMinMax(v, 0.0f, 1.0f);
+		v2 uv;
+		uv.x = v; uv.y = u;
+		c = cr_image_color_at(sc, bg.tex, bg.opt, uv);
+	} else if (bg.kind == CRG_BG_GRADIENT) {
+		c = cr_gradient_at(bg.f, dir);
+	} else {
+		c = c4make(bg.f[0], bg.f[1], bg.f[2], bg.f[3]);
+	}
+	return c4coef(bg.strength, c);
 }
 
 /* ---- hit reconstruction: everything intersectSphere/intersectMesh do after the closest primitive is known ------------------ */

@@ -85,6 +85,9 @@ void crgpu_prepared_free(crgpu_prepared *p);
  * leaf (1 diffuse, 2 metal, 3 glass, 4 emissive, 5 plastic over a diffuse) with flags[i] bit 0 = under the alpha wrapper, bit 1 =
  * the wrapper's alpha is an image, bit 2 = the leaf colour is an image.  Fills min(count, material count) entries. */
 int  crgpu_prepared_materials(const crgpu_prepared *p, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count);
+/* How the miss launch will sample the background: *kind = 0 through the node interpreter, else folded at upload with a constant
+ * strength and offset over a 1 constant, 2 image or 3 gradient colour. */
+int  crgpu_prepared_background(const crgpu_prepared *p, uint32_t *kind);
 int  crgpu_scene_create_prepared(const crgpu_prepared *p, int device, crgpu_scene **out);
 
 /* Device memory released by crgpu_scene_destroy is kept in a per-device cache for the next scene (a frame's 35 GB of
