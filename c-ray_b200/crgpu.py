@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(HERE, "libcrgpu.so")
 FLAG_COUNT = 0x1
 FLAG_TIME_KERNELS = 0x2
 FLAG_ASYNC = 0x4
+STOPPED = 1          # CRGPU_STOPPED: an armed render call ended at a pass boundary because a stop was requested
 
 
 class Prefs(C.Structure):
@@ -115,6 +116,10 @@ def lib():
         L.crgpu_scene_create_prepared.argtypes = [P, C.c_int, C.POINTER(P)]
         L.crgpu_scene_info.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.crgpu_device_trim.argtypes = [C.c_int]
+        L.crgpu_stop_enable.argtypes = [P, C.c_int]
+        L.crgpu_request_stop.argtypes = [P]
+        L.crgpu_clear_stop.argtypes = [P]
+        L.crgpu_progress.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.crscene_load.argtypes = [C.POINTER(FlatScene), C.c_char_p]
         L.crscene_free.argtypes = [C.POINTER(FlatScene)]
         L.crscene_set_config.argtypes = [C.POINTER(FlatScene)] + [C.c_int] * 4
@@ -123,6 +128,7 @@ def lib():
                   "crgpu_framebuffer_to_srgb8", "crgpu_framebuffer_device_ptr", "crgpu_trace_kat", "crgpu_trace_rays", "crscene_load",
                   "crgpu_shade_rays", "crgpu_libm_eval", "crgpu_prepared_background",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
+                  "crgpu_stop_enable", "crgpu_request_stop", "crgpu_clear_stop", "crgpu_progress",
                   "crscene_set_config"):
             getattr(L, f).restype = C.c_int
         _lib = L
@@ -182,22 +188,49 @@ class GpuScene:
             _check(L.crgpu_set_max_paths_in_flight(self.handle, int(max_paths)), "crgpu_set_max_paths_in_flight")
 
     def render_tile(self, x0, y0, x1, y1, pass_begin=0, pass_count=None, flags=0):
+        """Returns the call's stats (None with FLAG_ASYNC); on an armed scene the dict has "stopped": whether the call ended early."""
         st = Stats()
         if pass_count is None:
             pass_count = self.samples - pass_begin
-        _check(lib().crgpu_render_tile(self.handle, x0, y0, x1, y1, pass_begin, pass_count, flags, C.byref(st)),
-               "crgpu_render_tile")
-        return None if (flags & FLAG_ASYNC) else st.as_dict()
+        rc = lib().crgpu_render_tile(self.handle, x0, y0, x1, y1, pass_begin, pass_count, flags, C.byref(st))
+        return self._render_result(rc, flags, st, "crgpu_render_tile")
 
     def render_tiles(self, rects, pass_begin=0, pass_count=None, flags=0):
-        """Render a union of tiles [(x0, y0, x1, y1), ...] as ONE wavefront."""
+        """Render a union of tiles [(x0, y0, x1, y1), ...] as ONE wavefront (the result as for render_tile)."""
         st = Stats()
         if pass_count is None:
             pass_count = self.samples - pass_begin
         arr = np.ascontiguousarray(rects, dtype=np.int32).reshape(-1, 4)
-        _check(lib().crgpu_render_tiles(self.handle, arr.ctypes.data, len(arr), pass_begin, pass_count, flags, C.byref(st)),
-               "crgpu_render_tiles")
-        return None if (flags & FLAG_ASYNC) else st.as_dict()
+        rc = lib().crgpu_render_tiles(self.handle, arr.ctypes.data, len(arr), pass_begin, pass_count, flags, C.byref(st))
+        return self._render_result(rc, flags, st, "crgpu_render_tiles")
+
+    def _render_result(self, rc, flags, st, what):
+        if rc != STOPPED:
+            _check(rc, what)
+        if flags & FLAG_ASYNC:
+            return None
+        d = st.as_dict()
+        if getattr(self, "armed", False):
+            d["stopped"] = rc == STOPPED
+        return d
+
+    def enable_stop(self, on=True):
+        """Arm (or disarm) the scene: its render calls can then be stopped at a pass boundary (crgpu_stop_enable)."""
+        _check(lib().crgpu_stop_enable(self.handle, 1 if on else 0), "crgpu_stop_enable")
+        self.armed = bool(on)
+
+    def request_stop(self):
+        """Ask the call in flight (and every later call, until clear_stop) to end at the next pass boundary; any thread may call it."""
+        _check(lib().crgpu_request_stop(self.handle), "crgpu_request_stop")
+
+    def clear_stop(self):
+        _check(lib().crgpu_clear_stop(self.handle), "crgpu_clear_stop")
+
+    def progress(self):
+        """(committed pass index of the call in flight or of the last one, whether a call is in flight), without synchronising."""
+        done, busy = C.c_int(0), C.c_int(0)
+        _check(lib().crgpu_progress(self.handle, C.byref(done), C.byref(busy)), "crgpu_progress")
+        return done.value, bool(busy.value)
 
     def set_stream(self, cuda_stream_ptr):
         """Enqueue on a caller-owned cudaStream_t (int pointer, e.g. torch.cuda.current_stream().cuda_stream)."""

@@ -53,6 +53,12 @@ def lib():
         L.takeRankTiles.argtypes = [P, P, P]
         L.crhostTileOwners.argtypes = [P, C.c_int, P]
         L.crhostTileOwners.restype = None
+        L.crhostAbort.argtypes = [P, C.c_int]
+        L.crhostAbort.restype = None
+        L.crhostSetPaused.argtypes = [P, C.c_int]
+        L.crhostSetPaused.restype = None
+        L.crhostProgress.argtypes = [P, C.POINTER(C.c_ulonglong)]
+        L.crhostWorkerPasses.argtypes = [P, C.c_int]
         _lib = L
     return _lib
 
@@ -90,13 +96,36 @@ class Renderer:
             raise RuntimeError(f"joinRanks(rank {rank} of {world}, device {device}) failed")
 
     def render(self):
-        """renderFrame: upload -> tiles -> (gather) -> renderBuffer + 8-bit image on the host.  Returns (seconds, rays)."""
+        """renderFrame: upload -> tiles -> (gather) -> renderBuffer + 8-bit image on the host.  Returns (seconds, rays), or None
+        when the frame was aborted without saving (abort(save=False) from another thread)."""
         L = lib()
+        self._discard = False
         img = L.renderFrame(self.r)
         if not img:
+            if self._discard:
+                return None
             raise RuntimeError("renderFrame failed (see stderr)")
         L.destroyTexture8(img)
         return L.crhostRenderSeconds(self.r), int(L.crhostTotalRays(self.r))
+
+    # Controls of a frame in flight (any thread; render() releases the GIL while the frame renders).
+    def abort(self, save=True):
+        """Stop the frame at a pass boundary; with save, render() returns the committed passes, without it no image."""
+        self._discard = not save
+        lib().crhostAbort(self.r, 1 if save else 0)
+
+    def set_paused(self, on):
+        lib().crhostSetPaused(self.r, 1 if on else 0)
+
+    def progress(self):
+        """(whether a frame renders, tile-passes committed by all workers so far)"""
+        done = C.c_ulonglong(0)
+        busy = lib().crhostProgress(self.r, C.byref(done))
+        return bool(busy), int(done.value)
+
+    def worker_passes(self, t):
+        """passes worker t has committed in the current (or last) frame: its tiles hold exactly passes [0, that)"""
+        return int(lib().crhostWorkerPasses(self.r, t))
 
     def rank_tiles(self, rank, world):
         """(rects (n,4) int32, owner (tileCount,) int32, all_rects (tileCount,4)): this rank's share of the tile queue as the C

@@ -188,6 +188,9 @@ struct crgpu_scene {
 	uint32_t *pixels;          /* device pixel list of the last crgpu_render_tiles tile set */
 	size_t pixel_cap;
 	std::vector<int> pixel_key;
+	bool armed;                /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
+	unsigned *stop_host;       /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight (NULL until armed once) */
+	unsigned *stop_ctl;        /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets */
 };
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
@@ -550,6 +553,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	if (s->evFork) cudaEventDestroy(s->evFork);
 	if (s->stream2) cudaStreamDestroy(s->stream2);
 	if (s->own_stream) cudaStreamDestroy(s->own_stream);
+	if (s->stop_host) cudaFreeHost(s->stop_host);
 	delete s;
 	return CRGPU_OK;
 }
@@ -913,6 +917,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	memset(&s->wb2, 0, sizeof s->wb2);
 	s->wave_sets = 0; s->stream2 = nullptr; s->evAcc[0] = s->evAcc[1] = nullptr; s->evFork = nullptr;
 	s->pixels = nullptr; s->pixel_cap = 0;
+	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr;
 	s->device = device; s->xnodes = p->xnodes; s->dev_copy = nullptr; s->fb = nullptr; s->fb8 = nullptr; s->stream = nullptr; s->own_stream = nullptr; s->cap_paths = 0;
 	s->slab = nullptr; s->slab_bytes = 0; s->small = nullptr; s->small_bytes = 0; s->wave = nullptr; s->wave_bytes = 0; s->fb_floats = 0;
 	memset(s->fetched, 0, sizeof s->fetched);
@@ -979,9 +984,9 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->fb_floats = (size_t)d.image_width * d.image_height * 3u;
 	{ void *q = nullptr; FAIL_IF(ctx_alloc(device, s->fb_floats * sizeof(float), &q)); s->fb = static_cast<float *>(q); }
 	CUS(cudaMemsetAsync(s->fb, 0, s->fb_floats * sizeof(float), s->stream));
-	{	/* per wave set: hist[1024] + counts[64] + box[CRG_BOX_SLOTS][12]; then the shared stats[80] */
+	{	/* per wave set: hist[1024] + counts[64] + box[CRG_BOX_SLOTS][12]; then the shared stats[80] and the stop words[16] */
 		const size_t set_bytes = 1024 * sizeof(unsigned) + 256 + CRG_BOX_SLOTS * 12 * sizeof(unsigned);
-		s->small_bytes = 2 * set_bytes + 80 * sizeof(unsigned long long);
+		s->small_bytes = 2 * set_bytes + 80 * sizeof(unsigned long long) + 16 * sizeof(unsigned);
 		FAIL_IF(ctx_alloc(device, s->small_bytes, &s->small));
 		CUS(cudaMemsetAsync(s->small, 0, s->small_bytes, s->stream));
 		uint8_t *sm = static_cast<uint8_t *>(s->small);
@@ -992,6 +997,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 		s->wb2.counts = s->wb2.hist + 1024;
 		s->wb2.box = s->wb2.hist + 1024 + 64;
 		s->wb.stats = s->wb2.stats = reinterpret_cast<unsigned long long *>(sm + 2 * set_bytes);
+		s->stop_ctl = reinterpret_cast<unsigned *>(sm + 2 * set_bytes + 80 * sizeof(unsigned long long));
 	}
 	{
 		/* Paths in flight per wavefront batch.  Every batch pays a fixed ~7 ms (the serial chain of its bounces: each
@@ -1041,11 +1047,24 @@ static int check_rect(const crgpu_scene *s, int x0, int y0, int x1, int y1) {
 	return CRGPU_OK;
 }
 
+/* How render_pixels runs the gates of an armed call (render_armed).  A whole call: every batch checks the stop word and publishes.
+ * A piece of a pass-major walk (one batch of passes over one piece): only the first piece of a pass batch checks the stop word,
+ * the later ones follow its decision, and the last piece publishes the pass batch. */
+struct StopArm {
+	bool first;                /* reset the abandoned flag at the first gate and check the stop word at every gate */
+	bool last;                 /* publish after K5 */
+	bool whole;                /* a whole call: stop enqueueing batches once the stop word is set */
+	uint64_t call_pixels;      /* pixels of the whole call (a pass batch commits call_pixels * passes paths) */
+};
+static int render_armed(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats);
+static bool stop_requested(const crgpu_scene *s) { return __atomic_load_n(&s->stop_host[0], __ATOMIC_ACQUIRE) != 0u; }
+
 /* the wavefront driver: passes [pass_begin, +pass_count) over a pixel set (a rectangle, or an explicit list) */
 static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count,
-						 unsigned flags, struct crgpu_stats *stats) {
+						 unsigned flags, struct crgpu_stats *stats, const StopArm *arm = nullptr) {
 	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
+	if (s->armed && !arm) return render_armed(s, base, tile_pixels, pass_begin, pass_count, flags, stats);
 	if (tile_pixels > s->max_paths) {
 		/* more pixels than paths in flight: walk the pixel set in pieces (rows of the rectangle / ranges of the list) */
 		const unsigned inner = flags | CRGPU_FLAG_ASYNC;
@@ -1115,6 +1134,7 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	}
 	int bi = 0;
 	for (int pb = pass_begin; pb < pass_begin + pass_count; pb += (int)batch, ++bi) {
+		if (arm && arm->whole && stop_requested(s)) break;       /* its gates would abandon it anyway */
 		const int set = sets == 2 ? (bi & 1) : 0;
 		cudaStream_t st = set ? s->stream2 : s->stream;
 		const WaveBuffers &wb = set ? s->wb2 : s->wb;
@@ -1128,8 +1148,10 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 		/* bounces == 0: pathTrace's loop never runs and every sample is black (pathtrace.c:34-36,59).  L is write-once by
 		 * design (cr_add_radiance / cr_finish_path), so with no bounce nothing would write it: clear it here instead */
 		if (maxDepth == 0) CU(cudaMemsetAsync(wb.L, 0, (size_t)tile_pixels * (size_t)td.pass_count * sizeof(float4), st));
+		if (arm && maxDepth == 0) { crg_launch_stop_gate(wb.counts, 0, s->stop_ctl, set, s->stop_host, arm->first, arm->first, st); ++launches; }
 		int cur = 0;
 		for (int depth = 0; depth < maxDepth; ++depth) {
+			if (arm) { crg_launch_stop_gate(wb.counts, cur, s->stop_ctl, set, s->stop_host, arm->first && depth == 0, arm->first, st); ++launches; }
 			if (depth >= CRG_TAIL_FROM && !count) { crg_launch_tail(s->dev_copy, wb, cur, depth, maxDepth, s->xnodes, st); ++launches; }
 			if (timing) mark(tev, st);
 			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, knobs, st);
@@ -1153,8 +1175,12 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 			cur ^= 1;
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
-		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st); ++launches;
-		if (sets == 2) CU(cudaEventRecord(s->evAcc[set], st));
+		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, arm ? s->stop_ctl : nullptr, set); ++launches;
+		if (arm && arm->last) {
+			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, arm->call_pixels * (uint64_t)td.pass_count, wb.stats, st);
+			++launches;
+		}
+		if (sets == 2) CU(cudaEventRecord(s->evAcc[set], st));      /* after the publish step: the next K5 reads what it wrote */
 	}
 	if (sets == 2 && bi > 0) {      /* join: everything queued later on the scene's stream comes after both */
 		CU(cudaStreamWaitEvent(s->stream, s->evAcc[(bi - 1) & 1], 0));
@@ -1163,7 +1189,7 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	cudaStream_t st = s->stream;
 	if (timing) CU(cudaEventRecord(s->ev[1], st));
 	CU(cudaGetLastError());
-	s->pend_paths += tile_pixels * (uint64_t)pass_count;
+	if (!arm) s->pend_paths += tile_pixels * (uint64_t)pass_count;   /* an armed call counts what its publish steps committed */
 	s->pend_launches += launches;
 	if (timing) {
 		CU(cudaStreamSynchronize(st));
@@ -1194,6 +1220,100 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	}
 	if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
 	return crgpu_get_stats(s, stats);
+}
+
+/* An armed call.  Every batch commits in pass order or not at all (StopArm, k_accumulate<true>, k_stop_publish), so after the call
+ * the framebuffer holds exactly passes [0, committed) and a later call for [committed, end) finishes it bit for bit.  A pixel set
+ * larger than the paths in flight is walked pass-major: each batch of passes covers every piece before the next batch starts, so
+ * one pass count describes the whole set.  A stop is then taken only at the first piece of a pass batch (the later pieces must
+ * complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set. */
+static int render_armed(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats) {
+	const unsigned inner = flags | CRGPU_FLAG_ASYNC;
+	__atomic_store_n(&s->stop_host[1], (unsigned)pass_begin, __ATOMIC_RELEASE);
+	__atomic_store_n(&s->stop_host[2], 1u, __ATOMIC_RELEASE);
+	crg_launch_stop_begin(s->stop_ctl, s->stop_host, pass_begin, s->stream);
+	uint64_t launches = 2;
+	int rc = CRGPU_OK;
+	if (pass_count == 0 || tile_pixels == 0) {
+		/* nothing to render: the begin and end steps publish pass_begin */
+	} else if (tile_pixels <= s->max_paths) {
+		const StopArm a = { true, true, true, tile_pixels };
+		rc = render_pixels(s, base, tile_pixels, pass_begin, pass_count, inner, nullptr, &a);
+	} else {
+		std::vector<TileDesc> parts;
+		std::vector<uint64_t> counts;
+		if (base.pixels) {
+			for (uint64_t p0 = 0; p0 < tile_pixels; p0 += s->max_paths) {
+				TileDesc part = base;
+				part.pixels = base.pixels + p0;
+				parts.push_back(part);
+				counts.push_back(tile_pixels - p0 < s->max_paths ? tile_pixels - p0 : s->max_paths);
+			}
+		} else {
+			const uint64_t rows = s->max_paths / (uint64_t)base.tw;
+			if (rows < 1) rc = fail(CRGPU_ERR_BAD_ARGUMENT, "tile is %d pixels wide > max paths in flight %llu", base.tw, (unsigned long long)s->max_paths);
+			for (int y = 0; rc == CRGPU_OK && y < base.th; y += (int)rows) {
+				TileDesc part = base;
+				part.y0 = base.y0 + y;
+				part.th = base.th - y < (int)rows ? base.th - y : (int)rows;
+				parts.push_back(part);
+				counts.push_back((uint64_t)part.tw * (uint64_t)part.th);
+			}
+		}
+		uint64_t widest = 1;
+		for (uint64_t c : counts) widest = c > widest ? c : widest;
+		const int passes = (int)(s->max_paths / widest < 1 ? 1 : s->max_paths / widest);   /* one batch per piece */
+		for (int pb = pass_begin; rc == CRGPU_OK && pb < pass_begin + pass_count; pb += passes) {
+			if (stop_requested(s)) break;
+			const int n = pass_begin + pass_count - pb < passes ? pass_begin + pass_count - pb : passes;
+			for (size_t k = 0; rc == CRGPU_OK && k < parts.size(); ++k) {
+				const StopArm a = { k == 0, k + 1 == parts.size(), false, tile_pixels };
+				rc = render_pixels(s, parts[k], counts[k], pb, n, inner, nullptr, &a);
+			}
+		}
+	}
+	crg_launch_stop_end(s->stop_ctl, s->stop_host, s->stream);   /* also after a failed enqueue: the in-flight word must clear */
+	s->pend_launches += launches;
+	if (rc) return rc;
+	CU(cudaGetLastError());
+	if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
+	rc = crgpu_get_stats(s, stats);
+	if (rc) return rc;
+	return __atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE) < (unsigned)(pass_begin + pass_count) ? CRGPU_STOPPED : CRGPU_OK;
+}
+
+extern "C" int crgpu_stop_enable(crgpu_scene *s, int on) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	CU(cudaSetDevice(s->device));
+	CU(cudaStreamSynchronize(s->stream));                         /* no call of the other mode may still be in flight */
+	if (s->stream2) CU(cudaStreamSynchronize(s->stream2));   /* NULL would be the legacy default stream */
+	if (on && !s->stop_host) {
+		void *p = nullptr;
+		CU(cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable));   /* unified addressing: the same pointer on the device */
+		s->stop_host = static_cast<unsigned *>(p);
+	}
+	if (on) for (int k = 0; k < 16; ++k) __atomic_store_n(&s->stop_host[k], 0u, __ATOMIC_RELEASE);
+	s->armed = on != 0;
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_request_stop(crgpu_scene *s) {
+	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
+	__atomic_store_n(&s->stop_host[0], 1u, __ATOMIC_RELEASE);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_clear_stop(crgpu_scene *s) {
+	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
+	__atomic_store_n(&s->stop_host[0], 0u, __ATOMIC_RELEASE);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy) {
+	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
+	if (passes_done) *passes_done = (int)__atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE);
+	if (busy) *busy = (int)__atomic_load_n(&s->stop_host[2], __ATOMIC_ACQUIRE);
+	return CRGPU_OK;
 }
 
 extern "C" int crgpu_render_tile(crgpu_scene *s, int x0, int y0, int x1, int y1, int pass_begin, int pass_count,
@@ -1267,7 +1387,7 @@ extern "C" int crgpu_get_stats(crgpu_scene *s, struct crgpu_stats *stats) {
 	}
 	if (stats) {
 		memset(stats, 0, sizeof *stats);
-		stats->paths = s->pend_paths;
+		stats->paths = s->pend_paths + (h[5] - s->fetched[5]);   /* + the passes armed calls committed */
 		stats->rays = h[0] - s->fetched[0]; stats->node_pairs = h[1] - s->fetched[1]; stats->tri_tests = h[2] - s->fetched[2];
 		stats->sphere_tests = h[3] - s->fetched[3]; stats->inst_visits = h[4] - s->fetched[4];
 		stats->kernel_launches = s->pend_launches;

@@ -320,9 +320,13 @@ __global__ void __launch_bounds__(128) k_tail(const DevScene *__restrict__ scp, 
 	if (s_last && threadIdx.x == 0) { wb.counts[cur] = 0u; wb.counts[cur ^ 1] = 0u; wb.counts[3] = 0u; }
 }
 
-/* ---- K5 ------------------------------------------------------------------------------------------------------------------ */
+/* ---- K5 ------------------------------------------------------------------------------------------------------------------
+ * ARMED (a stoppable scene): the batch is added only if its gates did not abandon it and the running average has reached exactly
+ * its first pass — both written by earlier kernels in stream order, so every block takes the same decision. */
+template <bool ARMED>
 __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, const float4 *__restrict__ L, TileDesc td,
-													 int image_width, int image_height) {
+													 int image_width, int image_height, const unsigned *__restrict__ gate, int set) {
+	if (ARMED && (gate[1 + set] != 0u || gate[0] != (unsigned)td.pass_begin)) return;
 	const unsigned tile_pixels = td.npix;
 	for (unsigned px = blockIdx.x * blockDim.x + threadIdx.x; px < tile_pixels; px += gridDim.x * blockDim.x) {
 		int x, y;
@@ -499,8 +503,9 @@ __global__ void k_libm(int fn, const float *__restrict__ x, const float *__restr
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st) {
 	k_libm<<<256, 256, 0, st>>>(fn, x, y, out, n);
 }
-void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st) {
-	k_accumulate<<<grid, 256, 0, st>>>(fb, L, td, W, H);
+void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st, const unsigned *gate, int set) {
+	if (gate) k_accumulate<true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set);
+	else k_accumulate<false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0);
 }
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st) {
 	k_to_srgb8<<<grid, 256, 0, st>>>(fb, out, n);

@@ -189,6 +189,53 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st) {
 	k_generate<<<grid, 256, 0, st>>>(sc, wb, td);
 }
+
+/* ---- stop gates of an armed scene (crgpu_wave.cuh): one thread each ------------------------------------------------------------
+ * The host words are pinned, mapped memory: read and written at system scope, so a host store is seen by the next gate and
+ * a published pass count by the host without any synchronisation. */
+__device__ __forceinline__ unsigned crg_ld_sys(const unsigned *p) {
+	unsigned v;
+	asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+	return v;
+}
+__device__ __forceinline__ void crg_st_sys(unsigned *p, unsigned v) { asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+
+__global__ void k_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, const unsigned *host, int reset, int check) {
+	unsigned ab = reset ? 0u : ctl[1 + set];
+	if (!ab && check) ab = crg_ld_sys(host) != 0u ? 1u : 0u;
+	ctl[1 + set] = ab;
+	if (ab) { counts[cur] = 0u; counts[cur ^ 1] = 0u; counts[3] = 0u; }   /* exactly what k_tail's last block clears */
+}
+__global__ void k_stop_begin(unsigned *ctl, unsigned *host, int pass_begin) {
+	ctl[0] = (unsigned)pass_begin;
+	crg_st_sys(host + 1, (unsigned)pass_begin);
+	crg_st_sys(host + 2, 1u);
+	__threadfence_system();
+}
+__global__ void k_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
+                               unsigned long long *stats) {
+	if (ctl[1 + set] == 0u && ctl[0] == (unsigned)pass_begin) {       /* the decision K5 took */
+		ctl[0] = (unsigned)(pass_begin + pass_count);
+		stats[5] += paths;
+	}
+	crg_st_sys(host + 1, ctl[0]);
+	__threadfence_system();
+}
+__global__ void k_stop_end(const unsigned *ctl, unsigned *host) {
+	crg_st_sys(host + 1, ctl[0]);
+	__threadfence_system();
+	crg_st_sys(host + 2, 0u);
+	__threadfence_system();
+}
+void crg_launch_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, const unsigned *host, bool reset, bool check, cudaStream_t st) {
+	k_stop_gate<<<1, 1, 0, st>>>(counts, cur, ctl, set, host, reset ? 1 : 0, check ? 1 : 0);
+}
+void crg_launch_stop_begin(unsigned *ctl, unsigned *host, int pass_begin, cudaStream_t st) { k_stop_begin<<<1, 1, 0, st>>>(ctl, host, pass_begin); }
+void crg_launch_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
+                             unsigned long long *stats, cudaStream_t st) {
+	k_stop_publish<<<1, 1, 0, st>>>(ctl, set, host, pass_begin, pass_count, paths, stats);
+}
+void crg_launch_stop_end(unsigned *ctl, unsigned *host, cudaStream_t st) { k_stop_end<<<1, 1, 0, st>>>(ctl, host); }
 /* K2 is persistent: the grid is exactly the number of blocks the device can keep resident (the occupancy query below also
  * counts the staged nodes' dynamic shared memory, so CRGPU_TRACE_STAGE=1024 gets fewer blocks).  MINB (blocks per SM the compiler
  * must make room for: 2 -> <=128 registers, 3 -> <=80, 4 -> <=64) trades registers for latency-hiding warps.  K2 is bound by

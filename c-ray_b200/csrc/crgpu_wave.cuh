@@ -43,7 +43,8 @@ struct WaveBuffers {
 	unsigned *box;          /* [CRG_BOX_SLOTS][12]: bounds of the origins K3 wrote at depth min(d, CRG_BOX_SLOTS - 1), for the origin cell of
 	                           dir mode 4.  [0..5] = this batch (lo x,y,z as ~crg_ord(lo), hi x,y,z as crg_ord(hi); atomicMax, 0 = empty),
 	                           [6..11] = the previous batch of this wave set: K3 keys its rays with those, K4b moves [0..5] there */
-	unsigned long long *stats; /* [0] rays, [1] pairs, [2] tris, [3] spheres, [4] insts */
+	unsigned long long *stats; /* [0] rays, [1] pairs, [2] tris, [3] spheres, [4] insts, [5] paths committed by armed calls,
+	                              [7] traversal watchdog */
 };
 
 /* Half h of a ping-pong state array.  Indexing the kernel-parameter array (wb.stA[cur]) with a runtime value makes the compiler
@@ -110,6 +111,23 @@ int crg_shade_launches_per_bounce(const ShadeKnobs &kn);
 bool crg_shade_flat_order(const ShadeKnobs &kn);
 /* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
-void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st);
+/* gate: NULL, or the stop words of an armed scene (below): K5 then adds the batch only if wave set `set`'s batch was not abandoned
+ * and the committed pass index equals td.pass_begin */
+void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st,
+                           const unsigned *gate = nullptr, int set = 0);
+
+/* ---- stopping an armed scene at a pass boundary (crgpu_stop_enable) ----------------------------------------------------------------
+ * ctl (device memory): [0] the pass index the running average has reached in this call, [1 + set] wave set `set`'s batch was
+ * abandoned.  host (pinned, mapped): [0] stop request, [1] committed pass index (published), [2] a call is in flight.
+ * The gate runs after K1 and before every bounce; if the stop is requested (and `check`) it abandons the batch and leaves the wave
+ * set as k_tail leaves it, so the rest of the batch's kernels run on zero rays.  `reset`: the first gate of a batch.  No kernel
+ * waits for the host: pausing is the host's business. */
+void crg_launch_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, const unsigned *host, bool reset, bool check, cudaStream_t st);
+void crg_launch_stop_begin(unsigned *ctl, unsigned *host, int pass_begin, cudaStream_t st);
+/* after K5: advance ctl[0] past the batch if K5 added it (and count its paths in stats[5]), then publish ctl[0] */
+void crg_launch_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
+                             unsigned long long *stats, cudaStream_t st);
+/* the call's last kernel: publish ctl[0] and clear the in-flight word */
+void crg_launch_stop_end(unsigned *ctl, unsigned *host, cudaStream_t st);
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st);
 void crg_launch_kat(const DevScene *dsc, const int32_t *xyp, int count, void *out, cudaStream_t st);

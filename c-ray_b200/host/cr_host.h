@@ -51,7 +51,7 @@ struct renderer;
 struct renderThreadState {         /* renderer.h:14-31 */
 	int thread_num;                /* = CUDA device ordinal of this worker */
 	bool threadComplete;
-	bool paused;                   /* set by the host (reference: the 'p' key, ui.c): the worker stops taking tiles until cleared */
+	bool paused;                   /* set by the host (reference: the 'p' key, ui.c): the worker stops at a pass boundary until cleared */
 	int currentTileNum;
 	int completedSamples;
 	uint64_t totalSamples;
@@ -60,6 +60,7 @@ struct renderThreadState {         /* renderer.h:14-31 */
 	crgpu_scene *gpu;              /* this worker's device-resident scene replica */
 	uint64_t rays;                 /* closest-hit queries traced by this worker */
 	int error;                     /* first CRGPU_ERR_* seen, 0 = none */
+	int tiles;                     /* tiles of this worker's share (the denominator of its progress) */
 };
 
 struct prefs {                     /* renderer.h:58-87 */
@@ -81,8 +82,12 @@ struct state {                     /* renderer.h:34-55 */
 	float *renderBuffer;           /* fp32 W*H*3, row H-1-y (scene.c:200, texture.c:24-28) */
 	int activeThreads;
 	bool isRendering, renderAborted;
+	bool saveImage;                /* ui.c: false when the frame was aborted without saving (renderFrame then returns no image) */
+	bool paused;                   /* crhostSetPaused: every worker pauses, as with its own renderThreadState::paused */
 	pthread_t *threads;
 	struct renderThreadState *threadStates;
+	int threadStateCount;          /* entries of threadStates: kept across frames (and swapped under doneMutex) so that
+	                                  crhostProgress may read them from any thread */
 	pthread_mutex_t tileMutex;
 	pthread_mutex_t doneMutex;     /* workers signal doneCond when they finish: renderFrame wakes up at once instead of at its next 16 ms poll */
 	pthread_cond_t doneCond;
@@ -147,6 +152,16 @@ void crhostSetRank(struct renderer *r, int rank, int world);
 void crhostResetQueue(struct renderer *r);
 int takeRankTiles(struct renderer *r, int *rects, int *nums);
 void crhostTileOwners(struct renderer *r, int world, int *owners);   /* owner rank of every tile, in queue order */
+/* Controls of a frame in flight, for hosts without the reference's UI (ui.c: Ctrl-C / 'X' abort without saving, 'S' aborts and
+ * saves, 'P' pauses).  Workers stop at a pass boundary after the bounce in flight and the drain of the batches already queued
+ * (crgpu_request_stop; measured latencies in DESIGN §4); after an abort with save,
+ * renderFrame returns the committed passes of every worker, after one without it returns no image.
+ *   crhostProgress  1 while a frame renders, else 0; *passes_done_total = tile-passes committed by all workers so far
+ *   crhostWorkerPasses  the passes worker t has committed (its tiles hold exactly passes [0, that)) */
+void crhostAbort(struct renderer *r, int save);
+void crhostSetPaused(struct renderer *r, int on);
+int crhostProgress(const struct renderer *r, unsigned long long *passes_done_total);
+int crhostWorkerPasses(const struct renderer *r, int t);
 
 /* worker entry point with the signature of renderThread (void *(*)(void *)) */
 void *gpuRenderThread(void *arg);

@@ -244,7 +244,7 @@ void *gpuRenderThread(void *arg) {
 		r->state.renderAborted = true;
 	}
 	while (!ts->error && r->state.isRendering && !r->state.renderAborted) {
-		while (ts->paused && !r->state.renderAborted) sleep_ms(100);       /* renderer.c:310-312 */
+		while ((ts->paused || r->state.paused) && !r->state.renderAborted) sleep_ms(16);   /* renderer.c:310-312 */
 		int got = 0;
 		if (ranked) {
 			got = takeRankTiles(r, rects, nums);
@@ -268,23 +268,47 @@ void *gpuRenderThread(void *arg) {
 		}
 		if (got == 0) break;
 		ts->currentTileNum = nums[0];
+		ts->tiles = got;
+		/* The share is ONE armed, asynchronous call.  Like renderThread's loop (renderer.c:271-320), this thread polls about every
+		 * 16 ms: it publishes the committed passes, forwards renderAborted and the pause flags as a stop (the call ends at the next
+		 * pass boundary), waits while paused, and resumes from the committed pass: the frame is the same bit for bit. */
+		const int spp = r->prefs.sampleCount;
 		const double t0 = now_s();
-		struct crgpu_stats st;
-		const int rc = crgpu_render_tiles(ts->gpu, rects, got, 0, r->prefs.sampleCount, 0u, &st);
+		int rc = crgpu_stop_enable(ts->gpu, 1);
+		int begin = 0;
+		while (rc == CRGPU_OK && begin < spp) {
+			rc = crgpu_render_tiles(ts->gpu, rects, got, begin, spp - begin, CRGPU_FLAG_ASYNC, NULL);
+			if (rc != CRGPU_OK) break;
+			int done = begin, busy = 1;
+			bool stopping = false;
+			for (;;) {
+				crgpu_progress(ts->gpu, &done, &busy);
+				ts->completedSamples = done;
+				ts->totalSamples = (uint64_t)done * (uint64_t)got;                    /* tile-passes done, renderer.c:307 */
+				if (done > 0) ts->avgSampleTime = (long)(1e6 * (now_s() - t0) / ((double)done * got));
+				if (!busy) break;
+				if (!stopping && (r->state.renderAborted || ts->paused || r->state.paused)) { crgpu_request_stop(ts->gpu); stopping = true; }
+				sleep_ms(1);      /* a poll is three loads of pinned memory; a 16 ms period would add 8 ms to the frame on average */
+			}
+			struct crgpu_stats st;
+			rc = crgpu_get_stats(ts->gpu, &st);
+			if (rc != CRGPU_OK) break;
+			ts->rays += st.rays;
+			begin = done;
+			if (begin >= spp) break;
+			while ((ts->paused || r->state.paused) && !r->state.renderAborted) sleep_ms(16);   /* renderer.c:310-312 */
+			if (r->state.renderAborted) break;
+			rc = crgpu_clear_stop(ts->gpu);
+		}
 		if (rc != CRGPU_OK) {
 			fprintf(stderr, "gpuRenderThread[%d]: %s\n", ts->thread_num, crgpu_last_error());
 			ts->error = rc;
 			r->state.renderAborted = true;
 			break;
 		}
-		ts->rays += st.rays;
-		ts->totalSamples += (uint64_t)r->prefs.sampleCount * (uint64_t)got;      /* tile-passes done, renderer.c:307 */
-		ts->completedSamples = r->prefs.sampleCount;
-		ts->avgSampleTime = (long)(1e6 * (now_s() - t0) / ((double)r->prefs.sampleCount * got));
 		for (int i = 0; i < got; ++i) {
 			r->state.renderTiles[nums[i]].isRendering = false;                    /* renderer.c:315-316 */
-			r->state.renderTiles[nums[i]].renderComplete = true;
-			if (!ranked) r->state.tileOwner[nums[i]] = ts->thread_num;
+			r->state.renderTiles[nums[i]].renderComplete = begin >= spp;
 		}
 		ts->currentTileNum = -1;
 		break;                                                                    /* the worker's whole share was one trip */
@@ -320,12 +344,25 @@ struct texture8 *renderFrame(struct renderer *r) {
 	struct texture8 *output = calloc(1, sizeof *output);          /* renderer.c:41 */
 	output->width = W; output->height = H;
 	output->data = calloc((size_t)W * H * 3, 1);
-	free(r->state.threads); free(r->state.threadStates);
+	if (r->state.threadStateCount != n) {
+		/* a host thread may be reading the worker states (crhostProgress): swap the array under doneMutex, and only when its size
+		 * changes; between frames of the same size the entries are re-initialised in place */
+		struct renderThreadState *states = calloc((size_t)n, sizeof *states);
+		pthread_mutex_lock(&r->state.doneMutex);
+		free(r->state.threadStates);
+		r->state.threadStates = states;
+		r->state.threadStateCount = n;
+		pthread_mutex_unlock(&r->state.doneMutex);
+	}
+	free(r->state.threads);
 	r->state.threads = calloc((size_t)n, sizeof *r->state.threads);
-	r->state.threadStates = calloc((size_t)n, sizeof *r->state.threadStates);
+	/* every tile's owner (worker or rank) is fixed by the spatial interleave before any worker starts, so that the gather sees the
+	 * same table on every rank even when a rank is aborted before it has taken its tiles */
+	for (int i = 0; i < r->state.tileCount; ++i) r->state.tileOwner[i] = tile_rank(r, &r->state.renderTiles[i], ranked ? r->world : n);
 	bool *started = calloc((size_t)n, sizeof *started);
-	r->state.isRendering = true;
+	r->state.saveImage = true;                                    /* ui.c */
 	r->state.renderAborted = false;
+	r->state.isRendering = true;
 	r->state.finishedTileCount = 0;
 	r->state.activeThreads = 0;
 	for (int i = 0; i < r->state.tileCount; ++i) { r->state.renderTiles[i].renderComplete = false; r->state.renderTiles[i].isRendering = false; }
@@ -357,15 +394,17 @@ struct texture8 *renderFrame(struct renderer *r) {
 		}
 		if (!r->prefs.quiet && ++pauser >= 280 / 16) {            /* the progress line, ~4x/s (renderer.c:137-158) */
 			pauser = 0;
-			uint64_t done = 0;
-			for (int t = 0; t < n; ++t) done += r->state.threadStates[t].totalSamples;
-			const uint64_t all = (uint64_t)r->state.tileCount * (uint64_t)r->prefs.sampleCount;
+			uint64_t done = 0, mine = 0;
+			for (int t = 0; t < n; ++t) { done += r->state.threadStates[t].totalSamples; mine += (uint64_t)r->state.threadStates[t].tiles; }
+			/* this process' share of the tile-passes: the whole frame in-process, this rank's tiles in a ranked job */
+			const uint64_t all = (mine ? mine : (uint64_t)r->state.tileCount) * (uint64_t)r->prefs.sampleCount;
 			const double el = now_s() - t0;
 			const double usPerPath = done ? 1e6 * el / ((double)done * r->prefs.tileWidth * r->prefs.tileHeight) : 0.0;
 			char rem[64];
 			smart_time(done ? el * (double)(all - done) / (double)done : 0.0, rem, sizeof rem);
-			printf("[%.0f%%] us/path: %.04f, etf: %s, %.02lfMs/s %s        \r", 100.0 * (double)r->state.finishedTileCount / (double)(r->state.tileCount ? r->state.tileCount : 1),
-				   usPerPath, done ? rem : "?", usPerPath > 0.0 ? 1.0 / usPerPath : 0.0, r->state.threadStates[0].paused ? "[PAUSED]" : "");
+			printf("[%.0f%%] us/path: %.04f, etf: %s, %.02lfMs/s %s        \r", 100.0 * (double)done / (double)(all ? all : 1),
+				   usPerPath, done ? rem : "?", usPerPath > 0.0 ? 1.0 / usPerPath : 0.0,
+				   r->state.threadStates[0].paused || r->state.paused ? "[PAUSED]" : "");
 			fflush(stdout);
 		}
 		int done = 0;
@@ -379,8 +418,10 @@ struct texture8 *renderFrame(struct renderer *r) {
 	r->state.totalRays = 0;
 	for (int t = 0; t < n; ++t) { err |= r->state.threadStates[t].error; r->state.totalRays += r->state.threadStates[t].rays; }
 	crgpu_scene *root_scene = r->state.threadStates[0].gpu;
+	const bool discard = !err && r->state.renderAborted && !r->state.saveImage;   /* aborted without saving (ui.c) */
 
-	if (!err && (n > 1 || ranked)) {
+	/* a rank takes part in the gather even when it discards its frame: every rank of the group must enter the collective */
+	if (!err && (ranked || (n > 1 && !discard))) {
 		/* every tile's owner is known (state.tileOwner): gather the float tiles on device 0 / rank 0 */
 		int *rects = malloc(sizeof(int) * 4 * (size_t)r->state.tileCount);
 		for (int i = 0; i < r->state.tileCount; ++i) {
@@ -397,19 +438,46 @@ struct texture8 *renderFrame(struct renderer *r) {
 		}
 		free(rects);
 	}
-	if (!err && (!ranked || r->rank == 0)) {
+	if (!err && !discard && (!ranked || r->rank == 0)) {
 		if (crgpu_framebuffer_read(root_scene, r->state.renderBuffer, 0, 0, 0, 0) != CRGPU_OK) err = CRGPU_ERR_CUDA;   /* renderBuffer, scene.c:200 */
 		if (!err && crgpu_framebuffer_to_srgb8(root_scene, output->data) != CRGPU_OK) err = CRGPU_ERR_CUDA;            /* renderer.c:297-300 */
 	}
 	r->state.renderSeconds = now_s() - t0;
 	for (int t = 0; t < n; ++t) if (r->state.threadStates[t].gpu) { crgpu_scene_destroy(r->state.threadStates[t].gpu); r->state.threadStates[t].gpu = NULL; }
-	if (!r->prefs.quiet && !err) {
+	if (!r->prefs.quiet && !err && !discard) {
 		const double samples = (double)W * H * r->prefs.sampleCount;
 		printf("\nFinished render in %.3f s: %.2f Msample/s, %.2f Mray/s (%llu rays)\n", r->state.renderSeconds,
 			   samples / r->state.renderSeconds / 1e6, (double)r->state.totalRays / r->state.renderSeconds / 1e6, (unsigned long long)r->state.totalRays);
 	}
-	if (err) { destroyTexture8(output); return NULL; }
+	if (discard && !r->prefs.quiet) printf("\nAborted: image not saved\n");
+	if (err || discard) { destroyTexture8(output); return NULL; }
 	return output;
+}
+
+void crhostAbort(struct renderer *r, int save) {
+	if (!r) return;
+	r->state.saveImage = save != 0;
+	r->state.renderAborted = true;
+}
+void crhostSetPaused(struct renderer *r, int on) { if (r) r->state.paused = on != 0; }
+/* the worker states are read under doneMutex: renderFrame swaps the array under it when the worker count changes */
+int crhostProgress(const struct renderer *r, unsigned long long *passes_done_total) {
+	if (!r) return 0;
+	unsigned long long done = 0;
+	pthread_mutex_t *m = (pthread_mutex_t *)&r->state.doneMutex;
+	pthread_mutex_lock(m);
+	for (int t = 0; t < r->state.threadStateCount; ++t) done += r->state.threadStates[t].totalSamples;
+	pthread_mutex_unlock(m);
+	if (passes_done_total) *passes_done_total = done;
+	return r->state.isRendering ? 1 : 0;
+}
+int crhostWorkerPasses(const struct renderer *r, int t) {
+	if (!r) return 0;
+	pthread_mutex_t *m = (pthread_mutex_t *)&r->state.doneMutex;
+	pthread_mutex_lock(m);
+	const int passes = t >= 0 && t < r->state.threadStateCount ? r->state.threadStates[t].completedSamples : 0;
+	pthread_mutex_unlock(m);
+	return passes;
 }
 
 void destroyTexture8(struct texture8 *t) { if (t) { free(t->data); free(t); } }

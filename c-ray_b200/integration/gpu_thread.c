@@ -92,15 +92,34 @@ void *gpuRenderThread(void *arg) {
 		if (got == 0) break;
 		ts->currentTileNum = nums[0];
 		startTimer(&timer);
-		struct crgpu_stats st;
-		if (crgpu_render_tiles(gpu, rects, got, 0, r->prefs.sampleCount, 0u, &st) != CRGPU_OK) {
+		/* One armed, asynchronous call per trip, polled like renderThread checks its flags (renderer.c:271-320): renderAborted and
+		 * paused become a stop at a pass boundary (after the bounce in flight and the drain of the queued batches, DESIGN §4);
+		 * while paused the worker waits, then resumes from the committed pass, which leaves the tiles bit-identical to an
+		 * uninterrupted trip. */
+		const uint64_t samplesBefore = ts->totalSamples;
+		int begin = 0, rc = crgpu_stop_enable(gpu, 1);
+		while (rc == CRGPU_OK && begin < r->prefs.sampleCount) {
+			rc = crgpu_render_tiles(gpu, rects, got, begin, r->prefs.sampleCount - begin, CRGPU_FLAG_ASYNC, NULL);
+			int done = begin, busy = rc == CRGPU_OK, stopping = 0;
+			while (busy) {
+				crgpu_progress(gpu, &done, &busy);
+				/* what the stats loop of renderFrame reads (renderer.c:126-158) */
+				ts->completedSamples = done > 0 ? done : 1;
+				ts->totalSamples = samplesBefore + (uint64_t)done * (uint64_t)got;
+				if (done > 0) ts->avgSampleTime = getUs(timer) / ((long)done * got);
+				if (!stopping && (r->state.renderAborted || ts->paused)) { crgpu_request_stop(gpu); stopping = 1; }
+				if (busy) sleepMSec(1);
+			}
+			if (rc == CRGPU_OK) rc = crgpu_get_stats(gpu, NULL);
+			begin = done;
+			if (begin >= r->prefs.sampleCount || r->state.renderAborted) break;
+			while (ts->paused && !r->state.renderAborted) sleepMSec(16);                   /* renderer.c:310-312 */
+			if (rc == CRGPU_OK) rc = crgpu_clear_stop(gpu);
+		}
+		if (rc != CRGPU_OK) {
 			logr(warning, "GPU worker %i: %s\n", ts->thread_num, crgpu_last_error());
 			break;
 		}
-		/* what the stats loop of renderFrame reads (renderer.c:126-158) */
-		ts->totalSamples += (uint64_t)r->prefs.sampleCount * (uint64_t)got;
-		ts->completedSamples = r->prefs.sampleCount;
-		ts->avgSampleTime = getUs(timer) / ((long)r->prefs.sampleCount * got);
 		/* renderer.c:294-300: the float tile into state.renderBuffer, the sRGB tile into the 8-bit output */
 		crgpu_framebuffer_to_srgb8(gpu, fb8);
 		for (int i = 0; i < got; ++i) {
@@ -113,11 +132,11 @@ void *gpuRenderThread(void *arg) {
 				memcpy(image->data.byte_p + off, fb8 + off, n);
 			}
 			r->state.renderTiles[nums[i]].isRendering = false;                           /* renderer.c:315-316 */
-			r->state.renderTiles[nums[i]].renderComplete = true;
+			r->state.renderTiles[nums[i]].renderComplete = begin >= r->prefs.sampleCount;
 		}
-		while (ts->paused && !r->state.renderAborted) sleepMSec(100);                    /* renderer.c:310-312 */
 		ts->currentTileNum = -1;
 		ts->completedSamples = 1;
+		if (r->state.renderAborted) break;                                                 /* renderer.c:272 */
 	}
 	free(rects); free(nums); free(fb); free(fb8);
 	crgpu_scene_destroy(gpu);

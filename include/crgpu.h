@@ -39,6 +39,7 @@ extern "C" {
 #define CRGPU_ERR_BAD_ARGUMENT  -3
 #define CRGPU_ERR_UNSUPPORTED   -4   /* node graph deeper than the device interpreter supports, etc. */
 #define CRGPU_ERR_NOMEM         -5
+#define CRGPU_STOPPED            1   /* not an error: an armed render call ended at a pass boundary because a stop was requested */
 
 typedef struct crgpu_scene crgpu_scene;
 
@@ -115,6 +116,28 @@ int crgpu_render_tile(crgpu_scene *s, int x0, int y0, int x1, int y1,
  * rank of a multi-GPU job renders its share of the tile grid without paying the per-tile launch tails. */
 int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects,
 					   int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats);
+
+/* Stopping a render at a pass boundary: renderThread's renderAborted / paused contract (reference renderer.c:258-327).
+ * On an ARMED scene every render call checks a stop word in pinned host memory after K1 and before every bounce, and adds each
+ * batch of passes to the framebuffer only in pass order and only if no stop was seen during it.  So after any call the
+ * framebuffer holds exactly the passes [pass_begin, passes_done) on top of what was there, and a later call for
+ * [passes_done, end) finishes the frame bit for bit.  A stop is seen by the next gate, i.e. after the bounce in flight (a pixel set larger than the
+ * paths in flight: after the pass batch in flight over the whole set); the call then returns once the batches already queued have
+ * drained: each still runs K1 and its bounce launches, on zero rays.  DESIGN §4 has measured latencies (11-49 ms on an H100 at
+ * 1-10 s frames).
+ *   crgpu_stop_enable   arm (1) or disarm (0); waits for the scene's queued work; arming clears the stop and the progress.
+ *                       An unarmed scene renders exactly as before (no gate, no extra kernel).
+ *   crgpu_request_stop  one store to pinned memory: thread-safe and async-signal-safe.  It stays set until crgpu_clear_stop, so
+ *                       a call made while it is set commits nothing and leaves the framebuffer untouched.
+ *   crgpu_progress      no synchronisation: the committed pass index (absolute, starting at pass_begin) of the call in flight
+ *                       or of the last one, and whether a call is in flight.
+ * A synchronous armed call returns CRGPU_STOPPED when it ended before pass_begin + pass_count; an asynchronous one
+ * (CRGPU_FLAG_ASYNC) is read with crgpu_progress.  stats.paths counts the committed passes only.  request_stop, clear_stop and
+ * progress on an unarmed scene fail with CRGPU_ERR_BAD_ARGUMENT. */
+int crgpu_stop_enable(crgpu_scene *s, int on);
+int crgpu_request_stop(crgpu_scene *s);
+int crgpu_clear_stop(crgpu_scene *s);
+int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy);
 
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
