@@ -1,7 +1,7 @@
 /*
- * crgpu_nccl.cu — framebuffer tile gather over NCCL (include/crgpu_nccl.h).  Plumbing only: tiles are packed by one copy
- * kernel per sender, exchanged with grouped ncclSend/ncclRecv and unpacked by one copy kernel per peer on the root; no
- * arithmetic touches the pixels.
+ * crgpu_nccl.cu — framebuffer tile gather over NCCL (include/crgpu_nccl.h).  Plumbing only: tiles are packed by a copy
+ * kernel per sender, exchanged with grouped ncclSend/ncclRecv and unpacked by a copy kernel per peer on the root (one launch
+ * per 32,768 tiles); no arithmetic touches the pixels.
  */
 #include "../../include/crgpu_nccl.h"
 #include <cuda_runtime.h>
@@ -95,9 +95,13 @@ static int copy_tiles(Member &m, float *fb, float *packed, const int *rects, con
 		CCHECK(cudaStreamSynchronize(m.stream));                    /* t and o are pageable locals */
 		m.list_key[(size_t)who] = key;
 	}
-	dim3 grid(4, (unsigned)t.size());
-	k_tiles_copy<PACK><<<grid, 256, 0, m.stream>>>(fb, packed, m.tiles + slot, m.offs + slot, W, H);
-	CCHECK(cudaGetLastError());
+	/* gridDim.y <= 65535: an 8K frame in 8x8 tiles on two GPUs is 259,200 tiles per peer.  offs are offsets into the whole
+	 * packed buffer, so a chunk only moves its view of the two lists. */
+	for (size_t first = 0; first < t.size(); first += 32768u) {
+		const size_t cnt = t.size() - first < 32768u ? t.size() - first : 32768u;
+		k_tiles_copy<PACK><<<dim3(4, (unsigned)cnt), 256, 0, m.stream>>>(fb, packed, m.tiles + slot + first, m.offs + slot + first, W, H);
+		CCHECK(cudaGetLastError());
+	}
 	return CRGPU_OK;
 }
 

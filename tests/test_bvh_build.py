@@ -40,21 +40,26 @@ def same_tree(a_nodes, a_prims, b_nodes, b_prims):
 
 
 def check_tree(nodes, prims, n):
-    """structural invariants of any valid result: every primitive in exactly one leaf, children allocated as pairs, boxes nested"""
-    assert len(nodes) >= 1 and sorted(prims.tolist()) == list(range(n))
+    """structural invariants of any valid result: every primitive in exactly one leaf, children allocated as pairs, boxes nested
+    (vectorised: the trees of tests/test_gpu_scale.py have millions of nodes)"""
+    assert len(nodes) >= 1 and np.array_equal(np.sort(prims), np.arange(n))
     leaf = (nodes["count_leaf"] & crscene.LEAF_BIT) != 0
-    cnt = nodes["count_leaf"] & crscene.COUNT_MASK
+    cnt = (nodes["count_leaf"] & crscene.COUNT_MASK).astype(np.int64)
     assert len(nodes) == 2 * int(leaf.sum()) - 1
-    covered = np.zeros(n, dtype=np.int32)
-    for f, c in zip(nodes["first"][leaf], cnt[leaf]):
-        covered[f:f + c] += 1
-    assert (covered == 1).all()
-    for i in np.nonzero(~leaf)[0]:
-        for ch in (nodes["first"][i], nodes["first"][i] + 1):
-            assert ch > i and ch < len(nodes)
-            pb, cb = nodes["bounds"][i], nodes["bounds"][ch]
-            if not (nodes["count_leaf"][ch] & crscene.COUNT_MASK) == 0 or not leaf[ch]:      # empty leaves carry the empty box
-                assert (cb[0::2] >= pb[0::2]).all() and (cb[1::2] <= pb[1::2]).all()
+    full = leaf & (cnt > 0)
+    first, c = nodes["first"][full].astype(np.int64), cnt[full]
+    assert (first + c <= n).all()
+    edges = np.zeros(n + 1, dtype=np.int64)                 # +1 where a leaf's range starts, -1 after it ends
+    np.add.at(edges, first, 1)
+    np.add.at(edges, first + c, -1)
+    assert (np.cumsum(edges[:n]) == 1).all()
+    inner = np.nonzero(~leaf)[0]
+    for side in (0, 1):
+        ch = nodes["first"][inner].astype(np.int64) + side
+        assert ((ch > inner) & (ch < len(nodes))).all()
+        keep = ~(leaf[ch] & (cnt[ch] == 0))                 # empty leaves carry the empty box
+        pb, cb = nodes["bounds"][inner[keep]], nodes["bounds"][ch[keep]]
+        assert (cb[:, 0::2] >= pb[:, 0::2]).all() and (cb[:, 1::2] <= pb[:, 1::2]).all()
 
 
 def synthetic_cases():
