@@ -120,6 +120,8 @@ def lib():
         L.crgpu_request_stop.argtypes = [P]
         L.crgpu_clear_stop.argtypes = [P]
         L.crgpu_progress.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        L.crgpu_scene_set_camera.argtypes = [P, C.POINTER(Camera)]
+        L.crgpu_scene_set_instances.argtypes = [P, P, C.c_uint32]
         L.crscene_load.argtypes = [C.POINTER(FlatScene), C.c_char_p]
         L.crscene_free.argtypes = [C.POINTER(FlatScene)]
         L.crscene_set_config.argtypes = [C.POINTER(FlatScene)] + [C.c_int] * 4
@@ -129,7 +131,7 @@ def lib():
                   "crgpu_shade_rays", "crgpu_libm_eval", "crgpu_prepared_background",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
                   "crgpu_stop_enable", "crgpu_request_stop", "crgpu_clear_stop", "crgpu_progress",
-                  "crscene_set_config"):
+                  "crgpu_scene_set_camera", "crgpu_scene_set_instances", "crscene_set_config"):
             getattr(L, f).restype = C.c_int
         _lib = L
     return _lib
@@ -231,6 +233,17 @@ class GpuScene:
         done, busy = C.c_int(0), C.c_int(0)
         _check(lib().crgpu_progress(self.handle, C.byref(done), C.byref(busy)), "crgpu_progress")
         return done.value, bool(busy.value)
+
+    def set_camera(self, camera):
+        """Move the camera of the resident scene (crgpu_scene_set_camera): a Camera of the scene's image size, taken bit for bit."""
+        _check(lib().crgpu_scene_set_camera(self.handle, C.byref(camera)), "crgpu_scene_set_camera")
+
+    def set_instances(self, instances):
+        """Re-place every instance (crgpu_scene_set_instances): an array of struct crs_instance (crscene.INSTANCE) with the uploaded
+        count, kinds and objects; A and Ainv are taken bit for bit and the top-level BVH is rebuilt on the device."""
+        import crscene
+        arr = np.ascontiguousarray(instances, dtype=crscene.INSTANCE)
+        _check(lib().crgpu_scene_set_instances(self.handle, arr.ctypes.data, len(arr)), "crgpu_scene_set_instances")
 
     def set_stream(self, cuda_stream_ptr):
         """Enqueue on a caller-owned cudaStream_t (int pointer, e.g. torch.cuda.current_stream().cuda_stream)."""

@@ -65,6 +65,8 @@ def loader():
         L = C.CDLL(LOADER_PATH)
         L.crloader_load_json.argtypes = [C.POINTER(FlatScene), C.c_char_p]
         L.crloader_load_json.restype = C.c_int
+        L.crloader_load_json_buf.argtypes = [C.POINTER(FlatScene), C.c_char_p, C.c_char_p, C.c_void_p]
+        L.crloader_load_json_buf.restype = C.c_int
         L.crloader_last_error.restype = C.c_char_p
         _loader = L
     return _loader
@@ -80,6 +82,19 @@ def load_json(path):
     rc = loader().crloader_load_json(C.byref(s), os.fsencode(path))
     if rc != 0:
         raise RuntimeError(f"crloader_load_json({path}) failed ({rc}): {loader().crloader_last_error().decode()}")
+    return s
+
+
+def load_json_buf(text, asset_path=None):
+    """Parse c-ray JSON text already in memory into a FlatScene (crloader_load_json_buf); mesh and HDR names are resolved against
+    asset_path (a directory; None = the working directory)."""
+    if asset_path is not None:
+        asset_path = os.path.join(os.fsdecode(asset_path), "")
+    s = FlatScene()
+    rc = loader().crloader_load_json_buf(C.byref(s), text.encode() if isinstance(text, str) else text,
+                                         None if asset_path is None else os.fsencode(asset_path), None)
+    if rc != 0:
+        raise RuntimeError(f"crloader_load_json_buf failed ({rc}): {loader().crloader_last_error().decode()}")
     return s
 
 

@@ -6,6 +6,7 @@
 #include "../../include/crgpu.h"
 #include "crgpu_wave.cuh"
 #include "crgpu_scene.cuh"
+#include "crgpu_bvh_build.cuh"
 
 #define CRG_HITKAT_BYTES 160
 #define CRG_TAIL_FROM 6      /* first bounce at which the tail kernel may take over (it only does when <= 16384 rays are left) */
@@ -15,6 +16,7 @@
 #include <cstring>
 #include <cstdarg>
 #include <vector>
+#include <unordered_map>
 #include <queue>
 #include <thread>
 #include <mutex>
@@ -158,6 +160,10 @@ struct crgpu_prepared {
 	bool pinned;
 	size_t slab_bytes;
 	size_t off[SEC_COUNT], len[SEC_COUNT];
+	/* what crgpu_scene_set_instances needs beyond the slab: kind and object of every instance, and the root bounds of every BVH
+	 * as stored (6 floats each; the slab keeps only pair nodes, whose roots' own boxes are not in it) */
+	std::vector<uint32_t> inst_kind, inst_object;
+	std::vector<float> bvh_root;
 };
 
 struct crgpu_scene {
@@ -191,6 +197,13 @@ struct crgpu_scene {
 	bool armed;                /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
 	unsigned *stop_host;       /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight (NULL until armed once) */
 	unsigned *stop_ctl;        /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets */
+	/* instance edits (crgpu_scene_set_instances) */
+	std::vector<uint32_t> inst_kind, inst_object;    /* as uploaded: an edit must keep them */
+	std::vector<float> bvh_root;                     /* crgpu_prepared::bvh_root */
+	uint32_t pair_count;       /* pair nodes uploaded (the edit block starts with a copy of them) */
+	uint32_t top_stage_cap;    /* staged top-level pairs reserved at upload */
+	void *edit; size_t edit_bytes;             /* NULL until the first instance edit: uploaded pairs, the top region, top_prims */
+	void *edit_scratch; size_t edit_scratch_bytes;   /* instance inputs, boxes, the new top level and the builder's scratch */
 };
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
@@ -548,6 +561,8 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->fb, s->fb_floats * sizeof(float));
 	ctx_free(s->device, s->fb8, s->fb_floats);
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
+	ctx_free(s->device, s->edit, s->edit_bytes);
+	ctx_free(s->device, s->edit_scratch, s->edit_scratch_bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -781,6 +796,12 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 		} else { return pfail(p, fail(CRGPU_ERR_UNSUPPORTED, "instance kind %u (volumes are not reachable from the scene loader)", src.kind)); }
 		insts[i] = d;
 	}
+	p->inst_kind.resize(f->instance_count);
+	p->inst_object.resize(f->instance_count);
+	for (uint32_t i = 0; i < f->instance_count; ++i) { p->inst_kind[i] = f->instances[i].kind; p->inst_object[i] = f->instances[i].object; }
+	p->bvh_root.assign(6 * (size_t)f->bvh_count, 0.0f);
+	for (uint32_t b = 0; b < f->bvh_count; ++b)
+		if (f->bvhs[b].node_count) memcpy(&p->bvh_root[6 * (size_t)b], f->bvh_nodes[f->bvhs[b].node_offset].bounds, 6 * sizeof(float));
 
 	/* textures (data pointers are byte offsets into the texture section here; patched per device at upload) */
 	std::vector<DevTexture> texs(f->texture_count);
@@ -918,6 +939,9 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->wave_sets = 0; s->stream2 = nullptr; s->evAcc[0] = s->evAcc[1] = nullptr; s->evFork = nullptr;
 	s->pixels = nullptr; s->pixel_cap = 0;
 	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr;
+	s->inst_kind = p->inst_kind; s->inst_object = p->inst_object; s->bvh_root = p->bvh_root;
+	s->pair_count = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode)); s->top_stage_cap = p->top.stage_count;
+	s->edit = nullptr; s->edit_bytes = 0; s->edit_scratch = nullptr; s->edit_scratch_bytes = 0;
 	s->device = device; s->xnodes = p->xnodes; s->dev_copy = nullptr; s->fb = nullptr; s->fb8 = nullptr; s->stream = nullptr; s->own_stream = nullptr; s->cap_paths = 0;
 	s->slab = nullptr; s->slab_bytes = 0; s->small = nullptr; s->small_bytes = 0; s->wave = nullptr; s->wave_bytes = 0; s->fb_floats = 0;
 	memset(s->fetched, 0, sizeof s->fetched);
@@ -1282,11 +1306,18 @@ static int render_armed(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int
 	return __atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE) < (unsigned)(pass_begin + pass_count) ? CRGPU_STOPPED : CRGPU_OK;
 }
 
+/* wait for the work queued on the scene's streams */
+static int drain(crgpu_scene *s) {
+	CU(cudaSetDevice(s->device));
+	CU(cudaStreamSynchronize(s->stream));
+	if (s->stream2) CU(cudaStreamSynchronize(s->stream2));   /* NULL would be the legacy default stream */
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_stop_enable(crgpu_scene *s, int on) {
 	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
-	CU(cudaSetDevice(s->device));
-	CU(cudaStreamSynchronize(s->stream));                         /* no call of the other mode may still be in flight */
-	if (s->stream2) CU(cudaStreamSynchronize(s->stream2));   /* NULL would be the legacy default stream */
+	int rc = drain(s);                                            /* no call of the other mode may still be in flight */
+	if (rc) return rc;
 	if (on && !s->stop_host) {
 		void *p = nullptr;
 		CU(cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable));   /* unified addressing: the same pointer on the device */
@@ -1313,6 +1344,113 @@ extern "C" int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy) {
 	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
 	if (passes_done) *passes_done = (int)__atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE);
 	if (busy) *busy = (int)__atomic_load_n(&s->stop_host[2], __ATOMIC_ACQUIRE);
+	return CRGPU_OK;
+}
+
+/* ---- scene edits between renders ----------------------------------------------------------------------------------------------------
+ * K1 and K2 take the host descriptor s->dev by value; K3, the tail kernel and the KAT read its HBM copy s->dev_copy: both change. */
+extern "C" int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam) {
+	if (!s || !cam) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (cam->width != (int32_t)s->dev.image_width || cam->height != (int32_t)s->dev.image_height)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "camera is %dx%d, the scene renders %ux%u", cam->width, cam->height, s->dev.image_width, s->dev.image_height);
+	int rc = drain(s);
+	if (rc) return rc;
+	DevCamera &c = s->dev.cam;
+	c.sensor_x = cam->sensor_x; c.sensor_y = cam->sensor_y; c.aperture = cam->aperture; c.focal_distance = cam->focal_distance;
+	memcpy(c.forward, cam->forward, 12); memcpy(c.right, cam->right, 12); memcpy(c.up, cam->up, 12);
+	c.width = cam->width; c.height = cam->height;
+	memcpy(c.A, cam->A, sizeof c.A);
+	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+/* Instance boxes, ray offsets and the top-level BVH of the edited instances are computed on the device, into scratch; only once the
+ * build has passed the upload's checks are they copied over the scene's instances, top region, top_prims and staged prefix. */
+extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
+	if (!s || !inst) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	if (count != n) return fail(CRGPU_ERR_BAD_ARGUMENT, "%u instances given, the scene has %u", count, n);
+	for (uint32_t i = 0; i < n; ++i)
+		if (inst[i].kind != s->inst_kind[i] || inst[i].object != s->inst_object[i])
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "instance %u changes its kind or object", i);
+	int rc = drain(s);
+	if (rc) return rc;
+	if (n == 0) return CRGPU_OK;
+	const size_t top_cap = n > 1u ? n - 1u : 1u;
+	auto align = [](size_t b) { return (b + 255u) & ~(size_t)255u; };
+	const size_t pairs_bytes = (size_t)s->pair_count * sizeof(PairNode), top_bytes = top_cap * sizeof(PairNode);
+	/* scratch: the caller's instances, last instance of each object, BVH roots, boxes, centres, offsets, new instance records,
+	 * new top pairs and prims, then the builder's own scratch */
+	const size_t sz[10] = { (size_t)n * sizeof(crs_instance), (size_t)n * 4u, s->bvh_root.size() * sizeof(float), (size_t)n * 24u, (size_t)n * 12u,
+	                        (size_t)n * 4u, (size_t)n * sizeof(DevInstance), top_bytes, (size_t)n * 4u, crg_bvh_scratch_bytes(n) };
+	size_t so[10], total = 0;
+	for (int k = 0; k < 10; ++k) { so[k] = total; total += align(sz[k]); }
+	cudaStream_t st = s->stream;
+	if (!s->edit) {
+		/* the scene's own pairs block: the uploaded pairs (mesh pair offsets do not move), then a top region that holds any top level
+		 * of n instances, then top_prims; the uploaded top level keeps rendering until an edit is committed */
+		const size_t edit_bytes = align(pairs_bytes + top_bytes) + (size_t)n * 4u;
+		void *e = nullptr, *q = nullptr;
+		rc = ctx_alloc(s->device, edit_bytes, &e);
+		if (!rc) rc = ctx_alloc(s->device, total, &q);
+		std::vector<uint32_t> last(n);
+		std::unordered_map<uint64_t, uint32_t> last_of;                  /* (kind, object) -> its last instance */
+		for (uint32_t i = n; i-- > 0;) {
+			const uint64_t key = ((uint64_t)s->inst_kind[i] << 32) | s->inst_object[i];
+			last[i] = last_of.emplace(key, i).first->second;
+		}
+		cudaError_t ce = cudaSuccess;
+		if (!rc) ce = cudaMemcpyAsync(e, s->dev.pairs, pairs_bytes, cudaMemcpyDeviceToDevice, st);
+		if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + so[1], last.data(), sz[1], cudaMemcpyHostToDevice, st);
+		if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + so[2], s->bvh_root.data(), sz[2], cudaMemcpyHostToDevice, st);
+		if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+		if (!rc && ce != cudaSuccess) rc = fail(CRGPU_ERR_CUDA, "set_instances: %s", cudaGetErrorString(ce));
+		if (rc) { ctx_free(s->device, e, edit_bytes); ctx_free(s->device, q, total); return rc; }
+		s->edit = e; s->edit_bytes = edit_bytes;
+		s->edit_scratch = q; s->edit_scratch_bytes = total;
+	}
+	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
+	float *bb = reinterpret_cast<float *>(sc + so[3]), *ctr = reinterpret_cast<float *>(sc + so[4]), *offs = reinterpret_cast<float *>(sc + so[5]);
+	DevInstance *new_insts = reinterpret_cast<DevInstance *>(sc + so[6]);
+	PairNode *new_pairs = reinterpret_cast<PairNode *>(sc + so[7]);
+	int32_t *new_prims = reinterpret_cast<int32_t *>(sc + so[8]);
+	CU(cudaMemcpyAsync(sc + so[0], inst, sz[0], cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(new_insts, s->dev.instances, sz[6], cudaMemcpyDeviceToDevice, st));
+	crg_launch_instance_boxes(reinterpret_cast<const crs_instance *>(sc + so[0]), new_insts, reinterpret_cast<const float *>(sc + so[2]),
+	                          reinterpret_cast<const uint32_t *>(sc + so[1]), n, bb, ctr, offs, st);
+	CU(cudaGetLastError());
+	CrgTopResult res;
+	rc = crg_bvh_build_top(bb, ctr, n, sc + so[9], st, new_pairs, new_prims, &res);
+	if (rc) return rc;
+	if (res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "BVH deeper than 64 levels");
+
+	/* commit */
+	DevBvh t;
+	memset(&t, 0, sizeof t);
+	t.pair_offset = s->pair_count;
+	t.pair_end = s->pair_count + res.pairs;
+	t.node_count = res.node_count;
+	if (res.node_count == 1u) { memcpy(t.root_bounds, res.bounds, sizeof t.root_bounds); t.root_first = res.root_first; t.root_count = res.root_count; }
+	t.stage_base = s->dev.top.stage_base;
+	t.stage_count = res.pairs < s->top_stage_cap ? res.pairs : s->top_stage_cap;
+	PairNode *top_pairs = static_cast<PairNode *>(s->edit) + s->pair_count;          /* = pairs + t.pair_offset */
+	int32_t *top_prims = reinterpret_cast<int32_t *>(static_cast<uint8_t *>(s->edit) + align(pairs_bytes + top_bytes));
+	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), new_insts, sz[6], cudaMemcpyDeviceToDevice, st));
+	if (res.pairs) CU(cudaMemcpyAsync(top_pairs, new_pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	CU(cudaMemcpyAsync(top_prims, new_prims, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
+	if (t.stage_count)
+		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + t.stage_base, new_pairs, (size_t)t.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	s->dev.top = t;
+	s->dev.pairs = reinterpret_cast<const PairNode *>(s->edit);
+	s->dev.top_prims = top_prims;
+	for (int k = 0; k < 3; ++k) {            /* as crgpu_prepare: the root's bounds */
+		const float lo = res.bounds[2 * k], e = res.bounds[2 * k + 1] - lo;
+		s->dev.world_lo[k] = lo;
+		s->dev.world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
+	}
+	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
+	CU(cudaStreamSynchronize(st));
 	return CRGPU_OK;
 }
 

@@ -23,6 +23,7 @@
  */
 #include "../../include/crgpu.h"
 #include "../../include/crscene.h"
+#include "crgpu_bvh_build.cuh"
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -355,6 +356,82 @@ __global__ void k_scan_add(unsigned long long *out, const unsigned long long *__
 	if (i < n && blk > 0u) out[i] += sums_incl[blk - 1u];
 }
 
+/* ---- the pair layout of an edited scene's top level (crgpu_api.cu build_pairs, on the device) ----------------------------------------
+ * build_pairs numbers internal nodes in BFS order, children left before right.  Records are created level by level, but in atomic
+ * order within a level, so one block walks the levels in BFS order: per level, an exclusive block scan of the internal-child counts
+ * of the level's internal nodes (in their BFS order) places their internal children in the next level. */
+__global__ void __launch_bounds__(1024) k_top_bfs(const Rec *__restrict__ recs, uint32_t *order, uint32_t *bfs_of, uint32_t *info) {
+	__shared__ uint32_t s_warp[32];
+	const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+	if (threadIdx.x == 0) { order[0] = 0u; bfs_of[0] = 0u; }
+	__syncthreads();
+	uint32_t lo = 0u, hi = 1u, tail = 1u, levels = 0u;
+	while (lo < hi) {
+		++levels;
+		for (uint32_t base = lo; base < hi; base += blockDim.x) {
+			const uint32_t j = base + threadIdx.x;
+			int32_t L = -1;
+			bool il = false, ir = false;
+			if (j < hi) { L = recs[order[j]].left; il = recs[L].left >= 0; ir = recs[L + 1].left >= 0; }
+			const uint32_t c = (il ? 1u : 0u) + (ir ? 1u : 0u);
+			uint32_t incl = c;
+			for (unsigned d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += x; }
+			if (lane == 31u) s_warp[w] = incl;
+			__syncthreads();
+			uint32_t woff = 0u, total = 0u;
+			for (unsigned k = 0; k < nw; ++k) { if (k < w) woff += s_warp[k]; total += s_warp[k]; }
+			if (j < hi) {
+				uint32_t p = tail + woff + incl - c;
+				if (il) { order[p] = (uint32_t)L; bfs_of[L] = p; ++p; }
+				if (ir) { order[p] = (uint32_t)L + 1u; bfs_of[L + 1] = p; }
+			}
+			tail += total;
+			__syncthreads();                 /* s_warp is reused; the next level reads what this one wrote */
+		}
+		lo = hi; hi = tail;
+	}
+	if (threadIdx.x == 0) { info[0] = tail; info[1] = levels; }
+}
+__global__ void k_top_pairs(const Rec *__restrict__ recs, const uint32_t *__restrict__ order, const uint32_t *__restrict__ bfs_of, uint32_t count,
+							PairNode *pairs) {
+	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r >= count) return;
+	const Rec &R = recs[order[r]];
+	PairNode p;
+	for (int side = 0; side < 2; ++side) {
+		const int32_t ci = R.left + side;
+		const Rec &c = recs[ci];
+		float *b = side ? p.rb : p.lb;
+		for (int k = 0; k < 6; ++k) b[k] = c.b[k];
+		const uint32_t ref = c.left >= 0 ? bfs_of[ci] : c.begin, meta = c.left >= 0 ? 0u : CRG_LEAF_BIT | ((c.end - c.begin) & CRS_BVH_COUNT_MASK);
+		if (side) { p.rref = ref; p.rmeta = meta; } else { p.lref = ref; p.lmeta = meta; }
+	}
+	pairs[r] = p;
+}
+
+/* the scratch of one build of n primitives, carved from one block (base == nullptr: only the size) */
+struct Scratch {
+	int32_t *prims, *owner;
+	Rec *recs;
+	Bins *bins;
+	uint32_t *open[2], *tmpR, *cnt, *order, *bfs_of, *info;
+	unsigned long long *flags, *S1, *mis, *S2, *sums, *sums2, *keys;
+};
+size_t carve(void *base, uint32_t n, Scratch *s) {
+	const size_t max_open = n / 2u + 1u, max_rec = 2u * (size_t)n;
+	size_t off = 0;
+	auto take = [&](size_t bytes) { void *p = base ? static_cast<uint8_t *>(base) + off : nullptr; off += (bytes + 255u) & ~(size_t)255u; return p; };
+	s->prims = (int32_t *)take((size_t)n * 4u); s->owner = (int32_t *)take((size_t)n * 4u);
+	s->recs = (Rec *)take(max_rec * sizeof(Rec)); s->bins = (Bins *)take(max_open * sizeof(Bins));
+	s->open[0] = (uint32_t *)take(max_open * 4u); s->open[1] = (uint32_t *)take(max_open * 4u);
+	s->flags = (unsigned long long *)take((size_t)n * 8u); s->S1 = (unsigned long long *)take((size_t)n * 8u);
+	s->mis = (unsigned long long *)take((size_t)n * 8u); s->S2 = (unsigned long long *)take((size_t)n * 8u);
+	s->tmpR = (uint32_t *)take((size_t)n * 4u); s->sums = (unsigned long long *)take(8u * ((size_t)n / BVB_SCAN_BLOCK + 2u));
+	s->sums2 = (unsigned long long *)take(8u * 64u); s->keys = (unsigned long long *)take(6u * 8u); s->cnt = (uint32_t *)take(4u * 4u);
+	s->order = (uint32_t *)take((size_t)n * 4u); s->bfs_of = (uint32_t *)take(max_rec * 4u); s->info = (uint32_t *)take(4u * 4u);
+	return off;
+}
+
 struct DevBuf {
 	void *p = nullptr;
 	~DevBuf() { if (p) cudaFree(p); }
@@ -381,6 +458,90 @@ static int scan64(const unsigned long long *in, unsigned long long *out, unsigne
 	return 0;
 }
 
+/* The tree of n >= 1 primitives (device boxes and centres) into the scratch s, on st: records level by level in s.recs, primitive
+ * order in s.prims.  Synchronises st once per level (the open-node count sizes the next launches). */
+static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scratch &s, cudaStream_t st,
+					  std::vector<uint32_t> &level_first, std::vector<uint32_t> &level_count, uint32_t *nrec_out) {
+	const uint32_t max_open = n / 2u + 1u;
+	const unsigned long long init_keys[6] = { KMIN_EMPTY, KMIN_EMPTY, KMIN_EMPTY, KMAX_EMPTY, KMAX_EMPTY, KMAX_EMPTY };
+	CUB(cudaMemcpyAsync(s.keys, init_keys, sizeof init_keys, cudaMemcpyHostToDevice, st));
+	const uint32_t gn = (n + 255u) / 256u;
+	Rec *recs = s.recs;
+	uint32_t *counters = s.cnt;
+	k_iota<<<gn, 256, 0, st>>>(s.prims, s.owner, n, n >= 2u ? 0 : -1);
+	k_root_keys<<<gn, 256, 0, st>>>(bb, n, s.keys);
+	k_root_init<<<1, 1, 0, st>>>(bb, n, s.keys, recs, counters);
+	const uint32_t zero = 0u;
+	CUB(cudaMemcpyAsync(s.open[0], &zero, 4u, cudaMemcpyHostToDevice, st));          /* the root is open node 0 of level 0 */
+	level_first.assign(1, 0u);
+	level_count.assign(1, 1u);
+	uint32_t h[4] = { 1u, n >= 2u ? 1u : 0u, 0u, 0u };
+	int cur = 0;
+	while (h[1] > 0u) {
+		const uint32_t nopen = h[1], go = (nopen + 127u) / 128u;
+		if (nopen > max_open) return crg_fail(CRGPU_ERR_CUDA, "crgpu_bvh_build: %u open nodes for %u primitives", nopen, n);
+		uint32_t *open_list = s.open[cur], *next_list = s.open[cur ^ 1];
+		{
+			const size_t blocks = ((size_t)nopen * (sizeof(Bins) / 8u) + 255u) / 256u;          /* grid-stride loop inside */
+			k_bins_clear<<<(unsigned)(blocks > 65535u ? 65535u : blocks), 256, 0, st>>>(s.bins, nopen);
+		}
+		k_bin<<<gn, 256, 0, st>>>(bb, ctr, s.prims, s.owner, recs, s.bins, n);
+		k_split<<<go, 128, 0, st>>>(bb, s.prims, recs, open_list, nopen, s.bins);
+		k_flag<<<gn, 256, 0, st>>>(ctr, s.prims, s.owner, recs, s.flags, n);
+		scan64(s.flags, s.S1, s.sums, s.sums2, n, st);
+		k_mid<<<go, 128, 0, st>>>(recs, open_list, nopen, s.S1);
+		k_misplaced<<<gn, 256, 0, st>>>(s.owner, recs, s.flags, s.mis, n);
+		scan64(s.mis, s.S2, s.sums, s.sums2, n, st);
+		k_scatter_right<<<gn, 256, 0, st>>>(s.owner, recs, s.mis, s.S2, s.tmpR, n);
+		k_swap<<<gn, 256, 0, st>>>(s.owner, recs, s.mis, s.S2, s.tmpR, s.prims, n);
+		k_children<<<go, 128, 0, st>>>(recs, open_list, nopen, next_list, counters);
+		k_owner<<<gn, 256, 0, st>>>(s.owner, recs, n);
+		CUB(cudaMemcpyAsync(h, counters, sizeof h, cudaMemcpyDeviceToHost, st));
+		CUB(cudaStreamSynchronize(st));
+		const uint32_t prev_total = level_first.back() + level_count.back();
+		if (h[0] > prev_total) { level_first.push_back(prev_total); level_count.push_back(h[0] - prev_total); }
+		k_level_advance<<<1, 1, 0, st>>>(counters);
+		h[1] = h[2];
+		cur ^= 1;
+		if (level_first.size() > BVB_MAX_DEPTH + 2u) return crg_fail(CRGPU_ERR_CUDA, "crgpu_bvh_build: deeper than %u levels", BVB_MAX_DEPTH);
+	}
+	*nrec_out = h[0];
+	return CRGPU_OK;
+}
+
+size_t crg_bvh_scratch_bytes(uint32_t n) { Scratch s; return carve(nullptr, n, &s); }
+
+int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, void *scratch, cudaStream_t st, PairNode *pairs_out, int32_t *prims_out,
+					  CrgTopResult *out) {
+	memset(out, 0, sizeof *out);
+	if (n == 0u) return CRGPU_OK;
+	if (n > 4194304u) return crg_fail(CRGPU_ERR_UNSUPPORTED, "crgpu_bvh_build: %u primitives (limit 4194304 per call)", n);
+	Scratch s;
+	carve(scratch, n, &s);
+	std::vector<uint32_t> level_first, level_count;
+	uint32_t nrec = 0u;
+	int rc = build_tree(bb, ctr, n, s, st, level_first, level_count, &nrec);
+	if (rc) return rc;
+	uint32_t info[2] = { 0u, 0u };
+	if (nrec > 1u) {
+		k_top_bfs<<<1, 1024, 0, st>>>(s.recs, s.order, s.bfs_of, s.info);
+		const uint32_t internal = (nrec - 1u) / 2u;                   /* a full binary tree */
+		k_top_pairs<<<(internal + 255u) / 256u, 256, 0, st>>>(s.recs, s.order, s.bfs_of, internal, pairs_out);
+		CUB(cudaMemcpyAsync(info, s.info, sizeof info, cudaMemcpyDeviceToHost, st));
+	}
+	CUB(cudaMemcpyAsync(prims_out, s.prims, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
+	Rec root;
+	CUB(cudaMemcpyAsync(&root, s.recs, sizeof root, cudaMemcpyDeviceToHost, st));
+	CUB(cudaStreamSynchronize(st));
+	CUB(cudaGetLastError());
+	out->node_count = nrec;
+	out->pairs = info[0];
+	out->levels = info[1];
+	memcpy(out->bounds, root.b, sizeof out->bounds);
+	if (nrec == 1u) { out->root_first = root.begin; out->root_count = root.end - root.begin; }
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_bvh_build(const float *bboxes, const float *centers, uint32_t n, int device,
 								struct crs_bvh_node *nodes_out, uint32_t *node_count_out, int32_t *prims_out) {
 	if (!nodes_out || !node_count_out || !prims_out || (n && (!bboxes || !centers))) return crg_fail(CRGPU_ERR_BAD_ARGUMENT, "crgpu_bvh_build: NULL argument");
@@ -392,74 +553,82 @@ extern "C" int crgpu_bvh_build(const float *bboxes, const float *centers, uint32
 	if (rc) return rc;
 	if (device < 0 || device >= ndev) return crg_fail(CRGPU_ERR_BAD_ARGUMENT, "crgpu_bvh_build: device %d out of range (have %d)", device, ndev);
 	CUB(cudaSetDevice(device));
-	const uint32_t max_open = n / 2u + 1u, max_rec = 2u * n;
+	const uint32_t max_rec = 2u * n;
 	size_t free_b = 0, total_b = 0;
 	CUB(cudaMemGetInfo(&free_b, &total_b));
-	const size_t need = (size_t)max_open * sizeof(Bins) + (size_t)max_rec * sizeof(Rec) + (size_t)n * 96u;
-	if (need > free_b / 2u) return crg_fail(CRGPU_ERR_NOMEM, "crgpu_bvh_build: %zu bytes of scratch for %u primitives, %zu free", need, n, free_b);
-	DevBuf d_bb, d_ctr, d_prims, d_owner, d_recs, d_bins, d_open[2], d_flags, d_S1, d_mis, d_S2, d_tmpR, d_sums, d_sums2, d_keys, d_cnt, d_out;
-	CUB(d_bb.alloc((size_t)n * 24u)); CUB(d_ctr.alloc((size_t)n * 12u)); CUB(d_prims.alloc((size_t)n * 4u)); CUB(d_owner.alloc((size_t)n * 4u));
-	CUB(d_recs.alloc((size_t)max_rec * sizeof(Rec))); CUB(d_bins.alloc((size_t)max_open * sizeof(Bins)));
-	CUB(d_open[0].alloc((size_t)max_open * 4u)); CUB(d_open[1].alloc((size_t)max_open * 4u));
-	CUB(d_flags.alloc((size_t)n * 8u)); CUB(d_S1.alloc((size_t)n * 8u)); CUB(d_mis.alloc((size_t)n * 8u)); CUB(d_S2.alloc((size_t)n * 8u));
-	CUB(d_tmpR.alloc((size_t)n * 4u)); CUB(d_sums.alloc(8u * ((size_t)n / BVB_SCAN_BLOCK + 2u))); CUB(d_sums2.alloc(8u * 64u));
-	CUB(d_keys.alloc(6u * 8u)); CUB(d_cnt.alloc(4u * 4u)); CUB(d_out.alloc((size_t)max_rec * sizeof(crs_bvh_node)));
+	const size_t scratch_bytes = crg_bvh_scratch_bytes(n);
+	if (scratch_bytes > free_b / 2u) return crg_fail(CRGPU_ERR_NOMEM, "crgpu_bvh_build: %zu bytes of scratch for %u primitives, %zu free", scratch_bytes, n, free_b);
+	DevBuf d_bb, d_ctr, d_scratch, d_out;
+	CUB(d_bb.alloc((size_t)n * 24u)); CUB(d_ctr.alloc((size_t)n * 12u)); CUB(d_scratch.alloc(scratch_bytes));
+	CUB(d_out.alloc((size_t)max_rec * sizeof(crs_bvh_node)));
+	Scratch s;
+	carve(d_scratch.p, n, &s);
 	cudaStream_t st = nullptr;
 	CUB(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
 	struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{ st };
 	CUB(cudaMemcpyAsync(d_bb.p, bboxes, (size_t)n * 24u, cudaMemcpyHostToDevice, st));
 	CUB(cudaMemcpyAsync(d_ctr.p, centers, (size_t)n * 12u, cudaMemcpyHostToDevice, st));
-	const unsigned long long init_keys[6] = { KMIN_EMPTY, KMIN_EMPTY, KMIN_EMPTY, KMAX_EMPTY, KMAX_EMPTY, KMAX_EMPTY };
-	CUB(cudaMemcpyAsync(d_keys.p, init_keys, sizeof init_keys, cudaMemcpyHostToDevice, st));
-	const uint32_t gn = (n + 255u) / 256u;
-	Rec *recs = d_recs.as<Rec>();
-	uint32_t *counters = d_cnt.as<uint32_t>();
-	k_iota<<<gn, 256, 0, st>>>(d_prims.as<int32_t>(), d_owner.as<int32_t>(), n, n >= 2u ? 0 : -1);
-	k_root_keys<<<gn, 256, 0, st>>>(d_bb.as<float>(), n, d_keys.as<unsigned long long>());
-	k_root_init<<<1, 1, 0, st>>>(d_bb.as<float>(), n, d_keys.as<unsigned long long>(), recs, counters);
-	const uint32_t zero = 0u;
-	CUB(cudaMemcpyAsync(d_open[0].p, &zero, 4u, cudaMemcpyHostToDevice, st));          /* the root is open node 0 of level 0 */
-	std::vector<uint32_t> level_first{ 0u }, level_count{ 1u };
-	uint32_t h[4] = { 1u, n >= 2u ? 1u : 0u, 0u, 0u };
-	int cur = 0;
-	while (h[1] > 0u) {
-		const uint32_t nopen = h[1], go = (nopen + 127u) / 128u;
-		if (nopen > max_open) return crg_fail(CRGPU_ERR_CUDA, "crgpu_bvh_build: %u open nodes for %u primitives", nopen, n);
-		uint32_t *open_list = d_open[cur].as<uint32_t>(), *next_list = d_open[cur ^ 1].as<uint32_t>();
-		{
-			const size_t blocks = ((size_t)nopen * (sizeof(Bins) / 8u) + 255u) / 256u;          /* grid-stride loop inside */
-			k_bins_clear<<<(unsigned)(blocks > 65535u ? 65535u : blocks), 256, 0, st>>>(d_bins.as<Bins>(), nopen);
-		}
-		k_bin<<<gn, 256, 0, st>>>(d_bb.as<float>(), d_ctr.as<float>(), d_prims.as<int32_t>(), d_owner.as<int32_t>(), recs, d_bins.as<Bins>(), n);
-		k_split<<<go, 128, 0, st>>>(d_bb.as<float>(), d_prims.as<int32_t>(), recs, open_list, nopen, d_bins.as<Bins>());
-		k_flag<<<gn, 256, 0, st>>>(d_ctr.as<float>(), d_prims.as<int32_t>(), d_owner.as<int32_t>(), recs, d_flags.as<unsigned long long>(), n);
-		scan64(d_flags.as<unsigned long long>(), d_S1.as<unsigned long long>(), d_sums.as<unsigned long long>(), d_sums2.as<unsigned long long>(), n, st);
-		k_mid<<<go, 128, 0, st>>>(recs, open_list, nopen, d_S1.as<unsigned long long>());
-		k_misplaced<<<gn, 256, 0, st>>>(d_owner.as<int32_t>(), recs, d_flags.as<unsigned long long>(), d_mis.as<unsigned long long>(), n);
-		scan64(d_mis.as<unsigned long long>(), d_S2.as<unsigned long long>(), d_sums.as<unsigned long long>(), d_sums2.as<unsigned long long>(), n, st);
-		k_scatter_right<<<gn, 256, 0, st>>>(d_owner.as<int32_t>(), recs, d_mis.as<unsigned long long>(), d_S2.as<unsigned long long>(), d_tmpR.as<uint32_t>(), n);
-		k_swap<<<gn, 256, 0, st>>>(d_owner.as<int32_t>(), recs, d_mis.as<unsigned long long>(), d_S2.as<unsigned long long>(), d_tmpR.as<uint32_t>(), d_prims.as<int32_t>(), n);
-		k_children<<<go, 128, 0, st>>>(recs, open_list, nopen, next_list, counters);
-		k_owner<<<gn, 256, 0, st>>>(d_owner.as<int32_t>(), recs, n);
-		CUB(cudaMemcpyAsync(h, counters, sizeof h, cudaMemcpyDeviceToHost, st));
-		CUB(cudaStreamSynchronize(st));
-		const uint32_t prev_total = level_first.back() + level_count.back();
-		if (h[0] > prev_total) { level_first.push_back(prev_total); level_count.push_back(h[0] - prev_total); }
-		k_level_advance<<<1, 1, 0, st>>>(counters);
-		h[1] = h[2];
-		cur ^= 1;
-		if (level_first.size() > BVB_MAX_DEPTH + 2u) return crg_fail(CRGPU_ERR_CUDA, "crgpu_bvh_build: deeper than %u levels", BVB_MAX_DEPTH);
-	}
-	const uint32_t nrec = h[0];
+	std::vector<uint32_t> level_first, level_count;
+	uint32_t nrec = 0u;
+	rc = build_tree(d_bb.as<float>(), d_ctr.as<float>(), n, s, st, level_first, level_count, &nrec);
+	if (rc) return rc;
+	Rec *recs = s.recs;
 	for (size_t l = level_first.size(); l-- > 0;)
 		k_count_internals<<<(level_count[l] + 255u) / 256u, 256, 0, st>>>(recs, level_first[l], level_count[l]);
 	for (size_t l = 0; l < level_first.size(); ++l)
 		k_assign<<<(level_count[l] + 255u) / 256u, 256, 0, st>>>(recs, level_first[l], level_count[l]);
 	k_emit<<<(nrec + 255u) / 256u, 256, 0, st>>>(recs, nrec, d_out.as<crs_bvh_node>());
 	CUB(cudaMemcpyAsync(nodes_out, d_out.p, (size_t)nrec * sizeof(crs_bvh_node), cudaMemcpyDeviceToHost, st));
-	CUB(cudaMemcpyAsync(prims_out, d_prims.p, (size_t)n * 4u, cudaMemcpyDeviceToHost, st));
+	CUB(cudaMemcpyAsync(prims_out, s.prims, (size_t)n * 4u, cudaMemcpyDeviceToHost, st));
 	CUB(cudaStreamSynchronize(st));
 	CUB(cudaGetLastError());
 	*node_count_out = nrec;
 	return CRGPU_OK;
+}
+
+/* ---- the top level's inputs for edited instances: instance_bbox of host/loader/cr_sceneload.c ---------------------------------------
+ * A mesh starts from its BVH root's bounds as stored (getRootBoundingBox), a sphere from its +-radius box; both go through transformBBox
+ * (crl_transform_bbox: every composite the JSON loader builds takes that branch for spheres) and the centre is the box centre (mesh)
+ * or A * 0 (sphere).  Plain fp32 operations in the loader's order; -fmad=false keeps them unfused. */
+__global__ void k_instance_boxes(const crs_instance *__restrict__ inst, DevInstance *insts, const float *__restrict__ bvh_root, uint32_t n,
+								 float *bb, float *ctr, float *offs) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const crs_instance &s = inst[i];
+	DevInstance &d = insts[i];
+	for (int k = 0; k < 12; ++k) { d.A[k] = s.A[k]; d.Ainv[k] = s.Ainv[k]; }
+	const float *m = s.A;                                                     /* row-major 4x4: m[4 * row + col] */
+	float mn[3], mx[3];
+	if (d.kind == CRS_INST_MESH) {
+		const float *b = bvh_root + 6 * (size_t)d.bvh;
+		for (int k = 0; k < 3; ++k) { mn[k] = b[2 * k]; mx[k] = b[2 * k + 1]; }
+	} else {
+		for (int k = 0; k < 3; ++k) { mn[k] = -d.radius; mx[k] = d.radius; }
+	}
+	float c[3], h[3], lo[3], hi[3];
+	for (int k = 0; k < 3; ++k) { c[k] = (mn[k] + mx[k]) * 0.5f; h[k] = (mx[k] - mn[k]) * 0.5f; }
+	for (int r = 0; r < 3; ++r) {                                             /* crl_vector / crl_point with |A| in the 3x3 part */
+		const float a0 = fabsf(m[4 * r]), a1 = fabsf(m[4 * r + 1]), a2 = fabsf(m[4 * r + 2]);
+		const float hr = a0 * h[0] + a1 * h[1] + a2 * h[2];
+		const float cr = a0 * c[0] + a1 * c[1] + a2 * c[2] + m[4 * r + 3];
+		lo[r] = cr - hr; hi[r] = cr + hr;
+	}
+	float cen[3];
+	for (int r = 0; r < 3; ++r)
+		cen[r] = d.kind == CRS_INST_MESH ? (hi[r] + lo[r]) * 0.5f : m[4 * r] * 0.0f + m[4 * r + 1] * 0.0f + m[4 * r + 2] * 0.0f + m[4 * r + 3];
+	for (int k = 0; k < 3; ++k) { bb[6 * (size_t)i + k] = lo[k]; bb[6 * (size_t)i + 3 + k] = hi[k]; ctr[3 * (size_t)i + k] = cen[k]; }
+	const float ex = hi[0] - lo[0], ey = hi[1] - lo[1], ez = hi[2] - lo[2];
+	offs[i] = 0.0001f * sqrtf(ex * ex + ey * ey + ez * ez);                  /* bbox.h:44-46 */
+}
+/* the reference stores the offset in the object while it builds the top level, so the last instance of an object sets it for all */
+__global__ void k_instance_offsets(DevInstance *insts, const uint32_t *__restrict__ last, const float *__restrict__ offs, uint32_t n) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) insts[i].ray_offset = offs[last[i]];
+}
+
+void crg_launch_instance_boxes(const crs_instance *inst, DevInstance *insts, const float *bvh_root, const uint32_t *last, uint32_t n,
+							   float *bb, float *ctr, float *offs, cudaStream_t st) {
+	if (n == 0u) return;
+	k_instance_boxes<<<(n + 255u) / 256u, 256, 0, st>>>(inst, insts, bvh_root, n, bb, ctr, offs);
+	k_instance_offsets<<<(n + 255u) / 256u, 256, 0, st>>>(insts, last, offs, n);
 }

@@ -1,0 +1,34 @@
+/*
+ * crgpu_bvh_build.cuh — the device SAH builder (crgpu_bvh_build.cu) as the scene-edit path uses it: on the scene's stream, from
+ * device-resident inputs, into caller-owned scratch, with the top level laid out as crgpu_api.cu build_pairs lays out an uploaded one.
+ */
+#pragma once
+#include <cuda_runtime.h>
+#include "crgpu_scene.cuh"
+
+/* Declared weak: a program that links the upload path without the builder (tests/stub/create_harness.c, which hashes the slab)
+ * still links; libcrgpu.so always defines them. */
+#define CRG_WEAK __attribute__((weak))
+
+/* bytes of device scratch crg_bvh_build_top needs for n primitives (reusable for any later build of at most n) */
+CRG_WEAK size_t crg_bvh_scratch_bytes(uint32_t n);
+
+struct CrgTopResult {
+	uint32_t node_count;            /* reference nodeCount (bvh.c) */
+	uint32_t pairs;                 /* internal nodes = pair nodes written (0 when node_count <= 1) */
+	uint32_t levels;                /* BFS levels holding internal nodes (the deepest internal node is at depth levels - 1) */
+	uint32_t root_first, root_count;/* node_count == 1: the root leaf's range */
+	float    bounds[6];             /* root bounds as stored (minx,maxx,miny,maxy,minz,maxz) */
+};
+
+/* The tree crgpu_bvh_build builds over n primitives (bb: n x 6 min xyz max xyz, ctr: n x 3, both device), enqueued on st.  Writes
+ * the internal nodes as PairNodes in build_pairs' BFS order with local refs into pairs_out (room for max(1, n - 1)) and the
+ * primitive order into prims_out (n, device); returns when both are written (st is synchronised). */
+CRG_WEAK int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, void *scratch, cudaStream_t st, PairNode *pairs_out, int32_t *prims_out,
+					  CrgTopResult *out);
+
+/* instance_bbox of the scene loader (host/loader/cr_sceneload.c) for n edited instances: each DevInstance takes A / Ainv from inst,
+ * bb / ctr (device, n x 6 and n x 3) receive the top-level build's inputs and every instance the ray offset of the last instance of
+ * its object (last[i]).  bvh_root: 6 floats per BVH, the root bounds of each mesh BVH as stored. */
+CRG_WEAK void crg_launch_instance_boxes(const crs_instance *inst, DevInstance *insts, const float *bvh_root, const uint32_t *last, uint32_t n,
+							   float *bb, float *ctr, float *offs, cudaStream_t st);

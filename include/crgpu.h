@@ -139,6 +139,20 @@ int crgpu_request_stop(crgpu_scene *s);
 int crgpu_clear_stop(crgpu_scene *s);
 int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy);
 
+/* Editing a resident scene between renders (c-ray's crMoveCamera / crTransformMesh, src/c-ray.h:95-103): the edited scene renders
+ * the same bits as the scene loaded fresh from the edited JSON.  Both calls first wait for the work queued on the scene's streams,
+ * never touch the framebuffer (clear it before rendering the edited frame) and leave the scene unchanged when they fail.
+ *   crgpu_scene_set_camera     copies every field of `cam` bit for bit; its width and height must be the scene's image size.
+ *   crgpu_scene_set_instances  takes A and Ainv of each instance bit for bit (Ainv is not recomputed); `count`, and each instance's
+ *                              kind and object, must be those uploaded (instances cannot be added or removed).  The instance
+ *                              boxes, ray offsets and the top-level BVH are rebuilt on the device, the tree that the scene loader
+ *                              builds.  The first call gives the scene its own copy of the BVH pair nodes (the uploaded pairs plus
+ *                              room for any top level of `count` instances); later calls reuse it.
+ * Edits apply to this device scene only: the crgpu_prepared it was created from, and any scene created from that later, are
+ * unedited. */
+int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam);
+int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
+
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
  * use) order the kernels with its own work and time them with its own events.  crgpu_use_own_stream goes
