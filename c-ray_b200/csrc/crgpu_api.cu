@@ -1071,53 +1071,84 @@ static int check_rect(const crgpu_scene *s, int x0, int y0, int x1, int y1) {
 	return CRGPU_OK;
 }
 
-/* How render_pixels runs the gates of an armed call (render_armed).  A whole call: every batch checks the stop word and publishes.
- * A piece of a pass-major walk (one batch of passes over one piece): only the first piece of a pass batch checks the stop word,
- * the later ones follow its decision, and the last piece publishes the pass batch. */
-struct StopArm {
-	bool first;                /* reset the abandoned flag at the first gate and check the stop word at every gate */
-	bool last;                 /* publish after K5 */
+/* The gates of an armed call in one batch loop (render_batches); an unarmed call runs none.  A whole call: every batch checks the
+ * stop word and publishes.  A piece of a pass-major walk (one batch of passes over one piece): only the first piece of a pass batch
+ * checks the stop word, the later ones follow its decision, and the last piece publishes the pass batch. */
+struct Gates {
+	bool check;                /* reset the abandoned flag at the first gate and check the stop word at every gate */
+	bool publish;              /* publish after K5 */
 	bool whole;                /* a whole call: stop enqueueing batches once the stop word is set */
 	uint64_t call_pixels;      /* pixels of the whole call (a pass batch commits call_pixels * passes paths) */
 };
-static int render_armed(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats);
 static bool stop_requested(const crgpu_scene *s) { return __atomic_load_n(&s->stop_host[0], __ATOMIC_ACQUIRE) != 0u; }
 
-/* the wavefront driver: passes [pass_begin, +pass_count) over a pixel set (a rectangle, or an explicit list) */
-static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count,
-						 unsigned flags, struct crgpu_stats *stats, const StopArm *arm = nullptr) {
-	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
-		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
-	if (s->armed && !arm) return render_armed(s, base, tile_pixels, pass_begin, pass_count, flags, stats);
-	if (tile_pixels > s->max_paths) {
-		/* more pixels than paths in flight: walk the pixel set in pieces (rows of the rectangle / ranges of the list) */
-		const unsigned inner = flags | CRGPU_FLAG_ASYNC;
-		if (base.pixels) {
-			for (uint64_t p0 = 0; p0 < tile_pixels; p0 += s->max_paths) {
-				TileDesc part = base;
-				part.pixels = base.pixels + p0;
-				const uint64_t cnt = tile_pixels - p0 < s->max_paths ? tile_pixels - p0 : s->max_paths;
-				int rc = render_pixels(s, part, cnt, pass_begin, pass_count, inner, nullptr);
-				if (rc) return rc;
-			}
-		} else {
-			const uint64_t rows = s->max_paths / (uint64_t)base.tw;
-			if (rows < 1) return fail(CRGPU_ERR_BAD_ARGUMENT, "tile is %d pixels wide > max paths in flight %llu", base.tw, (unsigned long long)s->max_paths);
-			for (int y = 0; y < base.th; y += (int)rows) {
-				TileDesc part = base;
-				part.y0 = base.y0 + y;
-				part.th = base.th - y < (int)rows ? base.th - y : (int)rows;
-				int rc = render_pixels(s, part, (uint64_t)part.tw * (uint64_t)part.th, pass_begin, pass_count, inner, nullptr);
-				if (rc) return rc;
-			}
+/* CRGPU_FLAG_TIME_KERNELS: events around the kernels of one batch loop.  Per batch K1's start and end (k1); per bounce TEV events
+ * (bounce): before K2, after K2, after K4, after each of K3's miss / flat / generic launches, after the K4b sort. */
+struct KernelTimes {
+	enum { TEV = 7 };
+	std::vector<cudaEvent_t> k1, bounce;
+	static void mark(std::vector<cudaEvent_t> &v, cudaStream_t on) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, on); v.push_back(e); }
+	~KernelTimes() {
+		for (cudaEvent_t e : k1) cudaEventDestroy(e);
+		for (cudaEvent_t e : bounce) cudaEventDestroy(e);
+	}
+	/* once the events have completed: add the loop's time (s->ev[0] .. s->ev[1]) and its K2 and K4 + K3 + K4b times to the scene's
+	 * pending stats, and report them on stderr under CRGPU_DUMP_TIMES */
+	void fold(crgpu_scene *s, int maxDepth) const {
+		float total_ms = 0.f, trace_ms = 0.f, shade_ms = 0.f;
+		cudaEventElapsedTime(&total_ms, s->ev[0], s->ev[1]);
+		const char *dump = getenv("CRGPU_DUMP_TIMES");
+		const int dump_level = dump ? atoi(dump) : 0;
+		/* CRGPU_DUMP_TIMES=2: K1 per batch, and per bounce K2 (trace), K4 + K3 (shade) and shade's parts: K4, K3's miss / flat / generic
+		 * launches (an unsplit K3 counts as miss), the rest (the K4b sort) */
+		for (size_t i = 0; dump_level > 1 && i + 2 <= k1.size(); i += 2) {
+			float g = 0.f;
+			cudaEventElapsedTime(&g, k1[i], k1[i + 1]);
+			fprintf(stderr, "crgpu: batch %zu k1 %.3f ms\n", i / 2, g);
 		}
-		if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
-		return crgpu_get_stats(s, stats);
+		for (size_t i = 0; i + TEV <= bounce.size(); i += TEV) {
+			float t[TEV - 1] = {};
+			for (int k = 0; k + 1 < TEV; ++k) cudaEventElapsedTime(&t[k], bounce[i + (size_t)k], bounce[i + (size_t)k + 1]);
+			const float a = t[0], b = t[1] + t[2] + t[3] + t[4] + t[5];
+			trace_ms += a; shade_ms += b;
+			const size_t n = i / TEV;
+			if (dump && (a > 5.f || b > 8.f || dump_level > 1))
+				fprintf(stderr, "crgpu: batch %zu depth %zu trace %.3f ms shade %.3f ms k4 %.3f miss %.3f flat %.3f generic %.3f sort %.3f\n",
+				        n / (size_t)maxDepth, n % (size_t)maxDepth, a, b, t[1], t[2], t[3], t[4], t[5]);
+		}
+		s->pend_trace_ms += trace_ms; s->pend_shade_ms += shade_ms; s->pend_total_ms += total_ms;
 	}
-	if (pass_count == 0 || tile_pixels == 0) {          /* an empty pass range is a no-op (and must not reach the batch arithmetic below) */
-		if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
-		return crgpu_get_stats(s, stats);
+};
+
+/* One bounce over half `cur` of a wave set: K2, K4 (the flat materials' buckets first when K3 has a flat launch), K3, and K4b when a
+ * sort mode is set and another bounce follows.  Returns the number of kernels it enqueued.  times: NULL, or the timing events. */
+static uint64_t enqueue_bounce(const crgpu_scene *s, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool count, bool sorted,
+                               bool xnodes, const TraceKnobs &kn, const ShadeKnobs &sk, cudaStream_t st, KernelTimes *times) {
+	const int grid = s->sm_count * 8;
+	if (times) times->mark(times->bounce, st);
+	crg_launch_trace(s->dev, wb, cur, count, sorted, kn, st);
+	if (times) times->mark(times->bounce, st);
+	if (crg_shade_flat_order(sk)) crg_launch_bucket(wb, cur, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
+	else crg_launch_bucket(wb, cur, grid, nullptr, 0, st);
+	cudaEvent_t k3ev[3] = { nullptr, nullptr, nullptr };
+	if (times) {
+		times->mark(times->bounce, st);
+		for (cudaEvent_t &e : k3ev) { cudaEventCreate(&e); times->bounce.push_back(e); }
 	}
+	const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
+	uint64_t launches = 2 + (uint64_t)crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, xnodes, s->dev.bg.kind != CRG_BG_NONE,
+	                                                   grid, sk, st, times ? k3ev : nullptr);
+	if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
+		crg_launch_dirsort(wb, cur ^ 1, dirmode == 4 ? (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1) : -1, grid, st);
+		++launches;
+	}
+	if (times) times->mark(times->bounce, st);
+	return launches;
+}
+
+/* The batch loop: passes [pass_begin, +pass_count) over one piece of at most max_paths pixels (pass_count > 0). */
+static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, const Gates &gates) {
+	const bool armed = s->armed;
 	const bool count = (flags & CRGPU_FLAG_COUNT) != 0;
 	const bool timing = (flags & CRGPU_FLAG_TIME_KERNELS) != 0;
 	/* Batches.  A batch pays a fixed cost of several ms: its bounces 5..12 hold too few rays to fill the SMs (132 on H100), and every bounce lasts
@@ -1145,20 +1176,15 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	const TraceKnobs &knobs = crg_trace_knobs_env();
 	const ShadeKnobs &sknobs = crg_shade_knobs_env();
 	uint64_t launches = 0;
-	float trace_ms = 0.f, shade_ms = 0.f;
+	KernelTimes times;
 	if (timing) CU(cudaEventRecord(s->ev[0], s->stream));
-	/* per-kernel events when timing: per batch K1's start and end (gev); per bounce CRG_TEV events (tev): before K2, after K2, after
-	 * K4, after each of K3's miss / flat / generic launches, after the K4b sort */
-	enum { CRG_TEV = 7 };
-	std::vector<cudaEvent_t> tev, gev;
-	auto mark = [&](std::vector<cudaEvent_t> &v, cudaStream_t on) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, on); v.push_back(e); };
 	if (sets == 2) {                /* fork: the second stream starts behind whatever is queued on the first */
 		CU(cudaEventRecord(s->evFork, s->stream));
 		CU(cudaStreamWaitEvent(s->stream2, s->evFork, 0));
 	}
 	int bi = 0;
 	for (int pb = pass_begin; pb < pass_begin + pass_count; pb += (int)batch, ++bi) {
-		if (arm && arm->whole && stop_requested(s)) break;       /* its gates would abandon it anyway */
+		if (armed && gates.whole && stop_requested(s)) break;       /* its gates would abandon it anyway */
 		const int set = sets == 2 ? (bi & 1) : 0;
 		cudaStream_t st = set ? s->stream2 : s->stream;
 		const WaveBuffers &wb = set ? s->wb2 : s->wb;
@@ -1166,42 +1192,25 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 		td.npix = (unsigned)tile_pixels;
 		td.pass_begin = pb;
 		td.pass_count = (pass_begin + pass_count - pb) < (int)batch ? (pass_begin + pass_count - pb) : (int)batch;
-		if (timing) mark(gev, st);
+		if (timing) times.mark(times.k1, st);
 		crg_launch_generate(s->dev, wb, td, grid, st); ++launches;
-		if (timing) mark(gev, st);
+		if (timing) times.mark(times.k1, st);
 		/* bounces == 0: pathTrace's loop never runs and every sample is black (pathtrace.c:34-36,59).  L is write-once by
 		 * design (cr_add_radiance / cr_finish_path), so with no bounce nothing would write it: clear it here instead */
 		if (maxDepth == 0) CU(cudaMemsetAsync(wb.L, 0, (size_t)tile_pixels * (size_t)td.pass_count * sizeof(float4), st));
-		if (arm && maxDepth == 0) { crg_launch_stop_gate(wb.counts, 0, s->stop_ctl, set, s->stop_host, arm->first, arm->first, st); ++launches; }
+		if (armed && maxDepth == 0) { crg_launch_stop_gate(wb.counts, 0, s->stop_ctl, set, s->stop_host, gates.check, gates.check, st); ++launches; }
 		int cur = 0;
 		for (int depth = 0; depth < maxDepth; ++depth) {
-			if (arm) { crg_launch_stop_gate(wb.counts, cur, s->stop_ctl, set, s->stop_host, arm->first && depth == 0, arm->first, st); ++launches; }
+			if (armed) { crg_launch_stop_gate(wb.counts, cur, s->stop_ctl, set, s->stop_host, gates.check && depth == 0, gates.check, st); ++launches; }
 			if (depth >= CRG_TAIL_FROM && !count) { crg_launch_tail(s->dev_copy, wb, cur, depth, maxDepth, s->xnodes, st); ++launches; }
-			if (timing) mark(tev, st);
-			crg_launch_trace(s->dev, wb, cur, count, dirmode != 0 && depth > 0, knobs, st);
-			if (timing) mark(tev, st);
-			if (crg_shade_flat_order(sknobs)) crg_launch_bucket(wb, cur, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
-			else crg_launch_bucket(wb, cur, grid, nullptr, 0, st);
-			cudaEvent_t k3ev[3] = { nullptr, nullptr, nullptr };
-			if (timing) {
-				mark(tev, st);
-				for (cudaEvent_t &e : k3ev) { cudaEventCreate(&e); tev.push_back(e); }
-			}
-			const bool sort_next = dirmode != 0 && depth + 1 < maxDepth;
-			crg_launch_shade(s->dev_copy, wb, cur, depth, maxDepth, sort_next ? dirmode : 0, s->xnodes, s->dev.bg.kind != CRG_BG_NONE, grid, sknobs, st,
-			                 timing ? k3ev : nullptr);
-			if (sort_next) {                                                               /* K4b: the next bounce's rays by direction bin */
-				crg_launch_dirsort(wb, cur ^ 1, dirmode == 4 ? (depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1) : -1, grid, st);
-				++launches;
-			}
-			if (timing) mark(tev, st);
-			launches += 2 + (uint64_t)crg_shade_launches_per_bounce(sknobs);
+			launches += enqueue_bounce(s, wb, cur, depth, maxDepth, dirmode, count, dirmode != 0 && depth > 0, s->xnodes, knobs, sknobs, st,
+			                           timing ? &times : nullptr);
 			cur ^= 1;
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
-		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, arm ? s->stop_ctl : nullptr, set); ++launches;
-		if (arm && arm->last) {
-			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, arm->call_pixels * (uint64_t)td.pass_count, wb.stats, st);
+		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set); ++launches;
+		if (armed && gates.publish) {
+			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats, st);
 			++launches;
 		}
 		if (sets == 2) CU(cudaEventRecord(s->evAcc[set], st));      /* after the publish step: the next K5 reads what it wrote */
@@ -1213,96 +1222,81 @@ static int render_pixels(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, in
 	cudaStream_t st = s->stream;
 	if (timing) CU(cudaEventRecord(s->ev[1], st));
 	CU(cudaGetLastError());
-	if (!arm) s->pend_paths += tile_pixels * (uint64_t)pass_count;   /* an armed call counts what its publish steps committed */
+	if (!armed) s->pend_paths += tile_pixels * (uint64_t)pass_count;   /* an armed call counts what its publish steps committed */
 	s->pend_launches += launches;
 	if (timing) {
 		CU(cudaStreamSynchronize(st));
-		float total_ms = 0.f;
-		cudaEventElapsedTime(&total_ms, s->ev[0], s->ev[1]);
-		const char *dump = getenv("CRGPU_DUMP_TIMES");
-		const int dump_level = dump ? atoi(dump) : 0;
-		/* CRGPU_DUMP_TIMES=2: K1 per batch, and per bounce K2 (trace), K4 + K3 (shade) and shade's parts: K4, K3's miss / flat / generic
-		 * launches (an unsplit K3 counts as miss), the rest (the K4b sort) */
-		for (size_t i = 0; dump_level > 1 && i + 2 <= gev.size(); i += 2) {
-			float g = 0.f;
-			cudaEventElapsedTime(&g, gev[i], gev[i + 1]);
-			fprintf(stderr, "crgpu: batch %zu k1 %.3f ms\n", i / 2, g);
-		}
-		for (size_t i = 0; i + CRG_TEV <= tev.size(); i += CRG_TEV) {
-			float t[CRG_TEV - 1] = {};
-			for (int k = 0; k + 1 < CRG_TEV; ++k) cudaEventElapsedTime(&t[k], tev[i + (size_t)k], tev[i + (size_t)k + 1]);
-			const float a = t[0], b = t[1] + t[2] + t[3] + t[4] + t[5];
-			trace_ms += a; shade_ms += b;
-			const size_t bounce = i / CRG_TEV;
-			if (dump && (a > 5.f || b > 8.f || dump_level > 1))
-				fprintf(stderr, "crgpu: batch %zu depth %zu trace %.3f ms shade %.3f ms k4 %.3f miss %.3f flat %.3f generic %.3f sort %.3f\n",
-				        bounce / (size_t)maxDepth, bounce % (size_t)maxDepth, a, b, t[1], t[2], t[3], t[4], t[5]);
-		}
-		for (cudaEvent_t e : tev) cudaEventDestroy(e);
-		for (cudaEvent_t e : gev) cudaEventDestroy(e);
-		s->pend_trace_ms += trace_ms; s->pend_shade_ms += shade_ms; s->pend_total_ms += total_ms;
+		times.fold(s, maxDepth);
 	}
-	if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
-	return crgpu_get_stats(s, stats);
+	return CRGPU_OK;
 }
 
-/* An armed call.  Every batch commits in pass order or not at all (StopArm, k_accumulate<true>, k_stop_publish), so after the call
- * the framebuffer holds exactly passes [0, committed) and a later call for [committed, end) finishes it bit for bit.  A pixel set
- * larger than the paths in flight is walked pass-major: each batch of passes covers every piece before the next batch starts, so
- * one pass count describes the whole set.  A stop is then taken only at the first piece of a pass batch (the later pieces must
- * complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set. */
-static int render_armed(crgpu_scene *s, TileDesc base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats) {
-	const unsigned inner = flags | CRGPU_FLAG_ASYNC;
-	__atomic_store_n(&s->stop_host[1], (unsigned)pass_begin, __ATOMIC_RELEASE);
-	__atomic_store_n(&s->stop_host[2], 1u, __ATOMIC_RELEASE);
-	crg_launch_stop_begin(s->stop_ctl, s->stop_host, pass_begin, s->stream);
-	uint64_t launches = 2;
-	int rc = CRGPU_OK;
-	if (pass_count == 0 || tile_pixels == 0) {
-		/* nothing to render: the begin and end steps publish pass_begin */
-	} else if (tile_pixels <= s->max_paths) {
-		const StopArm a = { true, true, true, tile_pixels };
-		rc = render_pixels(s, base, tile_pixels, pass_begin, pass_count, inner, nullptr, &a);
-	} else {
-		std::vector<TileDesc> parts;
-		std::vector<uint64_t> counts;
-		if (base.pixels) {
-			for (uint64_t p0 = 0; p0 < tile_pixels; p0 += s->max_paths) {
-				TileDesc part = base;
-				part.pixels = base.pixels + p0;
-				parts.push_back(part);
-				counts.push_back(tile_pixels - p0 < s->max_paths ? tile_pixels - p0 : s->max_paths);
-			}
-		} else {
-			const uint64_t rows = s->max_paths / (uint64_t)base.tw;
-			if (rows < 1) rc = fail(CRGPU_ERR_BAD_ARGUMENT, "tile is %d pixels wide > max paths in flight %llu", base.tw, (unsigned long long)s->max_paths);
-			for (int y = 0; rc == CRGPU_OK && y < base.th; y += (int)rows) {
-				TileDesc part = base;
-				part.y0 = base.y0 + y;
-				part.th = base.th - y < (int)rows ? base.th - y : (int)rows;
-				parts.push_back(part);
-				counts.push_back((uint64_t)part.tw * (uint64_t)part.th);
-			}
+/* A pixel set cut into pieces of at most max_paths pixels: rows of the rectangle, or ranges of the list.  A set that fits is one piece. */
+struct Piece { TileDesc td; uint64_t pixels; };
+static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, std::vector<Piece> &pieces) {
+	const uint64_t most = s->max_paths;
+	if (tile_pixels <= most) { pieces.push_back({ base, tile_pixels }); return CRGPU_OK; }
+	if (base.pixels) {
+		for (uint64_t p0 = 0; p0 < tile_pixels; p0 += most) {
+			Piece p = { base, tile_pixels - p0 < most ? tile_pixels - p0 : most };
+			p.td.pixels = base.pixels + p0;
+			pieces.push_back(p);
 		}
+		return CRGPU_OK;
+	}
+	const uint64_t rows = most / (uint64_t)base.tw;
+	if (rows < 1) return fail(CRGPU_ERR_BAD_ARGUMENT, "tile is %d pixels wide > max paths in flight %llu", base.tw, (unsigned long long)most);
+	for (int y = 0; y < base.th; y += (int)rows) {
+		Piece p = { base, 0 };
+		p.td.y0 = base.y0 + y;
+		p.td.th = base.th - y < (int)rows ? base.th - y : (int)rows;
+		p.pixels = (uint64_t)p.td.tw * (uint64_t)p.td.th;
+		pieces.push_back(p);
+	}
+	return CRGPU_OK;
+}
+
+/* A render call: passes [pass_begin, +pass_count) over a pixel set (a rectangle, or an explicit list).  Unarmed, the pieces are
+ * walked piece-major: every pass of a piece, its batches overlapped on the two wave sets, before the next piece.  Armed, every batch
+ * commits in pass order or not at all (Gates, k_accumulate<true>, k_stop_publish), so the framebuffer then holds exactly passes
+ * [0, committed) and a later call for [committed, end) finishes it bit for bit; several pieces are walked pass-major, each batch of
+ * passes over every piece, so that one pass count describes the set.  Only the first piece of a pass batch takes a stop (the later
+ * ones complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set. */
+static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats) {
+	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
+	const bool armed = s->armed;
+	if (armed) {
+		__atomic_store_n(&s->stop_host[1], (unsigned)pass_begin, __ATOMIC_RELEASE);
+		__atomic_store_n(&s->stop_host[2], 1u, __ATOMIC_RELEASE);
+		crg_launch_stop_begin(s->stop_ctl, s->stop_host, pass_begin, s->stream);
+	}
+	std::vector<Piece> pieces;
+	int rc = CRGPU_OK;
+	if (pass_count > 0 && tile_pixels > 0) rc = split_pieces(s, base, tile_pixels, pieces);   /* an empty call renders nothing */
+	if (!armed || pieces.size() < 2) {
+		for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
+			rc = render_batches(s, pieces[k].td, pieces[k].pixels, pass_begin, pass_count, flags, { true, true, true, tile_pixels });
+	} else {
 		uint64_t widest = 1;
-		for (uint64_t c : counts) widest = c > widest ? c : widest;
+		for (const Piece &p : pieces) widest = p.pixels > widest ? p.pixels : widest;
 		const int passes = (int)(s->max_paths / widest < 1 ? 1 : s->max_paths / widest);   /* one batch per piece */
 		for (int pb = pass_begin; rc == CRGPU_OK && pb < pass_begin + pass_count; pb += passes) {
 			if (stop_requested(s)) break;
 			const int n = pass_begin + pass_count - pb < passes ? pass_begin + pass_count - pb : passes;
-			for (size_t k = 0; rc == CRGPU_OK && k < parts.size(); ++k) {
-				const StopArm a = { k == 0, k + 1 == parts.size(), false, tile_pixels };
-				rc = render_pixels(s, parts[k], counts[k], pb, n, inner, nullptr, &a);
-			}
+			for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
+				rc = render_batches(s, pieces[k].td, pieces[k].pixels, pb, n, flags, { k == 0, k + 1 == pieces.size(), false, tile_pixels });
 		}
 	}
-	crg_launch_stop_end(s->stop_ctl, s->stop_host, s->stream);   /* also after a failed enqueue: the in-flight word must clear */
-	s->pend_launches += launches;
+	if (armed) {
+		crg_launch_stop_end(s->stop_ctl, s->stop_host, s->stream);   /* also after a failed enqueue: the in-flight word must clear */
+		s->pend_launches += 2;
+	}
 	if (rc) return rc;
 	CU(cudaGetLastError());
 	if (flags & CRGPU_FLAG_ASYNC) return CRGPU_OK;
 	rc = crgpu_get_stats(s, stats);
-	if (rc) return rc;
+	if (rc || !armed) return rc;
 	return __atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE) < (unsigned)(pass_begin + pass_count) ? CRGPU_STOPPED : CRGPU_OK;
 }
 
@@ -1464,7 +1458,7 @@ extern "C" int crgpu_render_tile(crgpu_scene *s, int x0, int y0, int x1, int y1,
 	memset(&td, 0, sizeof td);
 	td.x0 = x0; td.y0 = y0; td.tw = x1 - x0; td.th = y1 - y0;
 	td.pixels = nullptr;
-	return render_pixels(s, td, (uint64_t)td.tw * (uint64_t)td.th, pass_begin, pass_count, flags, stats);
+	return render_call(s, td, (uint64_t)td.tw * (uint64_t)td.th, pass_begin, pass_count, flags, stats);
 }
 
 extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, int pass_begin, int pass_count,
@@ -1510,7 +1504,7 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 	TileDesc td;
 	memset(&td, 0, sizeof td);
 	td.pixels = s->pixels;
-	return render_pixels(s, td, total, pass_begin, pass_count, flags, stats);
+	return render_call(s, td, total, pass_begin, pass_count, flags, stats);
 }
 
 extern "C" int crgpu_get_stats(crgpu_scene *s, struct crgpu_stats *stats) {
@@ -1609,6 +1603,38 @@ extern "C" int crgpu_scene_info(crgpu_scene *s, int *device, int *width, int *he
 	return CRGPU_OK;
 }
 
+/* ---- test entries: a batch of rays or path states in half 0 of wave set 0 -----------------------------------------------------------
+ * stage_half0 takes the counters of earlier work (so that the stats afterwards are this batch's), makes room for n paths, loads stA,
+ * stB and (path states) stC, sets the live count to n and clears K2's histogram.  read_trace_records copies K2's write-back of the
+ * batch (crg_launch_trace_records) to the host and waits for the stream. */
+static int stage_half0(crgpu_scene *s, uint32_t n, const float4 *a, const float4 *b, const uint4 *c) {
+	int rc = crgpu_get_stats(s, nullptr);
+	if (rc) return rc;
+	rc = alloc_wave(s, n ? n : 1, 1);
+	if (rc) return rc;
+	const WaveBuffers &wb = s->wb;
+	cudaStream_t st = s->stream;
+	const unsigned counts[5] = { n, 0u, 0u, 0u, 0u };
+	CU(cudaMemcpyAsync(wb.stA[0], a, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(wb.stB[0], b, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
+	if (c) CU(cudaMemcpyAsync(wb.stC[0], c, (size_t)n * sizeof(uint4), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(wb.counts, counts, sizeof counts, cudaMemcpyHostToDevice, st));
+	CU(cudaMemsetAsync(wb.hist, 0, 1024 * sizeof(unsigned), st));
+	return CRGPU_OK;
+}
+static int read_trace_records(crgpu_scene *s, uint32_t n, struct crgpu_ray_record *out, const char *entry) {
+	if (!n) return CRGPU_OK;
+	void *drec = nullptr;
+	CU(cudaMalloc(&drec, (size_t)n * sizeof *out));
+	crg_launch_trace_records(s->dev, s->wb, n, drec, s->sm_count * 8, s->stream);
+	cudaError_t e = cudaGetLastError();
+	if (e == cudaSuccess) e = cudaMemcpyAsync(out, drec, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, s->stream);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+	cudaFree(drec);
+	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "%s: %s", entry, cudaGetErrorString(e));
+	return CRGPU_OK;
+}
+
 /* Closest hits of a ray batch through the production K2 (k_trace, by the launch path and launch shape of a frame) and K4. */
 extern "C" int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, const struct crgpu_trace_opts *opts,
 								struct crgpu_ray_record *records_out, uint32_t *perm_out, uint32_t *misses_out, struct crgpu_stats *stats_out) {
@@ -1625,25 +1651,17 @@ extern "C" int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, c
 		}
 	}
 	CU(cudaSetDevice(s->device));
-	int rc = crgpu_get_stats(s, nullptr);               /* earlier work done and its counters taken: the deltas below are this batch's */
-	if (rc) return rc;
-	rc = alloc_wave(s, n ? n : 1, 1);
-	if (rc) return rc;
-	const WaveBuffers &wb = s->wb;
-	cudaStream_t st = s->stream;
-	const int grid = s->sm_count * 8;
 	std::vector<float4> a(n), b(n);
 	for (uint32_t i = 0; i < n; ++i) {
 		const float *r = rays + 6 * (size_t)i;
 		a[i] = make_float4(r[0], r[1], r[2], r[3]);
 		b[i] = make_float4(r[4], r[5], 1.0f, 1.0f);
 	}
-	const unsigned counts[5] = { n, 0u, 0u, 0u, 0u };
-	CU(cudaMemcpyAsync(wb.stA[0], a.data(), (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(wb.stB[0], b.data(), (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, st));
+	int rc = stage_half0(s, n, a.data(), b.data(), nullptr);
+	if (rc) return rc;
+	const WaveBuffers &wb = s->wb;
+	cudaStream_t st = s->stream;
 	if (opts->order) CU(cudaMemcpyAsync(wb.perm2, opts->order, (size_t)n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(wb.counts, counts, sizeof counts, cudaMemcpyHostToDevice, st));
-	CU(cudaMemsetAsync(wb.hist, 0, 1024 * sizeof(unsigned), st));
 	/* poison: no write-back produces a negative distance or the instance index -1515870811, and K4 must overwrite all of perm.
 	 * Every 8-bit value is some ray's key, so a key left behind shows only as a key that differs from the expected one; the
 	 * write-back stores hit, instance and key together, so a ray it missed also keeps the hit and instance poison */
@@ -1652,20 +1670,15 @@ extern "C" int crgpu_trace_rays(crgpu_scene *s, const float *rays, uint32_t n, c
 	CU(cudaMemsetAsync(wb.hitKey, 0xA5, (size_t)n, st));
 	CU(cudaMemsetAsync(wb.perm, 0xFF, (size_t)n * sizeof(unsigned), st));
 	crg_launch_trace(s->dev, wb, 0, opts->count != 0, opts->order != nullptr, kn, st);
-	crg_launch_bucket(wb, 0, grid, nullptr, 0, st);      /* buckets in key order */
+	crg_launch_bucket(wb, 0, s->sm_count * 8, nullptr, 0, st);      /* buckets in key order */
 	CU(cudaGetLastError());
-	void *drec = nullptr;
-	if (n) {
-		CU(cudaMalloc(&drec, (size_t)n * sizeof(struct crgpu_ray_record)));
-		crg_launch_trace_records(s->dev, wb, n, drec, grid, st);
-	}
+	rc = read_trace_records(s, n, records_out, "trace_rays");
+	if (rc) return rc;
 	unsigned cnt[5];
-	cudaError_t e = cudaGetLastError();
-	if (e == cudaSuccess && n) e = cudaMemcpyAsync(records_out, drec, (size_t)n * sizeof(struct crgpu_ray_record), cudaMemcpyDeviceToHost, st);
-	if (e == cudaSuccess && n) e = cudaMemcpyAsync(perm_out, wb.perm, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+	cudaError_t e = cudaSuccess;
+	if (n) e = cudaMemcpyAsync(perm_out, wb.perm, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
 	if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, wb.counts, sizeof cnt, cudaMemcpyDeviceToHost, st);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-	if (drec) cudaFree(drec);
 	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "trace_rays: %s", cudaGetErrorString(e));
 	if (misses_out) *misses_out = cnt[4];
 	return crgpu_get_stats(s, stats_out);               /* fails if the traversal watchdog fired */
@@ -1689,8 +1702,8 @@ extern "C" int crgpu_trace_kat(crgpu_scene *s, const int32_t *xyp, int count, vo
 	return CRGPU_OK;
 }
 
-/* One bounce of a batch of path states through the kernels of a frame's bounce, launched by the frame's own launch functions: K2 ->
- * K4 -> K3 (and K4b when a sort mode is set and another bounce follows), or the tail kernel.  The states go into the current half
+/* One bounce of a batch of path states through the frame's own bounce sequence (enqueue_bounce): K2 -> K4 -> K3 (and K4b when a
+ * sort mode is set and another bounce follows), or the tail kernel.  The states go into the current half
  * of the wave buffers with id = their index (| CRG_ID_HAS_L where has_l is set) and L as given; the other half is poisoned.  Each
  * result is found by the id K3 compacted it with. */
 #define CRG_ID_HAS_L_HOST 0x80000000u
@@ -1705,13 +1718,6 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 		opts->depth < 0 || opts->max_depth < 1 || opts->depth >= opts->max_depth)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "shade options out of range");
 	CU(cudaSetDevice(s->device));
-	int rc = crgpu_get_stats(s, nullptr);
-	if (rc) return rc;
-	rc = alloc_wave(s, n ? n : 1, 1);
-	if (rc) return rc;
-	const WaveBuffers &wb = s->wb;
-	cudaStream_t st = s->stream;
-	const int grid = s->sm_count * 8;
 	const bool xnodes = s->xnodes || opts->complete_interpreter;
 	std::vector<float4> a(n), b(n), L(n);
 	std::vector<uint4> c(n);
@@ -1724,12 +1730,12 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 		c[i] = make_uint4(wb32, i | (p.has_l ? CRG_ID_HAS_L_HOST : 0u), (uint32_t)(p.rng & 0xffffffffull), (uint32_t)(p.rng >> 32));
 		L[i] = make_float4(p.L[0], p.L[1], p.L[2], 0.0f);
 	}
-	const unsigned counts[5] = { n, 0u, 0u, 0u, 0u };
+	int rc = stage_half0(s, n, a.data(), b.data(), c.data());
+	if (rc) return rc;
+	const WaveBuffers &wb = s->wb;
+	cudaStream_t st = s->stream;
 	const size_t n4 = (size_t)n * sizeof(float4);
 	if (n) {
-		CU(cudaMemcpyAsync(wb.stA[0], a.data(), n4, cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(wb.stB[0], b.data(), n4, cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(wb.stC[0], c.data(), n4, cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(wb.L, L.data(), n4, cudaMemcpyHostToDevice, st));
 		CU(cudaMemsetAsync(wb.stA[1], 0xA5, n4, st));
 		CU(cudaMemsetAsync(wb.stB[1], 0xA5, n4, st));
@@ -1739,39 +1745,26 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 		CU(cudaMemsetAsync(wb.dirKey, 0xA5, (size_t)n, st));
 		CU(cudaMemsetAsync(wb.perm2, 0xFF, (size_t)n * sizeof(unsigned), st));
 	}
-	CU(cudaMemcpyAsync(wb.counts, counts, sizeof counts, cudaMemcpyHostToDevice, st));
-	CU(cudaMemsetAsync(wb.hist, 0, 1024 * sizeof(unsigned), st));
 	const int depth = opts->depth, maxDepth = opts->max_depth;
 	const int box_slot = depth < CRG_BOX_SLOTS ? depth : CRG_BOX_SLOTS - 1;
 	unsigned box[12];
 	CU(cudaMemcpyAsync(box, wb.box + 12 * box_slot, sizeof box, cudaMemcpyDeviceToHost, st));
-	if (opts->tail) {
-		crg_launch_tail(s->dev_copy, wb, 0, depth, maxDepth, xnodes, st);
-	} else {
-		crg_launch_trace(s->dev, wb, 0, false, false, crg_trace_knobs_env(), st);
-		if (crg_shade_flat_order(kn)) crg_launch_bucket(wb, 0, grid, s->dev.key_order, (int)s->dev.flat_keys, st);
-		else crg_launch_bucket(wb, 0, grid, nullptr, 0, st);
-		const bool sort_next = opts->dirmode != 0 && depth + 1 < maxDepth;
-		crg_launch_shade(s->dev_copy, wb, 0, depth, maxDepth, sort_next ? opts->dirmode : 0, xnodes, s->dev.bg.kind != CRG_BG_NONE, grid, kn, st);
-		if (sort_next) crg_launch_dirsort(wb, 1, opts->dirmode == 4 ? box_slot : -1, grid, st);
-	}
+	if (opts->tail) crg_launch_tail(s->dev_copy, wb, 0, depth, maxDepth, xnodes, st);
+	else enqueue_bounce(s, wb, 0, depth, maxDepth, opts->dirmode, false, false, xnodes, crg_trace_knobs_env(), kn, st, nullptr);
 	CU(cudaGetLastError());
-	void *drec = nullptr;
-	if (n && !opts->tail) {
-		CU(cudaMalloc(&drec, (size_t)n * sizeof(struct crgpu_ray_record)));
-		crg_launch_trace_records(s->dev, wb, n, drec, grid, st);
-	}
 	std::vector<crgpu_ray_record> rec(n);
+	if (!opts->tail) {
+		rc = read_trace_records(s, n, rec.data(), "shade_rays");
+		if (rc) return rc;
+	}
 	std::vector<float4> a2(n), b2(n), L2(n);
 	std::vector<uint4> c2(n);
 	std::vector<uint8_t> dk(n);
 	unsigned cnt[5];
-	cudaError_t e = cudaGetLastError();
-	if (e == cudaSuccess && drec) e = cudaMemcpyAsync(rec.data(), drec, (size_t)n * sizeof(struct crgpu_ray_record), cudaMemcpyDeviceToHost, st);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, wb.counts, sizeof cnt, cudaMemcpyDeviceToHost, st);
+	cudaError_t e = cudaMemcpyAsync(cnt, wb.counts, sizeof cnt, cudaMemcpyDeviceToHost, st);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
 	const uint32_t surv = opts->tail ? cnt[0] : cnt[1];
-	if (e == cudaSuccess && surv > n) { if (drec) cudaFree(drec); return fail(CRGPU_ERR_CUDA, "shade_rays: %u survivors of %u paths", surv, n); }
+	if (e == cudaSuccess && surv > n) return fail(CRGPU_ERR_CUDA, "shade_rays: %u survivors of %u paths", surv, n);
 	const int half = opts->tail ? 0 : 1;
 	if (e == cudaSuccess && surv) {
 		e = cudaMemcpyAsync(a2.data(), half ? wb.stA[1] : wb.stA[0], (size_t)surv * sizeof(float4), cudaMemcpyDeviceToHost, st);
@@ -1782,7 +1775,6 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 	}
 	if (e == cudaSuccess && n) e = cudaMemcpyAsync(L2.data(), wb.L, n4, cudaMemcpyDeviceToHost, st);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-	if (drec) cudaFree(drec);
 	if (e != cudaSuccess) return fail(CRGPU_ERR_CUDA, "shade_rays: %s", cudaGetErrorString(e));
 	for (uint32_t i = 0; i < n; ++i) {
 		crgpu_shade_result &r = results[i];

@@ -439,8 +439,8 @@ const ShadeKnobs &crg_shade_knobs_env(void) {
 	return kn;
 }
 template <bool X>
-static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, const ShadeKnobs &kn,
-                         bool flat_bg, cudaStream_t st, cudaEvent_t *ev) {
+static int launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, int grid, const ShadeKnobs &kn,
+                        bool flat_bg, cudaStream_t st, cudaEvent_t *ev) {
 	const int minb = kn.minb, split = kn.split, prefetch = kn.prefetch;
 	if (split) {
 		if (flat_bg) k_shade<4, 1, X, true><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
@@ -456,17 +456,18 @@ static void launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, in
 		else if (minb == 4) k_shade<4, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		else k_shade<2, 2, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 		if (ev) cudaEventRecord(ev[2], st);
-		return;
+		return kn.generic_only ? 2 : 3;
 	}
 	if (minb == 3) k_shade<3, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	else if (minb == 4) k_shade<4, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	else k_shade<2, 0, X><<<grid, 256, 0, st>>>(dsc, wb, cur, depth, maxDepth, dirmode, prefetch);
 	if (ev) for (int k = 0; k < 3; ++k) cudaEventRecord(ev[k], st);   /* one launch: it is all in the "miss" share */
+	return 1;
 }
-void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, bool flat_bg, int grid,
-                      const ShadeKnobs &kn, cudaStream_t st, cudaEvent_t *ev) {
-	if (xnodes) launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
-	else launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
+int crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, bool flat_bg, int grid,
+                     const ShadeKnobs &kn, cudaStream_t st, cudaEvent_t *ev) {
+	if (xnodes) return launch_shade<true>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
+	return launch_shade<false>(dsc, wb, cur, depth, maxDepth, dirmode, grid, kn, flat_bg, st, ev);
 }
 void crg_launch_dirsort(const WaveBuffers &wb, int nxt, int box_slot, int grid, cudaStream_t st) {
 	k_bucket<true><<<grid, 256, 0, st>>>(wb, nxt, box_slot, nullptr, 0);
@@ -475,7 +476,6 @@ int crg_dir_mode(void) {
 	static const int mode = [] { const char *e = getenv("CRGPU_TRACE_SORT"); const int v = e ? atoi(e) : 0; return v >= 0 && v <= 4 ? v : 0; }();
 	return mode;
 }
-int crg_shade_launches_per_bounce(const ShadeKnobs &kn) { return kn.split ? (kn.generic_only ? 2 : 3) : 1; }
 bool crg_shade_flat_order(const ShadeKnobs &kn) { return kn.split && !kn.generic_only; }
 
 /* ---- the libm stand-ins one by one (test entry crgpu_libm_eval; the order of include/crgpu.h CRGPU_LIBM_*) -------------------- */

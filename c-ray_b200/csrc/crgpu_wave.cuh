@@ -103,10 +103,10 @@ void crg_launch_tail(const DevScene *dsc, const WaveBuffers &wb, int cur, int de
 struct ShadeKnobs { int minb, split, prefetch, generic_only, flat_minb; };
 const ShadeKnobs &crg_shade_knobs_env(void);
 /* flat_bg: DevScene::bg is folded (the miss launch samples it inline).  ev: NULL, or three events recorded after the miss, the flat
- * and the generic launch (CRGPU_FLAG_TIME_KERNELS' per-launch split) */
-void crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, bool flat_bg, int grid,
-                      const ShadeKnobs &kn, cudaStream_t st, cudaEvent_t *ev = nullptr);
-int crg_shade_launches_per_bounce(const ShadeKnobs &kn);
+ * and the generic launch (CRGPU_FLAG_TIME_KERNELS' per-launch split).  Returns the number of kernels it launched.  The bounce
+ * sequence around it (K2, K4, this, K4b) is enqueue_bounce in crgpu_api.cu, for the frame and for crgpu_shade_rays alike. */
+int crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int depth, int maxDepth, int dirmode, bool xnodes, bool flat_bg, int grid,
+                     const ShadeKnobs &kn, cudaStream_t st, cudaEvent_t *ev);
 /* whether K4 must order the buckets for the flat launch (crg_launch_bucket's order) */
 bool crg_shade_flat_order(const ShadeKnobs &kn);
 /* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */

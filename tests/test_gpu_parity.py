@@ -211,7 +211,7 @@ def test_srgb8_output_byte_exact():
 
 def test_zero_bounces_is_black():
     """prefs.bounces == 0 (accepted by the reference and by the loader): every sample is black; the L buffer is write-once
-    in the kernels, so the driver has to clear it when no bounce runs (crgpu_api.cu render_pixels)."""
+    in the kernels, so the driver has to clear it when no bounce runs (crgpu_api.cu render_batches)."""
     g = crgpu.GpuScene(os.path.join(GOLDEN, "g_single.crscene"), force_bounces=0)
     g.write(np.full((g.H, g.W, 3), 7.0, dtype=np.float32))     # poison: the running average must overwrite it with zeros
     g.clear()
