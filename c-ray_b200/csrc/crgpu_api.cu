@@ -140,7 +140,7 @@ extern "C" void crgpu_host_free(void *p) { if (p) cudaFreeHost(p); }
  * crgpu_prepare() does everything about a scene that does not depend on the device: validation, BVH re-layout into pair nodes,
  * triangle packing, shading records.  crgpu_scene_create_prepared() is then one host->device copy of the slab plus two small
  * pointer-carrying tables.  A host that renders many frames of one scene, or one frame on many GPUs, prepares once. */
-enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_PRIMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_FLAT, SEC_ORDER, SEC_NODES, SEC_TEXS, SEC_LUT,
+enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_ITEMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_FLAT, SEC_ORDER, SEC_NODES, SEC_TEXS, SEC_LUT,
        SEC_TEXDATA, SEC_COUNT };
 struct crgpu_prepared {
 	crs_prefs prefs;
@@ -202,7 +202,7 @@ struct crgpu_scene {
 	std::vector<float> bvh_root;                     /* crgpu_prepared::bvh_root */
 	uint32_t pair_count;       /* pair nodes uploaded (the edit block starts with a copy of them) */
 	uint32_t top_stage_cap;    /* staged top-level pairs reserved at upload */
-	void *edit; size_t edit_bytes;             /* NULL until the first instance edit: uploaded pairs, the top region, top_prims */
+	void *edit; size_t edit_bytes;             /* NULL until the first instance edit: uploaded pairs, the top region, top_items */
 	void *edit_scratch; size_t edit_scratch_bytes;   /* instance inputs, boxes, the new top level and the builder's scratch */
 };
 
@@ -603,6 +603,16 @@ extern "C" int crgpu_prepared_background(const crgpu_prepared *p, uint32_t *kind
 	return CRGPU_OK;
 }
 
+extern "C" int crgpu_prepared_top_level(const crgpu_prepared *p, const void **items, size_t *item_bytes, const void **instances,
+                                        size_t *instance_bytes, const void **bvhs, size_t *bvh_bytes) {
+	if (!p || !items || !item_bytes || !instances || !instance_bytes || !bvhs || !bvh_bytes) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	static_assert(sizeof(DevInstance) == 128 && sizeof(DevBvh) == 60, "crgpu_prepared_top_level documents these record sizes");
+	*items = p->slab + p->off[SEC_TOP_ITEMS]; *item_bytes = p->len[SEC_TOP_ITEMS];
+	*instances = p->slab + p->off[SEC_INSTS]; *instance_bytes = p->len[SEC_INSTS];
+	*bvhs = p->slab + p->off[SEC_BVHS]; *bvh_bytes = p->len[SEC_BVHS];
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_prepared_slab(const crgpu_prepared *p, const void **slab, size_t *bytes) {
 	if (!p) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (slab) *slab = p->slab;
@@ -775,6 +785,7 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	if (herr.code) { return pfail(p, fail(herr.code, "%s", herr.msg)); }
 
 	/* instances */
+	if (f->instance_count > CRG_ITEM_INDEX + 1u) { return pfail(p, fail(CRGPU_ERR_UNSUPPORTED, "more than 2^30 instances")); }
 	std::vector<DevInstance> insts(f->instance_count);
 	for (uint32_t i = 0; i < f->instance_count; ++i) {
 		const crs_instance &src = f->instances[i];
@@ -853,6 +864,9 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	}
 	p->top = bvhs[f->top_bvh];
 	p->stage_pairs = (uint32_t)stage.size();
+	/* the instance step's record of every top-level leaf item (the staging above has set every stage_count) */
+	std::vector<DevTopItem> items(top_prims.size());
+	for (size_t i = 0; i < top_prims.size(); ++i) items[i] = crg_top_item(insts[top_prims[i]], bvhs.data(), (uint32_t)top_prims[i]);
 	{	/* world bounds = bounds of the top-level BVH root (both children of pair 0, or the single leaf's box) */
 		float lo[3] = { 0.f, 0.f, 0.f }, hi[3] = { 1.f, 1.f, 1.f };
 		const crs_bvh &tb = f->bvhs[f->top_bvh];
@@ -892,10 +906,10 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	for (int i = 0; i < 256; ++i) { volatile float num = (float)i, den = 255.0f; lut[i] = num / den; }   /* IEEE divss == __fdiv_rn */
 
 	/* lay the sections out in one slab (256-byte aligned each) and copy them in on the host threads */
-	const void *src[SEC_COUNT] = { stage.data(), pairs.data(), tris.data(), slot_poly.data(), keys.data(), spolys.data(), top_prims.data(), bvhs.data(),
+	const void *src[SEC_COUNT] = { stage.data(), pairs.data(), tris.data(), slot_poly.data(), keys.data(), spolys.data(), items.data(), bvhs.data(),
 								   insts.data(), mats.data(), flat.data(), order.data(), nodes.data(), texs.data(), lut.data(), f->texdata };
 	const size_t len[SEC_COUNT] = { stage.size() * sizeof(PairNode), pairs.size() * sizeof(PairNode), tris.size() * sizeof(PackedTri),
-									slot_poly.size() * sizeof(uint32_t), keys.size(), spolys.size() * sizeof(ShadePoly), top_prims.size() * sizeof(int32_t),
+									slot_poly.size() * sizeof(uint32_t), keys.size(), spolys.size() * sizeof(ShadePoly), items.size() * sizeof(DevTopItem),
 									bvhs.size() * sizeof(DevBvh), insts.size() * sizeof(DevInstance), mats.size() * sizeof(DevMaterial),
 									flat.size() * sizeof(DevFlat), order.size(), nodes.size() * sizeof(crs_node), texs.size() * sizeof(DevTexture), lut.size() * sizeof(float), (size_t)f->texdata_bytes };
 	size_t total = 0;
@@ -990,7 +1004,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	d.slot_key = reinterpret_cast<const uint8_t *>(base + p->off[SEC_KEYS]);
 	d.inst_key = d.slot_key + p->key_inst_off;
 	d.spolys = reinterpret_cast<const ShadePoly *>(base + p->off[SEC_SPOLYS]);
-	d.top_prims = reinterpret_cast<const int32_t *>(base + p->off[SEC_TOP_PRIMS]);
+	d.top_items = reinterpret_cast<const DevTopItem *>(base + p->off[SEC_TOP_ITEMS]);
 	d.bvhs = reinterpret_cast<const DevBvh *>(base + p->off[SEC_BVHS]);
 	d.instances = reinterpret_cast<const DevInstance *>(base + p->off[SEC_INSTS]);
 	d.materials = reinterpret_cast<const DevMaterial *>(base + p->off[SEC_MATS]);
@@ -1360,7 +1374,8 @@ extern "C" int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *c
 }
 
 /* Instance boxes, ray offsets and the top-level BVH of the edited instances are computed on the device, into scratch; only once the
- * build has passed the upload's checks are they copied over the scene's instances, top region, top_prims and staged prefix. */
+ * build has passed the upload's checks are they copied over the scene's instances, top region and staged prefix, and the top-level
+ * item records rebuilt from them. */
 extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
 	if (!s || !inst) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	const uint32_t n = (uint32_t)s->inst_kind.size();
@@ -1383,8 +1398,8 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	cudaStream_t st = s->stream;
 	if (!s->edit) {
 		/* the scene's own pairs block: the uploaded pairs (mesh pair offsets do not move), then a top region that holds any top level
-		 * of n instances, then top_prims; the uploaded top level keeps rendering until an edit is committed */
-		const size_t edit_bytes = align(pairs_bytes + top_bytes) + (size_t)n * 4u;
+		 * of n instances, then its n item records; the uploaded top level keeps rendering until an edit is committed */
+		const size_t edit_bytes = align(pairs_bytes + top_bytes) + (size_t)n * sizeof(DevTopItem);
 		void *e = nullptr, *q = nullptr;
 		rc = ctx_alloc(s->device, edit_bytes, &e);
 		if (!rc) rc = ctx_alloc(s->device, total, &q);
@@ -1429,15 +1444,16 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	t.stage_base = s->dev.top.stage_base;
 	t.stage_count = res.pairs < s->top_stage_cap ? res.pairs : s->top_stage_cap;
 	PairNode *top_pairs = static_cast<PairNode *>(s->edit) + s->pair_count;          /* = pairs + t.pair_offset */
-	int32_t *top_prims = reinterpret_cast<int32_t *>(static_cast<uint8_t *>(s->edit) + align(pairs_bytes + top_bytes));
+	DevTopItem *top_items = reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->edit) + align(pairs_bytes + top_bytes));
 	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), new_insts, sz[6], cudaMemcpyDeviceToDevice, st));
 	if (res.pairs) CU(cudaMemcpyAsync(top_pairs, new_pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	CU(cudaMemcpyAsync(top_prims, new_prims, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
+	crg_launch_top_items(new_prims, new_insts, s->dev.bvhs, n, top_items, st);
+	CU(cudaGetLastError());
 	if (t.stage_count)
 		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + t.stage_base, new_pairs, (size_t)t.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	s->dev.top = t;
 	s->dev.pairs = reinterpret_cast<const PairNode *>(s->edit);
-	s->dev.top_prims = top_prims;
+	s->dev.top_items = top_items;
 	for (int k = 0; k < 3; ++k) {            /* as crgpu_prepare: the root's bounds */
 		const float lo = res.bounds[2 * k], e = res.bounds[2 * k + 1] - lo;
 		s->dev.world_lo[k] = lo;

@@ -632,3 +632,13 @@ void crg_launch_instance_boxes(const crs_instance *inst, DevInstance *insts, con
 	k_instance_boxes<<<(n + 255u) / 256u, 256, 0, st>>>(inst, insts, bvh_root, n, bb, ctr, offs);
 	k_instance_offsets<<<(n + 255u) / 256u, 256, 0, st>>>(insts, last, offs, n);
 }
+
+/* the edit's item records, from the committed instances' new state and the mesh BVHs (which an instance edit never moves) */
+__global__ void k_top_items(const int32_t *__restrict__ prims, const DevInstance *__restrict__ insts, const DevBvh *__restrict__ bvhs, uint32_t n,
+                            DevTopItem *__restrict__ items) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) items[i] = crg_top_item(insts[prims[i]], bvhs, (uint32_t)prims[i]);
+}
+void crg_launch_top_items(const int32_t *prims, const DevInstance *insts, const DevBvh *bvhs, uint32_t n, DevTopItem *items, cudaStream_t st) {
+	if (n) k_top_items<<<(n + 255u) / 256u, 256, 0, st>>>(prims, insts, bvhs, n, items);
+}

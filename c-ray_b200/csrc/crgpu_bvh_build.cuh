@@ -32,3 +32,6 @@ CRG_WEAK int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, vo
  * its object (last[i]).  bvh_root: 6 floats per BVH, the root bounds of each mesh BVH as stored. */
 CRG_WEAK void crg_launch_instance_boxes(const crs_instance *inst, DevInstance *insts, const float *bvh_root, const uint32_t *last, uint32_t n,
 							   float *bb, float *ctr, float *offs, cudaStream_t st);
+
+/* the top level's item records (DevTopItem) for the edited instances: item i describes instance prims[i] of insts (device, n each) */
+CRG_WEAK void crg_launch_top_items(const int32_t *prims, const DevInstance *insts, const DevBvh *bvhs, uint32_t n, DevTopItem *items, cudaStream_t st);

@@ -22,6 +22,7 @@
 #define CRG_XNODE_DEPTH 8     /* edges below the first node of a kind only the complete interpreter knows (NodeX: SURVEY 8 f4) */
 #define CRG_ADD_STACK 4       /* operand stack of nested ADD bsdfs */
 #include <stdint.h>
+#include <string.h>
 #include "../../include/crscene.h"
 
 #define CRG_LEAF_BIT 0x80000000u
@@ -51,7 +52,7 @@ struct DevBvh {
 	uint32_t pair_offset;           /* into pairs[] */
 	uint32_t pair_end;              /* one past this BVH's last pair node */
 	uint32_t node_count;            /* reference nodeCount (0, 1 or >1 select the code path, bvh.c:362-387) */
-	uint32_t slot_offset;           /* into tris[] / slot_poly[] (mesh) or top_prims[] (top level) */
+	uint32_t slot_offset;           /* into tris[] / slot_poly[] (mesh) or top_items[] (top level) */
 	uint32_t root_first, root_count;/* when node_count == 1: the root is a leaf */
 	float    root_bounds[6];
 	uint32_t stage_base;            /* the first stage_count pair nodes (BFS order = top of the tree) of this BVH are also */
@@ -69,6 +70,41 @@ struct __align__(16) DevInstance {
 	uint32_t material;              /* sphere: global material index */
 	uint32_t pad[3];
 };
+
+/* One top-level leaf item (DevScene::top_items, indexed like the top level's primIndices: top.slot_offset + item): what the
+ * traversal's instance step reads, in one 64-byte record it fetches with four 16-byte loads instead of three dependent lookups
+ * (primIndices, then the instance, then its mesh's DevBvh).  Only a mesh whose BVH has at most one node, or staged nodes, still
+ * sends the step to bvhs[instances[i].bvh].  crgpu_prepare builds the records from the uploaded scene, an instance edit
+ * (crgpu_scene_set_instances) rebuilds them on the device with k_top_items; both call crg_top_item. */
+#define CRG_ITEM_MESH  0x80000000u  /* bits of DevTopItem::inst above the instance index */
+#define CRG_ITEM_BVH   0x40000000u  /* a mesh whose BVH has node_count <= 1 or stage_count > 0 */
+#define CRG_ITEM_INDEX 0x3fffffffu
+struct __align__(16) DevTopItem {
+	float Ainv[12];                 /* the instance's */
+	uint32_t inst;                  /* instance index | CRG_ITEM_MESH | CRG_ITEM_BVH */
+	float    ray_offset;            /* the instance's */
+	uint32_t shape;                 /* sphere: radius (float bits); mesh: its BVH's pair_offset */
+	uint32_t slot_offset;           /* mesh: its BVH's slot_offset; sphere: 0 */
+};
+static_assert(sizeof(DevTopItem) == 64, "DevTopItem is one 64-byte record");
+
+__host__ __device__ inline DevTopItem crg_top_item(const DevInstance &in, const DevBvh *bvhs, uint32_t inst) {
+	DevTopItem t;
+	for (int k = 0; k < 12; ++k) t.Ainv[k] = in.Ainv[k];
+	t.inst = inst;
+	t.ray_offset = in.ray_offset;
+	t.shape = 0u;
+	t.slot_offset = 0u;
+	if (in.kind == CRS_INST_MESH) {
+		const DevBvh &b = bvhs[in.bvh];
+		t.inst |= CRG_ITEM_MESH | (b.node_count <= 1u || b.stage_count ? CRG_ITEM_BVH : 0u);
+		t.shape = b.pair_offset;
+		t.slot_offset = b.slot_offset;
+	} else {
+		memcpy(&t.shape, &in.radius, sizeof t.shape);
+	}
+	return t;
+}
 
 struct DevMaterial {
 	float emission[3];
@@ -142,7 +178,7 @@ struct DevScene {
 	const uint8_t    *slot_key;     /* prim slot -> shading key min(material + 1, 255) of its poly (K2's write-back: one load per hit) */
 	const uint8_t    *inst_key;     /* instance -> shading key of a sphere instance (0 for meshes) */
 	const ShadePoly  *spolys;
-	const int32_t    *top_prims;    /* top-level primIndices (instance indices) */
+	const DevTopItem *top_items;    /* one record per top-level primIndices entry (DevTopItem) */
 	const DevBvh     *bvhs;
 	const DevInstance*instances;
 	const DevMaterial*materials;

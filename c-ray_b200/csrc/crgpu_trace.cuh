@@ -128,12 +128,16 @@ CRD bool cr_node_test(const float *b, v3 invDir, v3 scaledStart, unsigned bits, 
 		if (deg & 2u) { const bool in = (b[2] <= o.y) && (o.y <= b[3]); tMinY = in ? -inf : inf; tMaxY = in ? inf : -inf; }
 		if (deg & 4u) { const bool in = (b[4] <= o.z) && (o.z <= b[5]); tMinZ = in ? -inf : inf; tMaxZ = in ? inf : -inf; }
 	}
-	float tMin = tMinX > tMinY ? tMinX : tMinY;
-	float tMax = tMaxX < tMaxY ? tMaxX : tMaxY;
-	tMin = tMin > tMinZ ? tMin : tMinZ;
-	tMax = tMax < tMaxZ ? tMax : tMaxZ;
-	tMin = tMin > 0 ? tMin : 0;
-	tMax = tMax < maxDist ? tMax : maxDist;
+	/* bvh.c:341-348 is a chain of `a > b ? a : b` (FSETP + FSEL each); fmaxf / fminf (one FMNMX) give the same value here.  No
+	 * operand is NaN: an axis whose -o/d is not finite was replaced by +-inf above, and on every other axis 1/d and -o/d are
+	 * finite, so b * (1/d) + (-o/d) is finite or +-inf for finite bounds.  The two forms can differ only in the sign of a zero
+	 * (-0 against +0), and a zero's sign decides nothing below: tMin <= tMax and the caller's tL > tR compare -0 and +0 equal. */
+	float tMin = fmaxf(tMinX, tMinY);
+	float tMax = fminf(tMaxX, tMaxY);
+	tMin = fmaxf(tMin, tMinZ);
+	tMax = fminf(tMax, tMaxZ);
+	tMin = fmaxf(tMin, 0.0f);
+	tMax = fminf(tMax, maxDist);
 	tEntry = tMin;
 	return tMin <= tMax;
 }
@@ -215,7 +219,9 @@ CRD void cr_object_ray(const float *Ainv, float ray_offset, v3 o, v3 d, v3 &oo, 
  *   - the top CRG_SSTACK entries of the traversal stack (deeper entries spill to a thread-local array that is touched only
  *     when a lane's stack is that deep);
  *   - cold state: the world ray (read by an instance step and on the way back from a mesh), u, v, prim slot and instance of the
- *     closest hit (written on a hit, read at write-back), the top-level node to resume after a mesh and the mesh's instance.
+ *     closest hit (written on a hit, read at write-back), the top-level node to resume after a mesh and the mesh's instance;
+ *   - the range of the current BVH's nodes that the block staged (CRGPU_TRACE_STAGE), read by a node step only when the block
+ *     staged any: as two registers it cost the unstaged default 1.5% of the frame in spills (DESIGN §4).
  * Every kernel that runs a Traversal has at most CRG_TRAV_NT threads per block. */
 #define CRG_SSTACK  8
 #define CRG_OVF     (2 * CRG_MAX_STACK + 2)   /* capacity of the whole stack: CRG_MAX_STACK entries per level */
@@ -228,6 +234,8 @@ struct TravShared {
 	uint32_t prim[CRG_TRAV_NT];                     /* its global prim slot (a triangle) */
 	int inst[CRG_TRAV_NT];                          /* its instance, -1 = miss */
 	uint32_t topNext[CRG_TRAV_NT];                  /* top-level node to resume when the current mesh is exhausted */
+	uint32_t stageBase[CRG_TRAV_NT], stageCount[CRG_TRAV_NT];   /* CRG_TF_STAGED: nodes [0, stageCount) of the current BVH are
+	                                                   at crg_stage_smem[stageBase + node] */
 	int curInst[CRG_TRAV_NT];                       /* the mesh instance being traversed */
 };
 
@@ -248,7 +256,6 @@ struct Traversal {
 	v3 invDir, scaledStart;/* its slab setup (RaySetup); the sign and degenerate-axis bits are in flags */
 	uint32_t flags;        /* CRG_RS_* | CRG_TF_* */
 	uint32_t pairOff;      /* first pair node of the current BVH in sc.pairs */
-	uint32_t stageBase, stageCount;/* nodes [0, stageCount) of the current BVH live at crg_stage_smem[stageBase + node]; 0 when not staged */
 	uint32_t slotBase, node;
 	uint32_t pendA, cntA, pendB, cntB;     /* pending top-level leaf items: A (left leaf) before B (right leaf) */
 	uint32_t leafA, leafB, leafN;          /* DEFER: bottom-level leaf triangles not yet tested — slots [leafA, +nA) then [leafB, +nB), leafN = nA | nB << 16 */
@@ -279,9 +286,10 @@ struct Traversal {
 		invDir = rs.invDir; scaledStart = rs.scaledStart;
 		flags = (flags & ~CRG_RS_MASK) | rs.bits;
 	}
+	CRD void set_stage(uint32_t base, uint32_t count) { sh().stageBase[tid()] = base; sh().stageCount[tid()] = count; }
 	CRD void set_top(const DevScene &sc) {
 		pairOff = sc.top.pair_offset;
-		stageBase = sc.top.stage_base; stageCount = (flags & CRG_TF_STAGED) ? sc.top.stage_count : 0u;
+		if (flags & CRG_TF_STAGED) set_stage(sc.top.stage_base, sc.top.stage_count);
 	}
 
 	/* staged: the block holds DevScene.stage_img in crg_stage_smem */
@@ -364,8 +372,8 @@ struct Traversal {
 			/* ---- one child-pair step (bvh.c:391-439) */
 			float4 q0, q1, q2;
 			uint4 q3;
-			if (node < stageCount) {                     /* top of the tree: staged in shared memory by TMA */
-				const float4 *p4 = reinterpret_cast<const float4 *>(reinterpret_cast<const PairNode *>(crg_stage_smem) + stageBase + node);
+			if ((flags & CRG_TF_STAGED) && node < sh().stageCount[tid()]) {      /* top of the tree: staged in shared memory by TMA */
+				const float4 *p4 = reinterpret_cast<const float4 *>(reinterpret_cast<const PairNode *>(crg_stage_smem) + sh().stageBase[tid()] + node);
 				q0 = p4[0]; q1 = p4[1]; q2 = p4[2];
 				q3 = *reinterpret_cast<const uint4 *>(p4 + 3);
 			} else {
@@ -411,6 +419,21 @@ struct Traversal {
 		}
 	}
 
+	/* into the BVH of mesh instance `inst` (pair_offset, slot_offset) with its object-space ray; nothing of it staged */
+	CRD void enter_mesh(v3 oo, v3 od, uint32_t pair_offset, uint32_t slot_offset, int inst) {
+		TravShared &s = sh();
+		const unsigned t = tid();
+		flags = (flags | CRG_TF_BOTTOM) & ~CRG_TF_INSTHIT;
+		s.topNext[t] = node;
+		set_ray(oo, od);
+		pairOff = pair_offset;
+		if (flags & CRG_TF_STAGED) set_stage(0u, 0u);
+		slotBase = slot_offset;
+		s.curInst[t] = inst;
+		spBase = sp;
+		node = 0u;
+	}
+
 	/* precondition: wants_instance() */
 	CRD void instance_step(const DevScene &sc, TraceCounters *ctr) {
 		{
@@ -419,44 +442,39 @@ struct Traversal {
 			const unsigned t = tid();
 			uint32_t idx;
 			if (cntA) { idx = pendA++; --cntA; } else { idx = pendB++; --cntB; }
-			const int cur = __ldg(sc.top_prims + sc.top.slot_offset + idx);
-			const DevInstance *inst = sc.instances + cur;
-			const float4 *m4 = reinterpret_cast<const float4 *>(inst->Ainv);
+			const float4 *m4 = reinterpret_cast<const float4 *>(sc.top_items + sc.top.slot_offset + idx);    /* one DevTopItem */
 			const float4 r0 = __ldg(m4 + 0), r1 = __ldg(m4 + 1), r2 = __ldg(m4 + 2);
 			const float Ainv[12] = { r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w, r2.x, r2.y, r2.z, r2.w };
-			const uint4 meta = __ldg(reinterpret_cast<const uint4 *>(&inst->kind));    /* kind, bvh, ray_offset, radius */
+			const uint4 meta = __ldg(reinterpret_cast<const uint4 *>(m4 + 3));    /* inst | CRG_ITEM_*, ray_offset, shape, slot_offset */
+			const int cur = (int)(meta.x & CRG_ITEM_INDEX);
 			v3 oo, od;
-			cr_object_ray(Ainv, __uint_as_float(meta.z), v3make(s.wo[0][t], s.wo[1][t], s.wo[2][t]), v3make(s.wd[0][t], s.wd[1][t], s.wd[2][t]), oo, od);
-			if (meta.x == CRS_INST_MESH) {                                         /* instance.c:169-175 */
+			cr_object_ray(Ainv, __uint_as_float(meta.y), v3make(s.wo[0][t], s.wo[1][t], s.wo[2][t]), v3make(s.wd[0][t], s.wd[1][t], s.wd[2][t]), oo, od);
+			if (meta.x & CRG_ITEM_MESH) {                                          /* instance.c:169-175 */
 				if (COUNT) ctr->insts++;
-				const DevBvh *bvh = sc.bvhs + meta.y;
-				const uint32_t nodeCount = __ldg(&bvh->node_count);
-				const uint32_t slotOff = __ldg(&bvh->slot_offset);
-				if (nodeCount < 1u) {
-					s.inst[t] = -1;                                                /* bvh.c:362-365 quirk */
-				} else if (nodeCount == 1u) {                                      /* bvh.c:382-387 */
-					const RaySetup ors = cr_ray_setup(oo, od);
-					float rbnd[6], te;
-					for (int k = 0; k < 6; ++k) rbnd[k] = __ldg(&bvh->root_bounds[k]);
-					if (cr_node_test(rbnd, ors.invDir, ors.scaledStart, ors.bits, oo, bestT, te))
-						if (cr_leaf_tris<COUNT>(sc, slotOff, __ldg(&bvh->root_first), __ldg(&bvh->root_count), 0u, 0u, oo, od, bestT, s.u[t], s.v[t], s.prim[t], ctr)) {
-							s.inst[t] = cur;
-							flags &= ~CRG_TF_SPHERE;
-						}
+				if (!(meta.x & CRG_ITEM_BVH)) {
+					enter_mesh(oo, od, meta.z, meta.w, cur);                       /* the common mesh: nothing beyond the record */
 				} else {
-					flags = (flags | CRG_TF_BOTTOM) & ~CRG_TF_INSTHIT;
-					s.topNext[t] = node;
-					set_ray(oo, od);
-					pairOff = __ldg(&bvh->pair_offset);
-					stageBase = __ldg(&bvh->stage_base); stageCount = (flags & CRG_TF_STAGED) ? __ldg(&bvh->stage_count) : 0u;
-					slotBase = slotOff;
-					s.curInst[t] = cur;
-					spBase = sp;
-					node = 0u;
+					const DevBvh *bvh = sc.bvhs + __ldg(&sc.instances[cur].bvh);
+					const uint32_t nodeCount = __ldg(&bvh->node_count);
+					if (nodeCount < 1u) {
+						s.inst[t] = -1;                                            /* bvh.c:362-365 quirk */
+					} else if (nodeCount == 1u) {                                  /* bvh.c:382-387 */
+						const RaySetup ors = cr_ray_setup(oo, od);
+						float rbnd[6], te;
+						for (int k = 0; k < 6; ++k) rbnd[k] = __ldg(&bvh->root_bounds[k]);
+						if (cr_node_test(rbnd, ors.invDir, ors.scaledStart, ors.bits, oo, bestT, te))
+							if (cr_leaf_tris<COUNT>(sc, meta.w, __ldg(&bvh->root_first), __ldg(&bvh->root_count), 0u, 0u, oo, od, bestT, s.u[t], s.v[t], s.prim[t], ctr)) {
+								s.inst[t] = cur;
+								flags &= ~CRG_TF_SPHERE;
+							}
+					} else {                                                       /* a mesh with staged nodes */
+						enter_mesh(oo, od, meta.z, meta.w, cur);
+						if (flags & CRG_TF_STAGED) set_stage(__ldg(&bvh->stage_base), __ldg(&bvh->stage_count));
+					}
 				}
 			} else {                                                               /* instance.c:45-51 */
 				if (COUNT) ctr->spheres++;
-				if (cr_sphere_test(oo, od, __uint_as_float(meta.w), bestT)) { s.inst[t] = cur; flags |= CRG_TF_SPHERE; }
+				if (cr_sphere_test(oo, od, __uint_as_float(meta.z), bestT)) { s.inst[t] = cur; flags |= CRG_TF_SPHERE; }
 			}
 		}
 	}

@@ -89,6 +89,12 @@ int  crgpu_prepared_materials(const crgpu_prepared *p, uint32_t *kinds, uint32_t
 /* How the miss launch will sample the background: *kind = 0 through the node interpreter, else folded at upload with a constant
  * strength and offset over a 1 constant, 2 image or 3 gradient colour. */
 int  crgpu_prepared_background(const crgpu_prepared *p, uint32_t *kind);
+/* The slab sections the traversal's instance step reads, valid while p lives: one 64-byte record per top-level primIndices entry
+ * (the instance's Ainv rows as 12 floats; its index | 1 << 31 for a mesh | 1 << 30 when the step must read the mesh's BVH record,
+ * which is when that BVH has at most one node or staged nodes; its ray offset; a sphere's radius or a mesh BVH's pair offset; a mesh
+ * BVH's slot offset), and the instance (128 B) and BVH (60 B) records they are built from.  Lengths in bytes. */
+int  crgpu_prepared_top_level(const crgpu_prepared *p, const void **items, size_t *item_bytes, const void **instances,
+                              size_t *instance_bytes, const void **bvhs, size_t *bvh_bytes);
 int  crgpu_scene_create_prepared(const crgpu_prepared *p, int device, crgpu_scene **out);
 
 /* Device memory released by crgpu_scene_destroy is kept in a per-device cache for the next scene (a frame's 35 GB of
