@@ -15,6 +15,7 @@ FLAG_COUNT = 0x1
 FLAG_TIME_KERNELS = 0x2
 FLAG_ASYNC = 0x4
 STOPPED = 1          # CRGPU_STOPPED: an armed render call ended at a pass boundary because a stop was requested
+PENDING = 2          # CRGPU_PENDING: the snapshot asked for has not been staged yet
 
 
 class Prefs(C.Structure):
@@ -131,8 +132,13 @@ def lib():
                   "crgpu_shade_rays", "crgpu_libm_eval", "crgpu_prepared_background",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
                   "crgpu_stop_enable", "crgpu_request_stop", "crgpu_clear_stop", "crgpu_progress",
+
                   "crgpu_scene_set_camera", "crgpu_scene_set_instances", "crscene_set_config"):
             getattr(L, f).restype = C.c_int
+        if hasattr(L, "crgpu_take_snapshot"):      # absent from libraries built before snapshots (tools/driver_check.py compares builds)
+            L.crgpu_request_snapshot.argtypes = [P]
+            L.crgpu_take_snapshot.argtypes = [P, P, C.POINTER(C.c_int)]
+            L.crgpu_request_snapshot.restype = L.crgpu_take_snapshot.restype = C.c_int
         _lib = L
     return _lib
 
@@ -233,6 +239,21 @@ class GpuScene:
         done, busy = C.c_int(0), C.c_int(0)
         _check(lib().crgpu_progress(self.handle, C.byref(done), C.byref(busy)), "crgpu_progress")
         return done.value, bool(busy.value)
+
+    def request_snapshot(self):
+        """Ask the next publish step of the call in flight to stage the image (crgpu_request_snapshot); any thread may call it."""
+        _check(lib().crgpu_request_snapshot(self.handle), "crgpu_request_snapshot")
+
+    def take_snapshot(self):
+        """(uint8 [H, W, 3] sRGB image, passes_done) once the requested image is staged, or with no call in flight the framebuffer
+        as it is; None while the snapshot is pending.  Never waits for the render."""
+        out = np.empty((self.H, self.W, 3), dtype=np.uint8)
+        done = C.c_int(0)
+        rc = lib().crgpu_take_snapshot(self.handle, out.ctypes.data, C.byref(done))
+        if rc == PENDING:
+            return None
+        _check(rc, "crgpu_take_snapshot")
+        return out, done.value
 
     def set_camera(self, camera):
         """Move the camera of the resident scene (crgpu_scene_set_camera): a Camera of the scene's image size, taken bit for bit."""

@@ -59,6 +59,8 @@ def lib():
         L.crhostSetPaused.restype = None
         L.crhostProgress.argtypes = [P, C.POINTER(C.c_ulonglong)]
         L.crhostWorkerPasses.argtypes = [P, C.c_int]
+        L.crhostCurrentImage.argtypes = [P, P]
+        L.crhostCurrentImagePasses.argtypes = [P, P, P, C.c_int]
         _lib = L
     return _lib
 
@@ -126,6 +128,14 @@ class Renderer:
     def worker_passes(self, t):
         """passes worker t has committed in the current (or last) frame: its tiles hold exactly passes [0, that)"""
         return int(lib().crhostWorkerPasses(self.r, t))
+
+    def current_image(self, workers=0):
+        """(whether a frame renders, uint8 [H, W, 3] image of the frame as it stands (crhostCurrentImage), and with workers > 0
+        the pass count each of the first `workers` workers' tiles show, read together with the image)"""
+        img = np.empty((self.H, self.W, 3), dtype=np.uint8)
+        passes = np.zeros(max(workers, 1), dtype=np.int32)
+        busy = lib().crhostCurrentImagePasses(self.r, img.ctypes.data, passes.ctypes.data if workers else None, workers)
+        return bool(busy), img, passes[:workers].tolist()
 
     def rank_tiles(self, rank, world):
         """(rects (n,4) int32, owner (tileCount,) int32, all_rects (tileCount,4)): this rank's share of the tile queue as the C

@@ -195,8 +195,12 @@ struct crgpu_scene {
 	size_t pixel_cap;
 	std::vector<int> pixel_key;
 	bool armed;                /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
-	unsigned *stop_host;       /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight (NULL until armed once) */
-	unsigned *stop_ctl;        /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets */
+	unsigned *stop_host;       /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight, [3] snapshot state
+	                              (0 idle, 1 requested, 2 staged), [4] its pass index (NULL until armed once) */
+	unsigned *stop_ctl;        /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets,
+	                              [3] the next publish step stages a snapshot, [4] its block count (crgpu_wave.cuh) */
+	uint8_t *snap8;            /* W*H*3 sRGB8 snapshot staged by a publish step (allocated by the first armed call) */
+	cudaStream_t snap_stream;  /* crgpu_take_snapshot's copies: never behind the render (created when first armed) */
 	/* instance edits (crgpu_scene_set_instances) */
 	std::vector<uint32_t> inst_kind, inst_object;    /* as uploaded: an edit must keep them */
 	std::vector<float> bvh_root;                     /* crgpu_prepared::bvh_root */
@@ -560,6 +564,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->small, s->small_bytes);
 	ctx_free(s->device, s->fb, s->fb_floats * sizeof(float));
 	ctx_free(s->device, s->fb8, s->fb_floats);
+	ctx_free(s->device, s->snap8, s->fb_floats);
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
 	ctx_free(s->device, s->edit, s->edit_bytes);
 	ctx_free(s->device, s->edit_scratch, s->edit_scratch_bytes);
@@ -568,6 +573,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	if (s->evFork) cudaEventDestroy(s->evFork);
 	if (s->stream2) cudaStreamDestroy(s->stream2);
 	if (s->own_stream) cudaStreamDestroy(s->own_stream);
+	if (s->snap_stream) cudaStreamDestroy(s->snap_stream);
 	if (s->stop_host) cudaFreeHost(s->stop_host);
 	delete s;
 	return CRGPU_OK;
@@ -952,7 +958,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	memset(&s->wb2, 0, sizeof s->wb2);
 	s->wave_sets = 0; s->stream2 = nullptr; s->evAcc[0] = s->evAcc[1] = nullptr; s->evFork = nullptr;
 	s->pixels = nullptr; s->pixel_cap = 0;
-	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr;
+	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr; s->snap8 = nullptr; s->snap_stream = nullptr;
 	s->inst_kind = p->inst_kind; s->inst_object = p->inst_object; s->bvh_root = p->bvh_root;
 	s->pair_count = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode)); s->top_stage_cap = p->top.stage_count;
 	s->edit = nullptr; s->edit_bytes = 0; s->edit_scratch = nullptr; s->edit_scratch_bytes = 0;
@@ -1222,9 +1228,11 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 			cur ^= 1;
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
-		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set); ++launches;
-		if (armed && gates.publish) {
-			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats, st);
+		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set,
+		                      armed && gates.publish ? s->stop_host : nullptr); ++launches;
+		if (armed && gates.publish) {       /* stages a snapshot when K5 found one requested (crgpu_request_snapshot) */
+			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats,
+			                        s->fb, s->snap8, s->fb_floats, s->sm_count * 4, st);
 			++launches;
 		}
 		if (sets == 2) CU(cudaEventRecord(s->evAcc[set], st));      /* after the publish step: the next K5 reads what it wrote */
@@ -1280,6 +1288,13 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
 	const bool armed = s->armed;
+	if (armed && !s->snap8) {
+		CU(cudaSetDevice(s->device));
+		void *q = nullptr;
+		int arc = ctx_alloc(s->device, s->fb_floats, &q);
+		if (arc) return arc;
+		s->snap8 = static_cast<uint8_t *>(q);
+	}
 	if (armed) {
 		__atomic_store_n(&s->stop_host[1], (unsigned)pass_begin, __ATOMIC_RELEASE);
 		__atomic_store_n(&s->stop_host[2], 1u, __ATOMIC_RELEASE);
@@ -1331,6 +1346,7 @@ extern "C" int crgpu_stop_enable(crgpu_scene *s, int on) {
 		CU(cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable));   /* unified addressing: the same pointer on the device */
 		s->stop_host = static_cast<unsigned *>(p);
 	}
+	if (on && !s->snap_stream) CU(cudaStreamCreateWithFlags(&s->snap_stream, cudaStreamNonBlocking));
 	if (on) for (int k = 0; k < 16; ++k) __atomic_store_n(&s->stop_host[k], 0u, __ATOMIC_RELEASE);
 	s->armed = on != 0;
 	return CRGPU_OK;
@@ -1352,6 +1368,36 @@ extern "C" int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy) {
 	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
 	if (passes_done) *passes_done = (int)__atomic_load_n(&s->stop_host[1], __ATOMIC_ACQUIRE);
 	if (busy) *busy = (int)__atomic_load_n(&s->stop_host[2], __ATOMIC_ACQUIRE);
+	return CRGPU_OK;
+}
+
+/* Snapshots: host word [3] goes 0 (idle) -> 1 (requested, by the host) -> 2 (staged, by a publish step) -> 0 (taken, by the host).
+ * Only the host leaves 2, so the device never writes the staging buffer while crgpu_take_snapshot may be copying it. */
+extern "C" int crgpu_request_snapshot(crgpu_scene *s) {
+	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
+	unsigned idle = 0u;                    /* a request already made, or an image staged and not yet taken, stays as it is */
+	__atomic_compare_exchange_n(&s->stop_host[3], &idle, 1u, false, __ATOMIC_ACQ_REL, __ATOMIC_ACQUIRE);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done) {
+	if (!s || !s->armed) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL or not armed (crgpu_stop_enable)");
+	if (!host_rgb8) return fail(CRGPU_ERR_BAD_ARGUMENT, "host_rgb8 is NULL");
+	unsigned *w = s->stop_host;
+	CU(cudaSetDevice(s->device));
+	if (__atomic_load_n(&w[3], __ATOMIC_ACQUIRE) != 2u) {
+		if (__atomic_load_n(&w[2], __ATOMIC_ACQUIRE) != 0u) return CRGPU_PENDING;
+		/* no call in flight (k_stop_end clears the word after the call's last publish step): the framebuffer is the committed image */
+		int rc = crgpu_framebuffer_to_srgb8(s, host_rgb8);
+		if (rc) return rc;
+		if (passes_done) *passes_done = (int)__atomic_load_n(&w[1], __ATOMIC_ACQUIRE);
+		__atomic_store_n(&w[3], 0u, __ATOMIC_RELEASE);
+		return CRGPU_OK;
+	}
+	CU(cudaMemcpyAsync(host_rgb8, s->snap8, s->fb_floats, cudaMemcpyDeviceToHost, s->snap_stream));
+	CU(cudaStreamSynchronize(s->snap_stream));
+	if (passes_done) *passes_done = (int)__atomic_load_n(&w[4], __ATOMIC_ACQUIRE);
+	__atomic_store_n(&w[3], 0u, __ATOMIC_RELEASE);
 	return CRGPU_OK;
 }
 

@@ -190,3 +190,11 @@ CRD uint64_t cr_f2sz(float x) {
 	if (!(x < 18446744073709551616.0f)) return 0x8000000000000000ull ^ 0x8000000000000000ull;
 	return ((uint64_t)__float2ll_rz(x - 9223372036854775808.0f)) ^ 0x8000000000000000ull;
 }
+
+/* colorToSRGB + setPixel(char_p) of one channel: renderer.c:297-300, texture.c:19-21 */
+CRD uint8_t cr_to_srgb8(float v) {
+	const float c = cr_linear_to_srgb(v);
+	const float s = CR_MIN(c * 255.0f, 255.0f);
+	/* (unsigned char) of a negative/NaN float is UB in C; x86 cvttss2si + truncation gives the low byte */
+	return (uint8_t)(cr_f2i(s) & 0xff);
+}

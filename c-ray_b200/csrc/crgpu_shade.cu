@@ -322,10 +322,15 @@ __global__ void __launch_bounds__(128) k_tail(const DevScene *__restrict__ scp, 
 
 /* ---- K5 ------------------------------------------------------------------------------------------------------------------
  * ARMED (a stoppable scene): the batch is added only if its gates did not abandon it and the running average has reached exactly
- * its first pass — both written by earlier kernels in stream order, so every block takes the same decision. */
+ * its first pass — both written by earlier kernels in stream order, so every block takes the same decision.
+ * snap_host (a batch that publishes): one thread reads the snapshot state once and tells the publish step that follows whether to
+ * stage the image (gate[3]).  K5s run in pass order with a publish step between, so the state read here is what the previous
+ * publish step left. */
 template <bool ARMED>
 __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, const float4 *__restrict__ L, TileDesc td,
-													 int image_width, int image_height, const unsigned *__restrict__ gate, int set) {
+													 int image_width, int image_height, unsigned *__restrict__ gate, int set,
+													 const unsigned *__restrict__ snap_host) {
+	if (ARMED && snap_host && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = crg_ld_sys(snap_host + 3) == 1u ? 1u : 0u;
 	if (ARMED && (gate[1 + set] != 0u || gate[0] != (unsigned)td.pass_begin)) return;
 	const unsigned tile_pixels = td.npix;
 	for (unsigned px = blockIdx.x * blockDim.x + threadIdx.x; px < tile_pixels; px += gridDim.x * blockDim.x) {
@@ -346,12 +351,7 @@ __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, cons
 
 /* colorToSRGB + setPixel(char_p): renderer.c:297-300, texture.c:19-21 */
 __global__ void k_to_srgb8(const float *__restrict__ fb, uint8_t *__restrict__ out, size_t n) {
-	for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-		const float c = cr_linear_to_srgb(fb[i]);
-		const float s = CR_MIN(c * 255.0f, 255.0f);
-		/* (unsigned char) of a negative/NaN float is UB in C; x86 cvttss2si + truncation gives the low byte */
-		out[i] = (uint8_t)(cr_f2i(s) & 0xff);
-	}
+	for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) out[i] = cr_to_srgb8(fb[i]);
 }
 
 /* ---- known-answer kernel (parity tests): one thread per (x, y, pass) ---------------------------------------------------------- */
@@ -503,9 +503,10 @@ __global__ void k_libm(int fn, const float *__restrict__ x, const float *__restr
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st) {
 	k_libm<<<256, 256, 0, st>>>(fn, x, y, out, n);
 }
-void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st, const unsigned *gate, int set) {
-	if (gate) k_accumulate<true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set);
-	else k_accumulate<false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0);
+void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st, unsigned *gate, int set,
+                           const unsigned *snap_host) {
+	if (gate) k_accumulate<true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, snap_host);
+	else k_accumulate<false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr);
 }
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st) {
 	k_to_srgb8<<<grid, 256, 0, st>>>(fb, out, n);

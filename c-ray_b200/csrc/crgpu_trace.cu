@@ -190,16 +190,8 @@ void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDe
 	k_generate<<<grid, 256, 0, st>>>(sc, wb, td);
 }
 
-/* ---- stop gates of an armed scene (crgpu_wave.cuh): one thread each ------------------------------------------------------------
- * The host words are pinned, mapped memory: read and written at system scope, so a host store is seen by the next gate and
- * a published pass count by the host without any synchronisation. */
-__device__ __forceinline__ unsigned crg_ld_sys(const unsigned *p) {
-	unsigned v;
-	asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-	return v;
-}
-__device__ __forceinline__ void crg_st_sys(unsigned *p, unsigned v) { asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-
+/* ---- stop gates of an armed scene (crgpu_wave.cuh): one thread each, but for a publish step that stages a snapshot ------------------
+ * The host words are read and written at system scope (crg_ld_sys / crg_st_sys). */
 __global__ void k_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, const unsigned *host, int reset, int check) {
 	unsigned ab = reset ? 0u : ctl[1 + set];
 	if (!ab && check) ab = crg_ld_sys(host) != 0u ? 1u : 0u;
@@ -212,14 +204,32 @@ __global__ void k_stop_begin(unsigned *ctl, unsigned *host, int pass_begin) {
 	crg_st_sys(host + 2, 1u);
 	__threadfence_system();
 }
-__global__ void k_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
-                               unsigned long long *stats) {
-	if (ctl[1 + set] == 0u && ctl[0] == (unsigned)pass_begin) {       /* the decision K5 took */
-		ctl[0] = (unsigned)(pass_begin + pass_count);
-		stats[5] += paths;
+/* Block 0's thread 0 publishes.  A snapshot (ctl[3], decided by K5 from the host state) is the framebuffer as K5 left it: exactly
+ * the passes [call's pass_begin, ctl[0]).  The next K5 to write the framebuffer waits for this kernel in stream order, so the image
+ * holds no later batch.  The last block to finish stages it: the pass index first, then the state, so that a host that sees
+ * "staged" reads the index and image of this step, never one the progress word has not yet reached. */
+__global__ void __launch_bounds__(256) k_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count,
+                                                      unsigned long long paths, unsigned long long *stats, const float *__restrict__ fb,
+                                                      uint8_t *__restrict__ snap, size_t n) {
+	if (blockIdx.x == 0 && threadIdx.x == 0) {
+		if (ctl[1 + set] == 0u && ctl[0] == (unsigned)pass_begin) {       /* the decision K5 took */
+			ctl[0] = (unsigned)(pass_begin + pass_count);
+			stats[5] += paths;
+		}
+		crg_st_sys(host + 1, ctl[0]);
+		__threadfence_system();
 	}
-	crg_st_sys(host + 1, ctl[0]);
-	__threadfence_system();
+	if (ctl[3] == 0u) return;                                             /* no snapshot requested: the usual one-thread step */
+	for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) snap[i] = cr_to_srgb8(fb[i]);
+	__threadfence();
+	__syncthreads();
+	if (threadIdx.x == 0 && atomicAdd(&ctl[4], 1u) == gridDim.x - 1u) {
+		ctl[4] = 0u;
+		crg_st_sys(host + 4, *(volatile unsigned *)&ctl[0]);            /* block 0 wrote it before its count */
+		__threadfence_system();
+		crg_st_sys(host + 3, 2u);
+		__threadfence_system();
+	}
 }
 __global__ void k_stop_end(const unsigned *ctl, unsigned *host) {
 	crg_st_sys(host + 1, ctl[0]);
@@ -232,8 +242,8 @@ void crg_launch_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, con
 }
 void crg_launch_stop_begin(unsigned *ctl, unsigned *host, int pass_begin, cudaStream_t st) { k_stop_begin<<<1, 1, 0, st>>>(ctl, host, pass_begin); }
 void crg_launch_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
-                             unsigned long long *stats, cudaStream_t st) {
-	k_stop_publish<<<1, 1, 0, st>>>(ctl, set, host, pass_begin, pass_count, paths, stats);
+                             unsigned long long *stats, const float *fb, uint8_t *snap, size_t n, int grid, cudaStream_t st) {
+	k_stop_publish<<<grid, 256, 0, st>>>(ctl, set, host, pass_begin, pass_count, paths, stats, fb, snap, n);
 }
 void crg_launch_stop_end(unsigned *ctl, unsigned *host, cudaStream_t st) { k_stop_end<<<1, 1, 0, st>>>(ctl, host); }
 /* K2 is persistent: the grid is exactly the number of blocks the device can keep resident (the occupancy query below also

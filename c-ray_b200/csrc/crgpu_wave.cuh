@@ -53,6 +53,15 @@ struct WaveBuffers {
  * without: k_trace<false,3,0> 768 B / 186 B and 568 B / 110 B; K3's hit kernel (k_shade<2,2,false>) 416 B / 124 B and 304 B / 170 B. */
 template <class T> __device__ __forceinline__ T *crg_half(T *const (&a)[2], int h) { return h ? a[1] : a[0]; }
 
+/* The host words of an armed scene are pinned, mapped memory: read and written at system scope, so a host store is seen by the next
+ * kernel that reads it and a device store by the host without any synchronisation. */
+__device__ __forceinline__ unsigned crg_ld_sys(const unsigned *p) {
+	unsigned v;
+	asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+	return v;
+}
+__device__ __forceinline__ void crg_st_sys(unsigned *p, unsigned v) { asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+
 struct TileDesc {
 	int x0, y0, tw, th;     /* tile origin and size (pixels); y up */
 	int pass_begin, pass_count; /* this batch */
@@ -112,21 +121,26 @@ bool crg_shade_flat_order(const ShadeKnobs &kn);
 /* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
 /* gate: NULL, or the stop words of an armed scene (below): K5 then adds the batch only if wave set `set`'s batch was not abandoned
- * and the committed pass index equals td.pass_begin */
+ * and the committed pass index equals td.pass_begin.  snap_host: NULL, or (a batch that publishes) the host words, whose snapshot
+ * state K5 reads once into gate[3] for the publish step */
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st,
-                           const unsigned *gate = nullptr, int set = 0);
+                           unsigned *gate = nullptr, int set = 0, const unsigned *snap_host = nullptr);
 
 /* ---- stopping an armed scene at a pass boundary (crgpu_stop_enable) ----------------------------------------------------------------
  * ctl (device memory): [0] the pass index the running average has reached in this call, [1 + set] wave set `set`'s batch was
- * abandoned.  host (pinned, mapped): [0] stop request, [1] committed pass index (published), [2] a call is in flight.
+ * abandoned, [3] the publish step stages a snapshot (written by K5), [4] the publish step's count of finished blocks.
+ * host (pinned, mapped): [0] stop request, [1] committed pass index (published), [2] a call is in flight, [3] snapshot state
+ * (0 idle, 1 requested, 2 staged), [4] the pass index of the staged snapshot.
  * The gate runs after K1 and before every bounce; if the stop is requested (and `check`) it abandons the batch and leaves the wave
  * set as k_tail leaves it, so the rest of the batch's kernels run on zero rays.  `reset`: the first gate of a batch.  No kernel
  * waits for the host: pausing is the host's business. */
 void crg_launch_stop_gate(unsigned *counts, int cur, unsigned *ctl, int set, const unsigned *host, bool reset, bool check, cudaStream_t st);
 void crg_launch_stop_begin(unsigned *ctl, unsigned *host, int pass_begin, cudaStream_t st);
-/* after K5: advance ctl[0] past the batch if K5 added it (and count its paths in stats[5]), then publish ctl[0] */
+/* after K5: advance ctl[0] past the batch if K5 added it (and count its paths in stats[5]), then publish ctl[0].  When K5 found a
+ * snapshot requested (ctl[3]), the grid also converts the whole framebuffer fb (n floats) to sRGB8 into snap, and its last block
+ * publishes ctl[0] as the snapshot's pass index and sets the state to staged.  Otherwise every block but the first returns at once. */
 void crg_launch_stop_publish(unsigned *ctl, int set, unsigned *host, int pass_begin, int pass_count, unsigned long long paths,
-                             unsigned long long *stats, cudaStream_t st);
+                             unsigned long long *stats, const float *fb, uint8_t *snap, size_t n, int grid, cudaStream_t st);
 /* the call's last kernel: publish ctl[0] and clear the in-flight word */
 void crg_launch_stop_end(unsigned *ctl, unsigned *host, cudaStream_t st);
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st);

@@ -11,6 +11,7 @@
 #include "../../include/cray_api.h"
 #include "cr_host.h"
 #include <libgen.h>
+#include <pthread.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -18,6 +19,7 @@
 
 static struct renderer *g_renderer;
 static struct texture8 *g_image;
+static pthread_mutex_t g_image_lock = PTHREAD_MUTEX_INITIALIZER;   /* crGetCurrentImage may run while crStartRenderer renders */
 static char *g_asset_path;
 static struct crloader_output g_output;
 static bool g_antialiasing = true;
@@ -167,7 +169,9 @@ void crInitRenderer(void) {
 }
 
 void crDestroyRenderer(void) {
+	pthread_mutex_lock(&g_image_lock);
 	if (g_image) { destroyTexture8(g_image); g_image = NULL; }
+	pthread_mutex_unlock(&g_image_lock);
 	if (g_renderer) { destroyRenderer(g_renderer); g_renderer = NULL; }
 	free(g_asset_path); g_asset_path = NULL;
 }
@@ -211,12 +215,24 @@ int crLoadSceneFromFile(char *filePath) {
 
 void crStartRenderer(void) {
 	if (!g_renderer) return;
+	pthread_mutex_lock(&g_image_lock);
 	if (g_image) { destroyTexture8(g_image); g_image = NULL; }
-	g_image = renderFrame(g_renderer);                               /* c-ray.c:257 */
-	if (!g_image) fprintf(stderr, "[ERR ] render failed: %s\n", crgpu_last_error());
+	pthread_mutex_unlock(&g_image_lock);
+	struct texture8 *img = renderFrame(g_renderer);                  /* c-ray.c:257 */
+	if (!img) fprintf(stderr, "[ERR ] render failed: %s\n", crgpu_last_error());
+	pthread_mutex_lock(&g_image_lock);
+	if (g_image) destroyTexture8(g_image);                           /* taken by crGetCurrentImage during the frame */
+	g_image = img;
+	pthread_mutex_unlock(&g_image_lock);
 }
 
-void crWriteImage(void) {                                            /* c-ray.c:77-98, encoder.c:22-39 */
+static void write_image_locked(void);
+void crWriteImage(void) {
+	pthread_mutex_lock(&g_image_lock);
+	write_image_locked();
+	pthread_mutex_unlock(&g_image_lock);
+}
+static void write_image_locked(void) {                               /* c-ray.c:77-98, encoder.c:22-39 */
 	if (!g_image || !g_renderer) return;
 	char *path = NULL;
 	if (asprintf(&path, "%s%s_%04d.%s", g_renderer->prefs.imgFilePath, g_renderer->prefs.imgFileName, g_renderer->prefs.imgCount,
@@ -269,7 +285,21 @@ void crGetRenderOrder(void) { not_available("crGetRenderOrder"); }
 void crStartRenderWorker(void) { not_available("the network render worker (src/utils/protocol/worker.c)"); }
 void crStartInteractive(void) { not_available("crStartInteractive"); }
 void crPauseInteractive(void) { not_available("crPauseInteractive"); }
-void crGetCurrentImage(void) { not_available("crGetCurrentImage"); }
+/* "Just get the current buffer" (src/c-ray.h:97): the current image becomes the frame as it stands (crhostCurrentImage), from any
+ * thread, so that crWriteImage writes what a frame in flight shows at this moment */
+void crGetCurrentImage(void) {
+	if (!g_renderer || !g_renderer->prefs.imageWidth) return;
+	const unsigned W = g_renderer->prefs.imageWidth, H = g_renderer->prefs.imageHeight;
+	pthread_mutex_lock(&g_image_lock);
+	if (g_image && (g_image->width != W || g_image->height != H)) { destroyTexture8(g_image); g_image = NULL; }
+	if (!g_image) {
+		g_image = calloc(1, sizeof *g_image);
+		if (g_image) { g_image->width = W; g_image->height = H; g_image->data = malloc((size_t)W * H * 3); }
+		if (g_image && !g_image->data) { free(g_image); g_image = NULL; }
+	}
+	if (g_image) crhostCurrentImage(g_renderer, g_image->data);
+	pthread_mutex_unlock(&g_image_lock);
+}
 void crRestartInteractive(void) { }
 
 /* ---- additions ----------------------------------------------------------------------------------------------------- */

@@ -61,6 +61,7 @@ struct renderThreadState {         /* renderer.h:14-31 */
 	uint64_t rays;                 /* closest-hit queries traced by this worker */
 	int error;                     /* first CRGPU_ERR_* seen, 0 = none */
 	int tiles;                     /* tiles of this worker's share (the denominator of its progress) */
+	int previewPasses;             /* passes its tiles show in state.preview (under previewMutex) */
 };
 
 struct prefs {                     /* renderer.h:58-87 */
@@ -93,6 +94,11 @@ struct state {                     /* renderer.h:34-55 */
 	pthread_cond_t doneCond;
 	double renderSeconds;
 	uint64_t totalRays;
+	/* the live 8-bit image of the frame (W*H*3, the layout of struct texture8): blank when a frame starts, each worker's tiles
+	 * refreshed from GPU snapshots while it renders (gpuRenderThread), the final image once the frame is done */
+	uint8_t *preview;
+	size_t previewBytes;
+	pthread_mutex_t previewMutex;
 };
 
 struct renderer {
@@ -162,6 +168,17 @@ void crhostAbort(struct renderer *r, int save);
 void crhostSetPaused(struct renderer *r, int on);
 int crhostProgress(const struct renderer *r, unsigned long long *passes_done_total);
 int crhostWorkerPasses(const struct renderer *r, int t);
+/* The image of the frame as it stands, from any thread (crGetCurrentImage, reference src/c-ray.h:97): copies W*H*3 bytes into
+ * rgb8 and returns 1 while a frame renders, else 0 (the last frame's image, or blank before the first).  While a frame renders,
+ * each worker's tiles show the sRGB8 image of exactly the passes [0, k) it had committed at its latest snapshot; a worker takes
+ * one when its committed pass has advanced and CR_PREVIEW_INTERVAL_MS has passed since its previous one.  A rank of a
+ * one-process-per-GPU job shows its own tiles only, and only rank 0 (which receives the gathered frame) ends on the frame's
+ * image: another rank keeps its last snapshot of its own tiles.  The image always has the current image size: after a size
+ * change (applySceneConfig) it is blank until the next frame.  crhostCurrentImagePasses also gives, read under the same lock, the pass
+ * count k each worker's tiles show (passes[t] for t < min(workers, worker count)). */
+#define CR_PREVIEW_INTERVAL_MS 100
+int crhostCurrentImage(struct renderer *r, uint8_t *rgb8);
+int crhostCurrentImagePasses(struct renderer *r, uint8_t *rgb8, int *passes, int workers);
 
 /* worker entry point with the signature of renderThread (void *(*)(void *)) */
 void *gpuRenderThread(void *arg);

@@ -72,6 +72,7 @@ struct renderer *newRenderer(void) {                              /* renderer.c:
 	if (!r) return NULL;
 	pthread_mutex_init(&r->state.tileMutex, NULL);
 	pthread_mutex_init(&r->state.doneMutex, NULL);
+	pthread_mutex_init(&r->state.previewMutex, NULL);
 	pthread_cond_init(&r->state.doneCond, NULL);
 	r->prefs.threadCount = 1;
 	r->prefs.imgType = png;
@@ -133,6 +134,15 @@ static void free_render_buffer(struct renderer *r) {
 	r->state.renderBuffer = NULL;
 }
 
+/* the preview follows the image size: a blank W*H*3 image whenever the size changes (previewMutex held) */
+static void preview_resize_locked(struct renderer *r, size_t bytes) {
+	if (r->state.previewBytes == bytes) return;
+	free(r->state.preview);
+	r->state.preview = calloc(bytes ? bytes : 1, 1);
+	r->state.previewBytes = r->state.preview ? bytes : 0;
+	for (int t = 0; t < r->state.threadStateCount; ++t) r->state.threadStates[t].previewPasses = 0;
+}
+
 int applySceneConfig(struct renderer *r, int width, int height, int samples, int bounces) {
 	/* the part of loadScene (src/datatypes/scene.c:111-213) that follows parsing + BVH build */
 	crscene_set_config(&r->scene, width, height, samples, bounces);
@@ -149,6 +159,9 @@ int applySceneConfig(struct renderer *r, int width, int height, int samples, int
 	free(r->state.tileOwner);
 	r->state.tileOwner = calloc((size_t)r->state.tileCount + 1, sizeof(int));
 	free_render_buffer(r);
+	pthread_mutex_lock(&r->state.previewMutex);
+	preview_resize_locked(r, (size_t)r->prefs.imageWidth * r->prefs.imageHeight * 3u);
+	pthread_mutex_unlock(&r->state.previewMutex);
 	/* renderBuffer (scene.c:200): page-locked when a CUDA device is there, so the frame read-back is one DMA */
 	const size_t bytes = (size_t)r->prefs.imageWidth * r->prefs.imageHeight * 3 * sizeof(float);
 	r->state.renderBuffer = crgpu_host_alloc(bytes);
@@ -229,6 +242,23 @@ int takeRankTiles(struct renderer *r, int *rects, int *nums) {
 	return got;
 }
 
+/* copy the rows of a worker's tiles from a W*H*3 snapshot into the preview; both have the framebuffer's row order (row H-1-y) */
+static void preview_tiles(struct renderer *r, struct renderThreadState *ts, const uint8_t *snap, const int *rects, int got, int passes) {
+	const size_t W = r->prefs.imageWidth, H = r->prefs.imageHeight;
+	pthread_mutex_lock(&r->state.previewMutex);
+	if (r->state.preview && r->state.previewBytes == W * H * 3u) {
+		for (int i = 0; i < got; ++i) {
+			const int *t = rects + 4 * i;
+			for (int y = t[1]; y < t[3]; ++y) {
+				const size_t off = ((H - 1u - (size_t)y) * W + (size_t)t[0]) * 3u;
+				memcpy(r->state.preview + off, snap + off, (size_t)(t[2] - t[0]) * 3u);
+			}
+		}
+		ts->previewPasses = passes;
+	}
+	pthread_mutex_unlock(&r->state.previewMutex);
+}
+
 void *gpuRenderThread(void *arg) {
 	struct renderThreadState *ts = arg;
 	struct renderer *r = ts->renderer;
@@ -276,6 +306,17 @@ void *gpuRenderThread(void *arg) {
 		const double t0 = now_s();
 		int rc = crgpu_stop_enable(ts->gpu, 1);
 		int begin = 0;
+		/* The live preview: like renderThread, which writes each pixel's running average into the 8-bit image after every pass
+		 * (renderer.c:294-300), but at most every CR_PREVIEW_INTERVAL_MS.  The worker asks for a snapshot when its committed pass has
+		 * advanced; the device stages it at its next publish step, and this loop copies its tiles out once it is there. */
+		const size_t snap_bytes = (size_t)r->prefs.imageWidth * r->prefs.imageHeight * 3u;
+		uint8_t *snap = crgpu_host_alloc(snap_bytes);
+		const bool snap_pinned = snap != NULL;
+		if (!snap) snap = malloc(snap_bytes);
+		if (!snap) rc = CRGPU_ERR_NOMEM;
+		int shown = 0;
+		bool asked = false;
+		double last_snap = t0;
 		while (rc == CRGPU_OK && begin < spp) {
 			rc = crgpu_render_tiles(ts->gpu, rects, got, begin, spp - begin, CRGPU_FLAG_ASYNC, NULL);
 			if (rc != CRGPU_OK) break;
@@ -286,10 +327,25 @@ void *gpuRenderThread(void *arg) {
 				ts->completedSamples = done;
 				ts->totalSamples = (uint64_t)done * (uint64_t)got;                    /* tile-passes done, renderer.c:307 */
 				if (done > 0) ts->avgSampleTime = (long)(1e6 * (now_s() - t0) / ((double)done * got));
+				if (asked || !busy) {
+					/* with the call over, take answers from the framebuffer: a stop or pause shows its committed passes at once (a
+					 * finished share needs no snapshot: renderFrame's image follows) */
+					int k = 0;
+					const int trc = asked || (done > shown && done < spp) ? crgpu_take_snapshot(ts->gpu, snap, &k) : CRGPU_PENDING;
+					if (trc == CRGPU_OK) { preview_tiles(r, ts, snap, rects, got, k); shown = k; asked = false; last_snap = now_s(); }
+					else if (trc != CRGPU_PENDING) {            /* stop the call and wait for it before leaving */
+						rc = trc;
+						crgpu_request_stop(ts->gpu);
+						crgpu_get_stats(ts->gpu, NULL);
+						break;
+					}
+				}
 				if (!busy) break;
+				if (!asked && done > shown && now_s() - last_snap >= 1e-3 * CR_PREVIEW_INTERVAL_MS) { crgpu_request_snapshot(ts->gpu); asked = true; }
 				if (!stopping && (r->state.renderAborted || ts->paused || r->state.paused)) { crgpu_request_stop(ts->gpu); stopping = true; }
-				sleep_ms(1);      /* a poll is three loads of pinned memory; a 16 ms period would add 8 ms to the frame on average */
+				sleep_ms(1);      /* a poll is a few loads of pinned memory; a 16 ms period would add 8 ms to the frame on average */
 			}
+			if (rc != CRGPU_OK) break;
 			struct crgpu_stats st;
 			rc = crgpu_get_stats(ts->gpu, &st);
 			if (rc != CRGPU_OK) break;
@@ -300,6 +356,7 @@ void *gpuRenderThread(void *arg) {
 			if (r->state.renderAborted) break;
 			rc = crgpu_clear_stop(ts->gpu);
 		}
+		if (snap_pinned) crgpu_host_free(snap); else free(snap);
 		if (rc != CRGPU_OK) {
 			fprintf(stderr, "gpuRenderThread[%d]: %s\n", ts->thread_num, crgpu_last_error());
 			ts->error = rc;
@@ -344,6 +401,10 @@ struct texture8 *renderFrame(struct renderer *r) {
 	struct texture8 *output = calloc(1, sizeof *output);          /* renderer.c:41 */
 	output->width = W; output->height = H;
 	output->data = calloc((size_t)W * H * 3, 1);
+	pthread_mutex_lock(&r->state.previewMutex);                   /* the preview starts blank, like the output */
+	preview_resize_locked(r, (size_t)W * H * 3);
+	if (r->state.preview) memset(r->state.preview, 0, r->state.previewBytes);
+	pthread_mutex_unlock(&r->state.previewMutex);
 	if (r->state.threadStateCount != n) {
 		/* a host thread may be reading the worker states (crhostProgress): swap the array under doneMutex, and only when its size
 		 * changes; between frames of the same size the entries are re-initialised in place */
@@ -451,6 +512,12 @@ struct texture8 *renderFrame(struct renderer *r) {
 	}
 	if (discard && !r->prefs.quiet) printf("\nAborted: image not saved\n");
 	if (err || discard) { destroyTexture8(output); return NULL; }
+	if (!ranked || r->rank == 0) {                                /* the preview ends on the frame's image */
+		pthread_mutex_lock(&r->state.previewMutex);
+		if (r->state.preview && r->state.previewBytes == (size_t)W * H * 3) memcpy(r->state.preview, output->data, r->state.previewBytes);
+		for (int t = 0; t < n; ++t) r->state.threadStates[t].previewPasses = r->state.threadStates[t].completedSamples;
+		pthread_mutex_unlock(&r->state.previewMutex);
+	}
 	return output;
 }
 
@@ -471,6 +538,20 @@ int crhostProgress(const struct renderer *r, unsigned long long *passes_done_tot
 	if (passes_done_total) *passes_done_total = done;
 	return r->state.isRendering ? 1 : 0;
 }
+int crhostCurrentImagePasses(struct renderer *r, uint8_t *rgb8, int *passes, int workers) {
+	if (!r) return 0;
+	pthread_mutex_lock(&r->state.doneMutex);                      /* the worker states (see crhostProgress), then the preview */
+	pthread_mutex_lock(&r->state.previewMutex);
+	/* exactly the W*H*3 bytes of the current image size, whatever the preview holds */
+	const size_t bytes = (size_t)r->prefs.imageWidth * r->prefs.imageHeight * 3u;
+	if (rgb8 && r->state.preview && r->state.previewBytes == bytes) memcpy(rgb8, r->state.preview, bytes);
+	else if (rgb8) memset(rgb8, 0, bytes);
+	for (int t = 0; passes && t < workers && t < r->state.threadStateCount; ++t) passes[t] = r->state.threadStates[t].previewPasses;
+	pthread_mutex_unlock(&r->state.previewMutex);
+	pthread_mutex_unlock(&r->state.doneMutex);
+	return r->state.isRendering ? 1 : 0;
+}
+int crhostCurrentImage(struct renderer *r, uint8_t *rgb8) { return crhostCurrentImagePasses(r, rgb8, NULL, 0); }
 int crhostWorkerPasses(const struct renderer *r, int t) {
 	if (!r) return 0;
 	pthread_mutex_t *m = (pthread_mutex_t *)&r->state.doneMutex;
@@ -489,6 +570,8 @@ void destroyRenderer(struct renderer *r) {                       /* renderer.c:3
 	crscene_free(&r->scene);
 	free_render_buffer(r);
 	free(r->state.renderTiles); free(r->state.tileOwner); free(r->state.threads); free(r->state.threadStates);
+	free(r->state.preview);
+	pthread_mutex_destroy(&r->state.previewMutex);
 	pthread_mutex_destroy(&r->state.tileMutex);
 	pthread_mutex_destroy(&r->state.doneMutex);
 	pthread_cond_destroy(&r->state.doneCond);

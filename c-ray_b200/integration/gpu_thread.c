@@ -10,7 +10,10 @@
  *   - a trip to the tile queue takes several tiles (a GPU wavefront wants ~64M paths in flight; one 64x64 tile is 4096 pixels)
  *     and renders them as ONE wavefront with crgpu_render_tiles;
  *   - pixels land in the device framebuffer and are copied into state.renderBuffer / the 8-bit output per tile afterwards, with
- *     the layout of setPixel (texture.c:19-28), so the preview window, the stats loop and the encoders see what they expect.
+ *     the layout of setPixel (texture.c:19-28), so the preview window, the stats loop and the encoders see what they expect;
+ *   - while a trip renders, the 8-bit output of its tiles is refreshed from snapshots (crgpu_request_snapshot /
+ *     crgpu_take_snapshot) at most every GPU_PREVIEW_INTERVAL_MS, so the preview improves during the trip as renderThread's
+ *     does pass by pass (renderer.c:294-300).  The float renderBuffer is written once, at the end of the trip.
  */
 #include "includes.h"
 #include "renderer/renderer.h"
@@ -54,6 +57,18 @@ static crgpu_prepared *prepared_scene(const struct renderer *r) {
 }
 
 #define GPU_TRIP_MAX 1024
+#define GPU_PREVIEW_INTERVAL_MS 100      /* the host mirror's CR_PREVIEW_INTERVAL_MS */
+
+/* the rows of a trip's tiles from a W*H*3 image in setPixel's layout (texture.c:24-28) into another */
+static void copy_tile_rows(unsigned char *dst, const unsigned char *src, const int *rects, int got, unsigned W, unsigned H) {
+	for (int i = 0; i < got; ++i) {
+		const int *q = rects + 4 * i;
+		for (int y = q[1]; y < q[3]; ++y) {
+			const size_t off = ((size_t)q[0] + (size_t)(H - (unsigned)(y + 1)) * W) * 3u;
+			memcpy(dst + off, src + off, (size_t)(q[2] - q[0]) * 3u);
+		}
+	}
+}
 
 void *gpuRenderThread(void *arg) {
 	struct renderThreadState *ts = (struct renderThreadState *)threadUserData(arg);      /* thread.c:15-18 */
@@ -98,6 +113,8 @@ void *gpuRenderThread(void *arg) {
 		 * uninterrupted trip. */
 		const uint64_t samplesBefore = ts->totalSamples;
 		int begin = 0, rc = crgpu_stop_enable(gpu, 1);
+		int shown = 0, asked = 0;
+		long lastSnapUs = 0;
 		while (rc == CRGPU_OK && begin < r->prefs.sampleCount) {
 			rc = crgpu_render_tiles(gpu, rects, got, begin, r->prefs.sampleCount - begin, CRGPU_FLAG_ASYNC, NULL);
 			int done = begin, busy = rc == CRGPU_OK, stopping = 0;
@@ -107,6 +124,14 @@ void *gpuRenderThread(void *arg) {
 				ts->completedSamples = done > 0 ? done : 1;
 				ts->totalSamples = samplesBefore + (uint64_t)done * (uint64_t)got;
 				if (done > 0) ts->avgSampleTime = getUs(timer) / ((long)done * got);
+				if (asked) {                 /* staged by a publish step; or, once the call is over, the framebuffer as it is */
+					int k = 0;
+					if (crgpu_take_snapshot(gpu, fb8, &k) == CRGPU_OK) {
+						copy_tile_rows(image->data.byte_p, fb8, rects, got, W, H);
+						shown = k; asked = 0; lastSnapUs = getUs(timer);
+					}
+				}
+				if (busy && !asked && done > shown && getUs(timer) - lastSnapUs >= 1000L * GPU_PREVIEW_INTERVAL_MS) { crgpu_request_snapshot(gpu); asked = 1; }
 				if (!stopping && (r->state.renderAborted || ts->paused)) { crgpu_request_stop(gpu); stopping = 1; }
 				if (busy) sleepMSec(1);
 			}
@@ -122,14 +147,13 @@ void *gpuRenderThread(void *arg) {
 		}
 		/* renderer.c:294-300: the float tile into state.renderBuffer, the sRGB tile into the 8-bit output */
 		crgpu_framebuffer_to_srgb8(gpu, fb8);
+		copy_tile_rows(image->data.byte_p, fb8, rects, got, W, H);
 		for (int i = 0; i < got; ++i) {
 			const int *q = rects + 4 * i;
 			crgpu_framebuffer_read(gpu, fb, q[0], q[1], q[2], q[3]);
 			for (int y = q[1]; y < q[3]; ++y) {
 				const size_t off = ((size_t)q[0] + (size_t)(H - (unsigned)(y + 1)) * W) * 3u;       /* texture.c:24-28 */
-				const size_t n = (size_t)(q[2] - q[0]) * 3u;
-				memcpy(r->state.renderBuffer->data.float_p + off, fb + off, n * sizeof(float));
-				memcpy(image->data.byte_p + off, fb8 + off, n);
+				memcpy(r->state.renderBuffer->data.float_p + off, fb + off, (size_t)(q[2] - q[0]) * 3u * sizeof(float));
 			}
 			r->state.renderTiles[nums[i]].isRendering = false;                           /* renderer.c:315-316 */
 			r->state.renderTiles[nums[i]].renderComplete = begin >= r->prefs.sampleCount;

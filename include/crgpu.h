@@ -40,6 +40,7 @@ extern "C" {
 #define CRGPU_ERR_UNSUPPORTED   -4   /* node graph deeper than the device interpreter supports, etc. */
 #define CRGPU_ERR_NOMEM         -5
 #define CRGPU_STOPPED            1   /* not an error: an armed render call ended at a pass boundary because a stop was requested */
+#define CRGPU_PENDING            2   /* not an error: the snapshot asked for has not been staged yet (crgpu_take_snapshot) */
 
 typedef struct crgpu_scene crgpu_scene;
 
@@ -144,6 +145,26 @@ int crgpu_stop_enable(crgpu_scene *s, int on);
 int crgpu_request_stop(crgpu_scene *s);
 int crgpu_clear_stop(crgpu_scene *s);
 int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy);
+
+/* Reading the image of an armed scene while a call renders it (crGetCurrentImage, reference src/c-ray.h:97).  After each publish
+ * step the framebuffer holds exactly the passes [pass_begin, k), so an image taken there is exact: byte for byte the sRGB8 image of
+ * a render of [pass_begin, k) on top of what the framebuffer held before the call.  Pixels outside the call's tiles are whatever
+ * the framebuffer held.  A pixel set walked in pieces publishes after a pass batch over all of it, so the image always shows one
+ * pass boundary over the whole set.
+ *   crgpu_request_snapshot  one compare-and-swap on pinned memory: thread-safe and async-signal-safe.  The next publish step
+ *                           converts the whole framebuffer to sRGB8 (crgpu_framebuffer_to_srgb8's arithmetic and layout) into a
+ *                           device staging buffer of W*H*3 bytes and marks it staged.  A staged image that has not been taken
+ *                           stays staged, also past the end of the call: the device never writes the staging buffer until
+ *                           crgpu_take_snapshot has copied it, and the pass index it returns says which passes the image shows.
+ *   crgpu_take_snapshot     never waits for the render.  With an image staged it copies it to host_rgb8 (W*H*3 bytes) on a stream
+ *                           of its own and sets *passes_done (may be NULL) to the pass index it shows.  Otherwise, while a call is
+ *                           in flight, it returns CRGPU_PENDING; with no call in flight it converts the framebuffer as it is (on
+ *                           the scene's stream, as crgpu_framebuffer_to_srgb8 does) and gives the committed pass index.  Either
+ *                           answer completes the request.
+ * A render call that finds no request launches the same kernels as before; its publish step stays one thread's work.  Both calls
+ * fail with CRGPU_ERR_BAD_ARGUMENT on a NULL or unarmed scene, take also on a NULL buffer; crgpu_stop_enable clears the state. */
+int crgpu_request_snapshot(crgpu_scene *s);
+int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
 
 /* Editing a resident scene between renders (c-ray's crMoveCamera / crTransformMesh, src/c-ray.h:95-103): the edited scene renders
  * the same bits as the scene loaded fresh from the edited JSON.  Both calls first wait for the work queued on the scene's streams,
