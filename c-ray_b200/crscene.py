@@ -136,7 +136,7 @@ def build_bvh(bboxes, centers):
     L.crloader_build_bvh.restype = C.c_int
     rc, nodes, prims = _build(L.crloader_build_bvh, bboxes, centers)
     if rc != 0:
-        raise RuntimeError("crloader_build_bvh failed")
+        raise RuntimeError(f"crloader_build_bvh failed ({rc}): " + L.crloader_last_error().decode(errors="replace"))
     return nodes, prims
 
 

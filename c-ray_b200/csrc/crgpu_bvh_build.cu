@@ -27,6 +27,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+#include <utility>
 #include <vector>
 
 int crg_fail(int code, const char *fmt, ...);           /* crgpu_api.cu: sets crgpu_last_error() */
@@ -458,15 +459,28 @@ static int scan64(const unsigned long long *in, unsigned long long *out, unsigne
 	return 0;
 }
 
-/* The tree of n >= 1 primitives (device boxes and centres) into the scratch s, on st: records level by level in s.recs, primitive
- * order in s.prims.  Synchronises st once per level (the open-node count sizes the next launches). */
-static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scratch &s, cudaStream_t st,
+/* The records of a build: the scratch's 2n until a level could need more, then a device array of their own.  A tree needs more than
+ * 2n - 1 nodes only with empty leaves: when every primitive of a node falls into bin 0 of the chosen axis (zero extent: the bin scale
+ * is inf; an extent that overflows: it is 0), every cost is NaN or inf and the split sends everything left, so the node gets an empty
+ * right leaf and a left child with its primitives and box, down to the depth cap. */
+struct RecStore {
+	Rec *recs;
+	size_t cap;
+	DevBuf own;
+};
+
+/* The tree of n >= 1 primitives (device boxes and centres) into the scratch s, on st: records level by level in rs.recs, primitive
+ * order in s.prims.  Synchronises st once per level (the open-node count sizes the next launches); a level adds at most two records
+ * per open node, and the records grow before a level that could pass their end. */
+static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scratch &s, cudaStream_t st, RecStore &rs,
 					  std::vector<uint32_t> &level_first, std::vector<uint32_t> &level_count, uint32_t *nrec_out) {
 	const uint32_t max_open = n / 2u + 1u;
 	const unsigned long long init_keys[6] = { KMIN_EMPTY, KMIN_EMPTY, KMIN_EMPTY, KMAX_EMPTY, KMAX_EMPTY, KMAX_EMPTY };
 	CUB(cudaMemcpyAsync(s.keys, init_keys, sizeof init_keys, cudaMemcpyHostToDevice, st));
 	const uint32_t gn = (n + 255u) / 256u;
-	Rec *recs = s.recs;
+	rs.recs = s.recs;
+	rs.cap = 2u * (size_t)n;
+	Rec *recs = rs.recs;
 	uint32_t *counters = s.cnt;
 	k_iota<<<gn, 256, 0, st>>>(s.prims, s.owner, n, n >= 2u ? 0 : -1);
 	k_root_keys<<<gn, 256, 0, st>>>(bb, n, s.keys);
@@ -480,6 +494,17 @@ static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scrat
 	while (h[1] > 0u) {
 		const uint32_t nopen = h[1], go = (nopen + 127u) / 128u;
 		if (nopen > max_open) return crg_fail(CRGPU_ERR_CUDA, "crgpu_bvh_build: %u open nodes for %u primitives", nopen, n);
+		const size_t need = (size_t)h[0] + 2u * (size_t)nopen;
+		if (need > rs.cap) {
+			const size_t cap = need > 2u * rs.cap ? need : 2u * rs.cap;
+			DevBuf grown;
+			CUB(grown.alloc(cap * sizeof(Rec)));
+			CUB(cudaMemcpyAsync(grown.p, recs, (size_t)h[0] * sizeof(Rec), cudaMemcpyDeviceToDevice, st));
+			CUB(cudaStreamSynchronize(st));
+			std::swap(rs.own.p, grown.p);                                   /* the previous own array (if any) is freed here */
+			rs.recs = recs = rs.own.as<Rec>();
+			rs.cap = cap;
+		}
 		uint32_t *open_list = s.open[cur], *next_list = s.open[cur ^ 1];
 		{
 			const size_t blocks = ((size_t)nopen * (sizeof(Bins) / 8u) + 255u) / 256u;          /* grid-stride loop inside */
@@ -520,18 +545,21 @@ int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, void *scrat
 	carve(scratch, n, &s);
 	std::vector<uint32_t> level_first, level_count;
 	uint32_t nrec = 0u;
-	int rc = build_tree(bb, ctr, n, s, st, level_first, level_count, &nrec);
+	RecStore rs;
+	int rc = build_tree(bb, ctr, n, s, st, rs, level_first, level_count, &nrec);
 	if (rc) return rc;
+	if (nrec > 2u * n - 1u)                                               /* pairs_out, order and bfs_of hold a tree of 2n - 1 nodes */
+		return crg_fail(CRGPU_ERR_UNSUPPORTED, "crgpu_bvh_build: the tree of %u primitives needs %u nodes, more than 2n - 1", n, nrec);
 	uint32_t info[2] = { 0u, 0u };
 	if (nrec > 1u) {
-		k_top_bfs<<<1, 1024, 0, st>>>(s.recs, s.order, s.bfs_of, s.info);
+		k_top_bfs<<<1, 1024, 0, st>>>(rs.recs, s.order, s.bfs_of, s.info);
 		const uint32_t internal = (nrec - 1u) / 2u;                   /* a full binary tree */
-		k_top_pairs<<<(internal + 255u) / 256u, 256, 0, st>>>(s.recs, s.order, s.bfs_of, internal, pairs_out);
+		k_top_pairs<<<(internal + 255u) / 256u, 256, 0, st>>>(rs.recs, s.order, s.bfs_of, internal, pairs_out);
 		CUB(cudaMemcpyAsync(info, s.info, sizeof info, cudaMemcpyDeviceToHost, st));
 	}
 	CUB(cudaMemcpyAsync(prims_out, s.prims, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
 	Rec root;
-	CUB(cudaMemcpyAsync(&root, s.recs, sizeof root, cudaMemcpyDeviceToHost, st));
+	CUB(cudaMemcpyAsync(&root, rs.recs, sizeof root, cudaMemcpyDeviceToHost, st));
 	CUB(cudaStreamSynchronize(st));
 	CUB(cudaGetLastError());
 	out->node_count = nrec;
@@ -570,9 +598,14 @@ extern "C" int crgpu_bvh_build(const float *bboxes, const float *centers, uint32
 	CUB(cudaMemcpyAsync(d_ctr.p, centers, (size_t)n * 12u, cudaMemcpyHostToDevice, st));
 	std::vector<uint32_t> level_first, level_count;
 	uint32_t nrec = 0u;
-	rc = build_tree(d_bb.as<float>(), d_ctr.as<float>(), n, s, st, level_first, level_count, &nrec);
+	RecStore rs;
+	rc = build_tree(d_bb.as<float>(), d_ctr.as<float>(), n, s, st, rs, level_first, level_count, &nrec);
 	if (rc) return rc;
-	Rec *recs = s.recs;
+	if (nrec > max_rec - 1u) {                                              /* the caller has room for 2n - 1 nodes */
+		*node_count_out = nrec;
+		return crg_fail(CRGPU_ERR_UNSUPPORTED, "crgpu_bvh_build: the tree of %u primitives needs %u nodes, more than 2n - 1", n, nrec);
+	}
+	Rec *recs = rs.recs;
 	for (size_t l = level_first.size(); l-- > 0;)
 		k_count_internals<<<(level_count[l] + 255u) / 256u, 256, 0, st>>>(recs, level_first[l], level_count[l]);
 	for (size_t l = 0; l < level_first.size(); ++l)

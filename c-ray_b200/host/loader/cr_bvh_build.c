@@ -163,12 +163,15 @@ static int split_node(const struct builder *B, const float bounds[6], unsigned b
 	return 1;
 }
 
-/* Serial build of one subtree into nodes[]: nodes[0] is the subtree root (bounds already stored), descendants are
- * appended in the reference's allocation order (children as a pair when their parent is visited, left subtree first).
- * Child links are indices into this local array.  Returns the number of nodes. */
+/* Serial build of one subtree into *nodes (room for *cap nodes, grown with realloc as needed): (*nodes)[0] is the subtree root
+ * (bounds already stored), descendants are appended in the reference's allocation order (children as a pair when their parent is
+ * visited, left subtree first).  Child links are indices into this local array.  Returns the number of nodes, 0 when out of memory.
+ * A tree can need more than 2n-1 nodes: when every primitive of a node falls into bin 0 of the chosen axis (a zero extent, where the
+ * bin scale is inf, or an extent that overflows to inf, where it is 0), every cost is NaN or inf and the split sends everything left,
+ * so the node gets an empty right leaf and a left child with the same primitives and box, down to the depth cap. */
 struct work { unsigned node, begin, end, depth; };
 
-static unsigned build_subtree(const struct builder *B, struct crs_bvh_node *nodes, unsigned begin, unsigned end, unsigned depth) {
+static unsigned build_subtree(const struct builder *B, struct crs_bvh_node **nodes, size_t *cap, unsigned begin, unsigned end, unsigned depth) {
 	struct bin bins[3][BIN_COUNT];
 	struct work stack[MAX_DEPTH + 2];
 	unsigned node_count = 1;
@@ -176,17 +179,23 @@ static unsigned build_subtree(const struct builder *B, struct crs_bvh_node *node
 	stack[sp++] = (struct work){ 0, begin, end, depth };
 	while (sp) {
 		const struct work w = stack[--sp];
-		struct crs_bvh_node *node = &nodes[w.node];
 		bbox3 lb, rb;
 		unsigned beginRight;
-		if (!split_node(B, node->bounds, w.begin, w.end, w.depth, bins, &lb, &rb, &beginRight)) {
-			make_leaf(node, w.begin, w.end - w.begin);
+		if (!split_node(B, (*nodes)[w.node].bounds, w.begin, w.end, w.depth, bins, &lb, &rb, &beginRight)) {
+			make_leaf(&(*nodes)[w.node], w.begin, w.end - w.begin);
 			continue;
 		}
+		if ((size_t)node_count + 2 > *cap) {
+			const size_t grown = 2 * *cap + 2;
+			struct crs_bvh_node *p = realloc(*nodes, sizeof(**nodes) * grown);
+			if (!p) return 0;
+			*nodes = p; *cap = grown;
+		}
+		struct crs_bvh_node *node = &(*nodes)[w.node];
 		const unsigned left = node_count, right = left + 1;
 		node_count += 2;
-		store_bbox(&nodes[left], &lb);
-		store_bbox(&nodes[right], &rb);
+		store_bbox(&(*nodes)[left], &lb);
+		store_bbox(&(*nodes)[right], &rb);
 		node->first_child_or_prim = left;
 		node->prim_count_leaf = 0;
 		/* the reference recurses left first, so the left subtree claims node indices first: push right, then left */
@@ -201,7 +210,7 @@ static unsigned build_subtree(const struct builder *B, struct crs_bvh_node *node
  * those are built by a small pthread pool into private arrays; a final depth-first walk lays everything out in the
  * order the serial recursion would have produced, so the result does not depend on the thread count. */
 struct top { float bounds[6]; unsigned begin, end, depth; int left, right; int task; int leaf; };
-struct task { unsigned begin, end, depth; float bounds[6]; struct crs_bvh_node *nodes; unsigned count; };
+struct task { unsigned begin, end, depth; float bounds[6]; struct crs_bvh_node *nodes; size_t cap; unsigned count; };
 struct pool { const struct builder *B; struct task *tasks; int ntasks; int next; };
 
 static void *pool_worker(void *arg) {
@@ -211,7 +220,7 @@ static void *pool_worker(void *arg) {
 		if (t >= p->ntasks) return NULL;
 		struct task *k = &p->tasks[t];
 		memcpy(k->nodes[0].bounds, k->bounds, sizeof(k->bounds));
-		k->count = build_subtree(p->B, k->nodes, k->begin, k->end, k->depth);
+		k->count = build_subtree(p->B, &k->nodes, &k->cap, k->begin, k->end, k->depth);     /* 0: out of memory */
 	}
 }
 
@@ -289,7 +298,8 @@ int crl_build_bvh(void *user, crl_bbox_fn fn, unsigned count,
 	vec3 *centers = malloc(sizeof(vec3) * count);
 	bbox3 *bboxes = malloc(sizeof(bbox3) * count);
 	int32_t *prims = malloc(sizeof(int32_t) * count);
-	struct crs_bvh_node *nodes = calloc((size_t)2 * count - 1, sizeof(*nodes));
+	size_t node_cap = (size_t)2 * count - 1;              /* enough for any tree without empty leaves; grown when needed */
+	struct crs_bvh_node *nodes = calloc(node_cap, sizeof(*nodes));
 	if (!centers || !bboxes || !prims || !nodes) { free(centers); free(bboxes); free(prims); free(nodes); return -1; }
 
 	bbox3 root = crl_empty_bbox;
@@ -300,11 +310,12 @@ int crl_build_bvh(void *user, crl_bbox_fn fn, unsigned count,
 		root.max = v_max(root.max, bboxes[i].max);
 	}
 	const struct builder B = { bboxes, centers, prims };
-	unsigned node_count;
+	unsigned node_count = 0;
 	const int threads = crl_thread_count();
 	if (threads < 2 || count < PARALLEL_MIN_PRIMS) {
 		store_bbox(&nodes[0], &root);
-		node_count = build_subtree(&B, nodes, 0, count, 0);
+		node_count = build_subtree(&B, &nodes, &node_cap, 0, count, 0);
+		if (!node_count) { free(centers); free(bboxes); free(prims); free(nodes); return -1; }
 	} else {
 		/* 1. open the top of the tree serially, always splitting the largest open range */
 		const int want = threads * 4;
@@ -349,7 +360,8 @@ int crl_build_bvh(void *user, crl_bbox_fn fn, unsigned count,
 			n->task = i;
 			tasks[i] = (struct task){ .begin = n->begin, .end = n->end, .depth = n->depth };
 			memcpy(tasks[i].bounds, n->bounds, sizeof(n->bounds));
-			tasks[i].nodes = calloc((size_t)2 * (n->end - n->begin), sizeof(struct crs_bvh_node));
+			tasks[i].cap = (size_t)2 * (n->end - n->begin) + 1;          /* an empty range (an empty right leaf) still has its root */
+			tasks[i].nodes = calloc(tasks[i].cap, sizeof(struct crs_bvh_node));
 			if (!tasks[i].nodes) ok = 0;
 		}
 		if (ok) {
@@ -361,11 +373,19 @@ int crl_build_bvh(void *user, crl_bbox_fn fn, unsigned count,
 			pool_worker(&pool);
 			for (int i = 0; i < started; ++i) pthread_join(th[i], NULL);
 			free(th);
-			/* 3. lay out in the serial recursion's order */
-			unsigned counter = 1;
-			layout(tops, tasks, 0, 0, nodes, &counter);
-			node_count = counter;
-		} else node_count = 0;
+			/* 3. lay out in the serial recursion's order: every top node once, plus each task's nodes below its root */
+			size_t total = (size_t)ntops;
+			for (int i = 0; i < nopen; ++i) { if (!tasks[i].count) ok = 0; else total += tasks[i].count - 1; }
+			if (ok && total > node_cap) {
+				struct crs_bvh_node *p = realloc(nodes, sizeof(*nodes) * total);
+				if (p) nodes = p; else ok = 0;
+			}
+			if (ok) {
+				unsigned counter = 1;
+				layout(tops, tasks, 0, 0, nodes, &counter);
+				node_count = counter;
+			}
+		}
 		for (int i = 0; i < nopen; ++i) free(tasks[i].nodes);
 		free(tasks); free(tops); free(open); free(bins);
 		if (!ok) { free(centers); free(bboxes); free(prims); free(nodes); return -1; }
@@ -388,7 +408,7 @@ static void array_bbox(void *user, unsigned i, bbox3 *bbox, vec3 *center) {
 
 int crloader_build_bvh(const float *bboxes, const float *centers, uint32_t n,
                        struct crs_bvh_node *nodes_out, uint32_t *node_count_out, int32_t *prims_out) {
-	if (!node_count_out || (n && (!bboxes || !centers || !nodes_out || !prims_out))) return -1;
+	if (!node_count_out || (n && (!bboxes || !centers || !nodes_out || !prims_out))) { crl_set_error("crloader_build_bvh: NULL argument"); return -1; }
 	*node_count_out = 0;
 	if (n == 0) return 0;
 	struct array_user u = { bboxes, centers };
@@ -399,11 +419,17 @@ int crloader_build_bvh(const float *bboxes, const float *centers, uint32_t n,
 	g_builder = NULL;                                  /* always the host algorithm */
 	const int rc = crl_build_bvh(&u, array_bbox, n, &nodes, &cnt, &prims);
 	g_builder = saved;
-	if (rc == 0) {
+	int out = rc;
+	if (rc) crl_set_error("crloader_build_bvh: out of memory");
+	if (rc == 0 && cnt > 2 * (uint64_t)n - 1) {          /* the caller has room for 2n-1 nodes: report the size, write nothing */
+		*node_count_out = cnt;
+		crl_set_error("crloader_build_bvh: the tree of %u primitives needs %u nodes, more than 2n - 1", n, cnt);
+		out = -2;
+	} else if (rc == 0) {
 		memcpy(nodes_out, nodes, sizeof(*nodes) * cnt);
 		memcpy(prims_out, prims, sizeof(int32_t) * n);
 		*node_count_out = cnt;
 	}
 	free(nodes); free(prims);
-	return rc;
+	return out;
 }

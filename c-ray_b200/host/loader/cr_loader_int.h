@@ -94,6 +94,9 @@ typedef void (*crl_bbox_fn)(void *user, unsigned i, bbox3 *bbox, vec3 *center);
 int crl_build_bvh(void *user, crl_bbox_fn fn, unsigned count,
                   struct crs_bvh_node **nodes, uint32_t *node_count, int32_t **prims);
 
+/* cr_sceneload.c: the message of crloader_last_error() */
+void crl_set_error(const char *fmt, ...) __attribute__((format(printf, 1, 2)));
+
 /* cr_threads.c */
 int crl_thread_count(void);
 void crl_parallel_for(int n, void (*fn)(void *arg, int index), void *arg);

@@ -14,6 +14,7 @@
 #include "cr_loader_int.h"
 #include "cr_json.h"
 #include "../../../include/crloader.h"
+#include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -22,6 +23,12 @@
 
 static _Thread_local char g_err[512];
 const char *crloader_last_error(void) { return g_err; }
+void crl_set_error(const char *fmt, ...) {
+	va_list ap;
+	va_start(ap, fmt);
+	vsnprintf(g_err, sizeof(g_err), fmt, ap);
+	va_end(ap);
+}
 
 /* ---- small helpers ------------------------------------------------------------------------------------- */
 static char *slurp(const char *path) {

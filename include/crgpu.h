@@ -174,7 +174,9 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *                              kind and object, must be those uploaded (instances cannot be added or removed).  The instance
  *                              boxes, ray offsets and the top-level BVH are rebuilt on the device, the tree that the scene loader
  *                              builds.  The first call gives the scene its own copy of the BVH pair nodes (the uploaded pairs plus
- *                              room for any top level of `count` instances); later calls reuse it.
+ *                              room for any top level of `count` instances); later calls reuse it.  A top level that needs more
+ *                              than count - 1 pair nodes (a tree of more than 2 count - 1 nodes, which only instances whose boxes no
+ *                              split separates make: see crloader_build_bvh in crloader.h) is refused with CRGPU_ERR_UNSUPPORTED.
  * Edits apply to this device scene only: the crgpu_prepared it was created from, and any scene created from that later, are
  * unedited. */
 int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam);
@@ -281,7 +283,9 @@ int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *o
  *   bboxes   n x 6 floats: min.x min.y min.z max.x max.y max.z of every primitive (what getBBoxAndCenter returns, bvh.c:283-291)
  *   centers  n x 3 floats
  *   nodes_out  room for 2n-1 nodes;  prims_out  n indices (primIndices);  *node_count_out  nodes written
- * n == 0 writes nothing (an empty BVH, bvh.c:251).  At most 4,194,304 primitives per call. */
+ * n == 0 writes nothing (an empty BVH, bvh.c:251).  At most 4,194,304 primitives per call.
+ * A tree with empty leaves can need more than 2n-1 nodes (see crloader_build_bvh in crloader.h): then nothing is written to nodes_out
+ * or prims_out, *node_count_out is set to the number of nodes the tree needs and CRGPU_ERR_UNSUPPORTED is returned. */
 int crgpu_bvh_build(const float *bboxes, const float *centers, uint32_t n, int device,
                     struct crs_bvh_node *nodes_out, uint32_t *node_count_out, int32_t *prims_out);
 

@@ -37,7 +37,11 @@ const char *crloader_last_error(void);
 
 /* The BVH builder on its own (reference src/accelerators/bvh.c:245-296 buildBvhGeneric): n primitives given by their boxes
  * (n x 6 floats: min.xyz, max.xyz) and centers (n x 3); nodes_out has room for 2n-1 nodes, prims_out for n indices.
- * Host counterpart of crgpu_bvh_build (crgpu.h, SURVEY 8 f1), same outputs bit for bit.  0 on success. */
+ * Host counterpart of crgpu_bvh_build (crgpu.h, SURVEY 8 f1), same outputs bit for bit.  0 on success.
+ * A tree can need more than 2n-1 nodes: 17 or more primitives that no split separates (centres at one point, or a node whose extent
+ * overflows to inf) take the median fallback, which sends all of them left, so each such node gets an empty right leaf (count 0,
+ * the empty box) and a left child with the same primitives, down to depth 64.  Then nothing is written to nodes_out or prims_out,
+ * *node_count_out is set to the number of nodes the tree needs and -2 is returned.  crloader_load_json* store such trees whole. */
 int crloader_build_bvh(const float *bboxes, const float *centers, uint32_t n,
                        struct crs_bvh_node *nodes_out, uint32_t *node_count_out, int32_t *prims_out);
 
