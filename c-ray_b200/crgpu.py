@@ -139,6 +139,9 @@ def lib():
             L.crgpu_request_snapshot.argtypes = [P]
             L.crgpu_take_snapshot.argtypes = [P, P, C.POINTER(C.c_int)]
             L.crgpu_request_snapshot.restype = L.crgpu_take_snapshot.restype = C.c_int
+        if hasattr(L, "crgpu_scene_set_meshes"):   # absent from libraries built before mesh edits
+            L.crgpu_scene_set_meshes.argtypes = [P, C.POINTER(FlatScene), P, C.c_uint32]
+            L.crgpu_scene_set_meshes.restype = C.c_int
         _lib = L
     return _lib
 
@@ -265,6 +268,14 @@ class GpuScene:
         import crscene
         arr = np.ascontiguousarray(instances, dtype=crscene.INSTANCE)
         _check(lib().crgpu_scene_set_instances(self.handle, arr.ctypes.data, len(arr)), "crgpu_scene_set_instances")
+
+    def set_meshes(self, flat, meshes):
+        """Deform meshes of the resident scene (crgpu_scene_set_meshes): each mesh index in `meshes` takes its polys and the
+        vertices, normals and texcoords they index from the FlatScene `flat` (same topology as uploaded), and its BVH, triangles and
+        shading records, the instance boxes and the top level are rebuilt on the device."""
+        idx = np.ascontiguousarray(meshes, dtype=np.uint32).reshape(-1)
+        _check(lib().crgpu_scene_set_meshes(self.handle, C.byref(flat), idx.ctypes.data if len(idx) else None, len(idx)),
+               "crgpu_scene_set_meshes")
 
     def set_stream(self, cuda_stream_ptr):
         """Enqueue on a caller-owned cudaStream_t (int pointer, e.g. torch.cuda.current_stream().cuda_stream)."""

@@ -54,6 +54,22 @@ def arrays(scene):
     return out
 
 
+def write_back(scene, name, values):
+    """Write `values` over the FlatScene array `name` ("vertices", "normals", "texcoords" or "polys") in place, from its first
+    element: `arrays` returns copies, so an edited copy goes back this way (e.g. before crgpu.GpuScene.set_meshes).  The scene must
+    own writable arrays, as load_json and load_json_buf return (crscene_load maps its file read-only)."""
+    table = {n: (dtype, count_field, width) for n, dtype, count_field, width in _SECTIONS}
+    if name not in ("vertices", "normals", "texcoords", "polys"):
+        raise ValueError(f"write_back: {name!r} is not vertices, normals, texcoords or polys")
+    dtype, count_field, width = table[name]
+    a = np.ascontiguousarray(values, dtype=dtype).reshape(-1)
+    n = int(getattr(scene, count_field)) * width
+    if len(a) > n:
+        raise ValueError(f"write_back: {len(a)} elements of {name}, the scene has {n}")
+    if len(a):
+        C.memmove(getattr(scene, name), a.ctypes.data, a.nbytes)
+
+
 _loader = None
 
 

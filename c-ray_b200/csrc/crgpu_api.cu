@@ -164,6 +164,9 @@ struct crgpu_prepared {
 	 * as stored (6 floats each; the slab keeps only pair nodes, whose roots' own boxes are not in it) */
 	std::vector<uint32_t> inst_kind, inst_object;
 	std::vector<float> bvh_root;
+	/* what crgpu_scene_set_meshes checks an edit against: every mesh record and the primitive count of every BVH */
+	std::vector<crs_mesh> meshes;
+	std::vector<uint32_t> bvh_prims;
 };
 
 struct crgpu_scene {
@@ -206,8 +209,17 @@ struct crgpu_scene {
 	std::vector<float> bvh_root;                     /* crgpu_prepared::bvh_root */
 	uint32_t pair_count;       /* pair nodes uploaded (the edit block starts with a copy of them) */
 	uint32_t top_stage_cap;    /* staged top-level pairs reserved at upload */
-	void *edit; size_t edit_bytes;             /* NULL until the first instance edit: uploaded pairs, the top region, top_items */
+	void *edit; size_t edit_bytes;             /* NULL until the first edit of instances or meshes: edit_pairs pair nodes (the
+	                                              uploaded pairs, the top region, the edited meshes' regions), then top_items */
+	uint32_t edit_pairs;
 	void *edit_scratch; size_t edit_scratch_bytes;   /* instance inputs, boxes, the new top level and the builder's scratch */
+	/* mesh edits (crgpu_scene_set_meshes) */
+	std::vector<crs_mesh> meshes;              /* as uploaded: an edit must keep each record */
+	std::vector<uint32_t> bvh_prims;           /* primitives of each BVH as uploaded */
+	std::vector<DevBvh> bvhs;                  /* the committed BVH records (the slab's copy is what the kernels read) */
+	std::vector<uint32_t> stage_cap;           /* staged pairs reserved for each BVH at upload */
+	std::vector<uint32_t> mesh_region;         /* first pair of a mesh's own region in the edit block (UINT32_MAX: none yet) */
+	void *mesh_scratch; size_t mesh_scratch_bytes;   /* a mesh edit's inputs, its rebuilt records and the builder's scratch */
 };
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
@@ -568,6 +580,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
 	ctx_free(s->device, s->edit, s->edit_bytes);
 	ctx_free(s->device, s->edit_scratch, s->edit_scratch_bytes);
+	ctx_free(s->device, s->mesh_scratch, s->mesh_scratch_bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -819,6 +832,9 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	p->bvh_root.assign(6 * (size_t)f->bvh_count, 0.0f);
 	for (uint32_t b = 0; b < f->bvh_count; ++b)
 		if (f->bvhs[b].node_count) memcpy(&p->bvh_root[6 * (size_t)b], f->bvh_nodes[f->bvhs[b].node_offset].bounds, 6 * sizeof(float));
+	p->meshes.assign(f->meshes, f->meshes + f->mesh_count);
+	p->bvh_prims.resize(f->bvh_count);
+	for (uint32_t b = 0; b < f->bvh_count; ++b) p->bvh_prims[b] = f->bvhs[b].prim_count;
 
 	/* textures (data pointers are byte offsets into the texture section here; patched per device at upload) */
 	std::vector<DevTexture> texs(f->texture_count);
@@ -961,7 +977,14 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr; s->snap8 = nullptr; s->snap_stream = nullptr;
 	s->inst_kind = p->inst_kind; s->inst_object = p->inst_object; s->bvh_root = p->bvh_root;
 	s->pair_count = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode)); s->top_stage_cap = p->top.stage_count;
-	s->edit = nullptr; s->edit_bytes = 0; s->edit_scratch = nullptr; s->edit_scratch_bytes = 0;
+	s->edit = nullptr; s->edit_bytes = 0; s->edit_pairs = 0; s->edit_scratch = nullptr; s->edit_scratch_bytes = 0;
+	s->meshes = p->meshes; s->bvh_prims = p->bvh_prims;
+	s->bvhs.resize(p->len[SEC_BVHS] / sizeof(DevBvh));
+	memcpy(s->bvhs.data(), p->slab + p->off[SEC_BVHS], p->len[SEC_BVHS]);
+	s->stage_cap.resize(s->bvhs.size());
+	for (size_t b = 0; b < s->bvhs.size(); ++b) s->stage_cap[b] = s->bvhs[b].stage_count;
+	s->mesh_region.assign(p->meshes.size(), 0xffffffffu);
+	s->mesh_scratch = nullptr; s->mesh_scratch_bytes = 0;
 	s->device = device; s->xnodes = p->xnodes; s->dev_copy = nullptr; s->fb = nullptr; s->fb8 = nullptr; s->stream = nullptr; s->own_stream = nullptr; s->cap_paths = 0;
 	s->slab = nullptr; s->slab_bytes = 0; s->small = nullptr; s->small_bytes = 0; s->wave = nullptr; s->wave_bytes = 0; s->fb_floats = 0;
 	memset(s->fetched, 0, sizeof s->fetched);
@@ -1419,6 +1442,114 @@ extern "C" int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *c
 	return CRGPU_OK;
 }
 
+static size_t align256(size_t b) { return (b + 255u) & ~(size_t)255u; }
+
+/* The instance scratch of an edit that rebuilds the top level: the caller's instances, last instance of each object, BVH roots,
+ * boxes, centres, offsets, new instance records, new top pairs and prims, then the builder's own scratch. */
+enum { ES_INST, ES_LAST, ES_ROOTS, ES_BB, ES_CTR, ES_OFFS, ES_NEW_INSTS, ES_PAIRS, ES_PRIMS, ES_BUILD, ES_COUNT };
+struct EditLayout { size_t sz[ES_COUNT], so[ES_COUNT], total; };
+static EditLayout edit_layout(const crgpu_scene *s) {
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const size_t top_cap = n > 1u ? n - 1u : 1u;
+	EditLayout L;
+	const size_t sz[ES_COUNT] = { (size_t)n * sizeof(crs_instance), (size_t)n * 4u, s->bvh_root.size() * sizeof(float), (size_t)n * 24u, (size_t)n * 12u,
+	                              (size_t)n * 4u, (size_t)n * sizeof(DevInstance), top_cap * sizeof(PairNode), (size_t)n * 4u, crg_bvh_scratch_bytes(n) };
+	L.total = 0;
+	for (int k = 0; k < ES_COUNT; ++k) { L.sz[k] = sz[k]; L.so[k] = L.total; L.total += align256(sz[k]); }
+	return L;
+}
+static DevTopItem *edit_items(const crgpu_scene *s) {
+	return reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->edit) + align256((size_t)s->edit_pairs * sizeof(PairNode)));
+}
+
+/* The first edit of instances or meshes gives the scene its own pairs block: the uploaded pairs (unedited meshes' pair offsets do not
+ * move), then a top region that holds any top level of n instances, then its n item records; the uploaded top level keeps rendering
+ * until an edit is committed.  It also allocates the instance scratch. */
+static int ensure_edit(crgpu_scene *s) {
+	if (s->edit) return CRGPU_OK;
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const uint32_t top_cap = n > 1u ? n - 1u : 1u;
+	const EditLayout L = edit_layout(s);
+	const size_t edit_bytes = align256((size_t)(s->pair_count + top_cap) * sizeof(PairNode)) + (size_t)n * sizeof(DevTopItem);
+	cudaStream_t st = s->stream;
+	void *e = nullptr, *q = nullptr;
+	int rc = ctx_alloc(s->device, edit_bytes, &e);
+	if (!rc) rc = ctx_alloc(s->device, L.total, &q);
+	std::vector<uint32_t> last(n);
+	std::unordered_map<uint64_t, uint32_t> last_of;                  /* (kind, object) -> its last instance */
+	for (uint32_t i = n; i-- > 0;) {
+		const uint64_t key = ((uint64_t)s->inst_kind[i] << 32) | s->inst_object[i];
+		last[i] = last_of.emplace(key, i).first->second;
+	}
+	cudaError_t ce = cudaSuccess;
+	if (!rc) ce = cudaMemcpyAsync(e, s->dev.pairs, (size_t)s->pair_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st);
+	if (!rc && ce == cudaSuccess && n) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + L.so[ES_LAST], last.data(), L.sz[ES_LAST], cudaMemcpyHostToDevice, st);
+	if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + L.so[ES_ROOTS], s->bvh_root.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st);
+	if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (!rc && ce != cudaSuccess) rc = fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
+	if (rc) { ctx_free(s->device, e, edit_bytes); ctx_free(s->device, q, L.total); return rc; }
+	s->edit = e; s->edit_bytes = edit_bytes; s->edit_pairs = s->pair_count + top_cap;
+	s->edit_scratch = q; s->edit_scratch_bytes = L.total;
+	return CRGPU_OK;
+}
+
+/* Instance boxes, ray offsets and the top-level BVH into the instance scratch: A and Ainv from inst (device, in the scratch), or the
+ * scene's current instance records when inst is NULL; mesh boxes from the BVH roots in the scratch. */
+static int build_top(crgpu_scene *s, const crs_instance *inst, CrgBuildResult *res) {
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const EditLayout L = edit_layout(s);
+	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
+	cudaStream_t st = s->stream;
+	DevInstance *new_insts = reinterpret_cast<DevInstance *>(sc + L.so[ES_NEW_INSTS]);
+	CU(cudaMemcpyAsync(new_insts, s->dev.instances, L.sz[ES_NEW_INSTS], cudaMemcpyDeviceToDevice, st));
+	crg_launch_instance_boxes(inst, new_insts, reinterpret_cast<const float *>(sc + L.so[ES_ROOTS]), reinterpret_cast<const uint32_t *>(sc + L.so[ES_LAST]), n,
+	                          reinterpret_cast<float *>(sc + L.so[ES_BB]), reinterpret_cast<float *>(sc + L.so[ES_CTR]), reinterpret_cast<float *>(sc + L.so[ES_OFFS]), st);
+	CU(cudaGetLastError());
+	int rc = crg_bvh_build_pairs(reinterpret_cast<const float *>(sc + L.so[ES_BB]), reinterpret_cast<const float *>(sc + L.so[ES_CTR]), n, sc + L.so[ES_BUILD], st,
+	                             reinterpret_cast<PairNode *>(sc + L.so[ES_PAIRS]), reinterpret_cast<int32_t *>(sc + L.so[ES_PRIMS]), res);
+	if (rc) return rc;
+	if (res->levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "BVH deeper than 64 levels");
+	return CRGPU_OK;
+}
+
+/* Copies a built top level over the scene's instances, top region, item records and staged prefix, and the new descriptor to HBM.
+ * The BVH records the items read must already be committed. */
+static int commit_top(crgpu_scene *s, const CrgBuildResult &res) {
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const EditLayout L = edit_layout(s);
+	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
+	cudaStream_t st = s->stream;
+	const DevInstance *new_insts = reinterpret_cast<const DevInstance *>(sc + L.so[ES_NEW_INSTS]);
+	const PairNode *new_pairs = reinterpret_cast<const PairNode *>(sc + L.so[ES_PAIRS]);
+	DevBvh t;
+	memset(&t, 0, sizeof t);
+	t.pair_offset = s->pair_count;
+	t.pair_end = s->pair_count + res.pairs;
+	t.node_count = res.node_count;
+	if (res.node_count == 1u) { memcpy(t.root_bounds, res.bounds, sizeof t.root_bounds); t.root_first = res.root_first; t.root_count = res.root_count; }
+	t.stage_base = s->dev.top.stage_base;
+	t.stage_count = res.pairs < s->top_stage_cap ? res.pairs : s->top_stage_cap;
+	PairNode *top_pairs = static_cast<PairNode *>(s->edit) + s->pair_count;          /* = pairs + t.pair_offset */
+	DevTopItem *top_items = edit_items(s);
+	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), new_insts, L.sz[ES_NEW_INSTS], cudaMemcpyDeviceToDevice, st));
+	if (res.pairs) CU(cudaMemcpyAsync(top_pairs, new_pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	crg_launch_top_items(reinterpret_cast<const int32_t *>(sc + L.so[ES_PRIMS]), new_insts, s->dev.bvhs, n, top_items, st);
+	CU(cudaGetLastError());
+	if (t.stage_count)
+		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + t.stage_base, new_pairs, (size_t)t.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	s->dev.top = t;
+	s->dev.pairs = reinterpret_cast<const PairNode *>(s->edit);
+	s->dev.top_items = top_items;
+	for (int k = 0; k < 3; ++k) {            /* as crgpu_prepare: the root's bounds */
+		const float lo = res.bounds[2 * k], e = res.bounds[2 * k + 1] - lo;
+		s->dev.world_lo[k] = lo;
+		s->dev.world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
+	}
+	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
+	CU(cudaStreamSynchronize(st));
+	return CRGPU_OK;
+}
+
 /* Instance boxes, ray offsets and the top-level BVH of the edited instances are computed on the device, into scratch; only once the
  * build has passed the upload's checks are they copied over the scene's instances, top region and staged prefix, and the top-level
  * item records rebuilt from them. */
@@ -1432,79 +1563,221 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	int rc = drain(s);
 	if (rc) return rc;
 	if (n == 0) return CRGPU_OK;
-	const size_t top_cap = n > 1u ? n - 1u : 1u;
-	auto align = [](size_t b) { return (b + 255u) & ~(size_t)255u; };
-	const size_t pairs_bytes = (size_t)s->pair_count * sizeof(PairNode), top_bytes = top_cap * sizeof(PairNode);
-	/* scratch: the caller's instances, last instance of each object, BVH roots, boxes, centres, offsets, new instance records,
-	 * new top pairs and prims, then the builder's own scratch */
-	const size_t sz[10] = { (size_t)n * sizeof(crs_instance), (size_t)n * 4u, s->bvh_root.size() * sizeof(float), (size_t)n * 24u, (size_t)n * 12u,
-	                        (size_t)n * 4u, (size_t)n * sizeof(DevInstance), top_bytes, (size_t)n * 4u, crg_bvh_scratch_bytes(n) };
-	size_t so[10], total = 0;
-	for (int k = 0; k < 10; ++k) { so[k] = total; total += align(sz[k]); }
-	cudaStream_t st = s->stream;
-	if (!s->edit) {
-		/* the scene's own pairs block: the uploaded pairs (mesh pair offsets do not move), then a top region that holds any top level
-		 * of n instances, then its n item records; the uploaded top level keeps rendering until an edit is committed */
-		const size_t edit_bytes = align(pairs_bytes + top_bytes) + (size_t)n * sizeof(DevTopItem);
-		void *e = nullptr, *q = nullptr;
-		rc = ctx_alloc(s->device, edit_bytes, &e);
-		if (!rc) rc = ctx_alloc(s->device, total, &q);
-		std::vector<uint32_t> last(n);
-		std::unordered_map<uint64_t, uint32_t> last_of;                  /* (kind, object) -> its last instance */
-		for (uint32_t i = n; i-- > 0;) {
-			const uint64_t key = ((uint64_t)s->inst_kind[i] << 32) | s->inst_object[i];
-			last[i] = last_of.emplace(key, i).first->second;
-		}
-		cudaError_t ce = cudaSuccess;
-		if (!rc) ce = cudaMemcpyAsync(e, s->dev.pairs, pairs_bytes, cudaMemcpyDeviceToDevice, st);
-		if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + so[1], last.data(), sz[1], cudaMemcpyHostToDevice, st);
-		if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + so[2], s->bvh_root.data(), sz[2], cudaMemcpyHostToDevice, st);
-		if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-		if (!rc && ce != cudaSuccess) rc = fail(CRGPU_ERR_CUDA, "set_instances: %s", cudaGetErrorString(ce));
-		if (rc) { ctx_free(s->device, e, edit_bytes); ctx_free(s->device, q, total); return rc; }
-		s->edit = e; s->edit_bytes = edit_bytes;
-		s->edit_scratch = q; s->edit_scratch_bytes = total;
-	}
-	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
-	float *bb = reinterpret_cast<float *>(sc + so[3]), *ctr = reinterpret_cast<float *>(sc + so[4]), *offs = reinterpret_cast<float *>(sc + so[5]);
-	DevInstance *new_insts = reinterpret_cast<DevInstance *>(sc + so[6]);
-	PairNode *new_pairs = reinterpret_cast<PairNode *>(sc + so[7]);
-	int32_t *new_prims = reinterpret_cast<int32_t *>(sc + so[8]);
-	CU(cudaMemcpyAsync(sc + so[0], inst, sz[0], cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(new_insts, s->dev.instances, sz[6], cudaMemcpyDeviceToDevice, st));
-	crg_launch_instance_boxes(reinterpret_cast<const crs_instance *>(sc + so[0]), new_insts, reinterpret_cast<const float *>(sc + so[2]),
-	                          reinterpret_cast<const uint32_t *>(sc + so[1]), n, bb, ctr, offs, st);
-	CU(cudaGetLastError());
-	CrgTopResult res;
-	rc = crg_bvh_build_top(bb, ctr, n, sc + so[9], st, new_pairs, new_prims, &res);
+	rc = ensure_edit(s);
 	if (rc) return rc;
-	if (res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "BVH deeper than 64 levels");
+	const EditLayout L = edit_layout(s);
+	crs_instance *dinst = reinterpret_cast<crs_instance *>(static_cast<uint8_t *>(s->edit_scratch) + L.so[ES_INST]);
+	CU(cudaMemcpyAsync(dinst, inst, L.sz[ES_INST], cudaMemcpyHostToDevice, s->stream));
+	CrgBuildResult res;
+	rc = build_top(s, dinst, &res);
+	if (rc) return rc;
+	return commit_top(s, res);
+}
 
-	/* commit */
-	DevBvh t;
-	memset(&t, 0, sizeof t);
-	t.pair_offset = s->pair_count;
-	t.pair_end = s->pair_count + res.pairs;
-	t.node_count = res.node_count;
-	if (res.node_count == 1u) { memcpy(t.root_bounds, res.bounds, sizeof t.root_bounds); t.root_first = res.root_first; t.root_count = res.root_count; }
-	t.stage_base = s->dev.top.stage_base;
-	t.stage_count = res.pairs < s->top_stage_cap ? res.pairs : s->top_stage_cap;
-	PairNode *top_pairs = static_cast<PairNode *>(s->edit) + s->pair_count;          /* = pairs + t.pair_offset */
-	DevTopItem *top_items = reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->edit) + align(pairs_bytes + top_bytes));
-	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), new_insts, sz[6], cudaMemcpyDeviceToDevice, st));
-	if (res.pairs) CU(cudaMemcpyAsync(top_pairs, new_pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	crg_launch_top_items(new_prims, new_insts, s->dev.bvhs, n, top_items, st);
-	CU(cudaGetLastError());
-	if (t.stage_count)
-		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + t.stage_base, new_pairs, (size_t)t.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	s->dev.top = t;
-	s->dev.pairs = reinterpret_cast<const PairNode *>(s->edit);
-	s->dev.top_items = top_items;
-	for (int k = 0; k < 3; ++k) {            /* as crgpu_prepare: the root's bounds */
-		const float lo = res.bounds[2 * k], e = res.bounds[2 * k + 1] - lo;
-		s->dev.world_lo[k] = lo;
-		s->dev.world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
+/* ---- mesh edits ---------------------------------------------------------------------------------------------------------------------
+ * What one listed mesh reads from the caller's flat scene: its polys and the index ranges of vertices, normals and texcoords they use
+ * (checked as crgpu_prepare checks them), and where its inputs and rebuilt records sit in the mesh scratch. */
+struct MeshEdit {
+	uint32_t mesh, bvh, n;
+	uint32_t vlo, vhi, nlo, nhi, tlo, thi;          /* [lo, hi) index ranges; hi == lo: none */
+	size_t o_polys, o_verts, o_norms, o_uvs, o_bb, o_ctr, o_pairs, o_prims, o_tris, o_slot, o_keys, o_spolys;
+	CrgBuildResult res;
+};
+
+static int check_mesh_polys(const crs_scene *f, const crs_mesh &mesh, MeshEdit &e) {
+	struct Range { uint32_t lo = 0xffffffffu, hi = 0u; void add(int32_t i) { if ((uint32_t)i < lo) lo = (uint32_t)i; if ((uint32_t)i + 1u > hi) hi = (uint32_t)i + 1u; } };
+	HostError herr;
+	std::mutex merge;
+	Range V, N, T;
+	host_parallel_for(mesh.poly_count, [&](uint32_t lo, uint32_t hi) {
+		Range v, nn, t;
+		for (uint32_t i = lo; i < hi; ++i) {
+			const crs_poly &p = f->polys[mesh.poly_offset + i];
+			for (int k = 0; k < 3; ++k) {
+				if (p.v[k] < 0 || (uint32_t)p.v[k] >= f->vertex_count) { herr.set(CRGPU_ERR_BAD_ARGUMENT, "vertex index out of range"); return; }
+				v.add(p.v[k]);
+			}
+			if (p.has_normals)
+				for (int k = 0; k < 3; ++k) {
+					if (p.n[k] < 0 || (uint32_t)p.n[k] >= f->normal_count) { herr.set(CRGPU_ERR_BAD_ARGUMENT, "normal index out of range"); return; }
+					nn.add(p.n[k]);
+				}
+			if (mesh.texcoord_count != 0 && p.t[0] != -1)                                  /* instance.c:151-153 */
+				for (int k = 0; k < 3; ++k) {
+					if (p.t[k] < 0 || (uint32_t)p.t[k] >= f->texcoord_count) { herr.set(CRGPU_ERR_BAD_ARGUMENT, "texcoord index out of range"); return; }
+					t.add(p.t[k]);
+				}
+			if (p.material >= mesh.material_count) { herr.set(CRGPU_ERR_BAD_ARGUMENT, "poly material index out of range"); return; }
+		}
+		std::lock_guard<std::mutex> g(merge);
+		for (auto pr : { std::make_pair(&V, &v), std::make_pair(&N, &nn), std::make_pair(&T, &t) })
+			if (pr.second->hi) { if (pr.second->lo < pr.first->lo) pr.first->lo = pr.second->lo; if (pr.second->hi > pr.first->hi) pr.first->hi = pr.second->hi; }
+	});
+	if (herr.code) return fail(herr.code, "%s", herr.msg);
+	e.vlo = V.hi ? V.lo : 0u; e.vhi = V.hi ? V.hi : 0u;
+	e.nlo = N.hi ? N.lo : 0u; e.nhi = N.hi ? N.hi : 0u;
+	e.tlo = T.hi ? T.lo : 0u; e.thi = T.hi ? T.hi : 0u;
+	return CRGPU_OK;
+}
+
+/* Gives the edit block room for `add` more pair nodes behind its current ones (the queued work has been drained). */
+static int grow_edit(crgpu_scene *s, uint32_t add) {
+	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const uint32_t pairs = s->edit_pairs + add;
+	const size_t bytes = align256((size_t)pairs * sizeof(PairNode)) + (size_t)n * sizeof(DevTopItem);
+	void *e = nullptr;
+	int rc = ctx_alloc(s->device, bytes, &e);
+	if (rc) return rc;
+	cudaStream_t st = s->stream;
+	const DevTopItem *old_items = edit_items(s);
+	cudaError_t ce = cudaMemcpyAsync(e, s->edit, (size_t)s->edit_pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st);
+	if (ce == cudaSuccess && n)
+		ce = cudaMemcpyAsync(static_cast<uint8_t *>(e) + align256((size_t)pairs * sizeof(PairNode)), old_items, (size_t)n * sizeof(DevTopItem), cudaMemcpyDeviceToDevice, st);
+	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (ce != cudaSuccess) { ctx_free(s->device, e, bytes); return fail(CRGPU_ERR_CUDA, "set_meshes: %s", cudaGetErrorString(ce)); }
+	ctx_free(s->device, s->edit, s->edit_bytes);
+	const bool live = s->dev.pairs == s->edit;
+	s->edit = e; s->edit_bytes = bytes; s->edit_pairs = pairs;
+	if (live) { s->dev.pairs = static_cast<const PairNode *>(e); s->dev.top_items = edit_items(s); }
+	return CRGPU_OK;
+}
+
+/* Each listed mesh's triangle boxes, BVH, triangles, slot records and shading records, then the instances and the top level, are
+ * rebuilt on the device into scratch; only once every build has passed the upload's checks are they copied over the scene. */
+extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count) {
+	if (!s || !flat || (count && !meshes)) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	const uint32_t nm = (uint32_t)s->meshes.size();
+	std::vector<uint8_t> listed(nm, 0u);
+	std::vector<MeshEdit> edits;
+	for (uint32_t k = 0; k < count; ++k) {
+		const uint32_t m = meshes[k];
+		if (m >= nm || m >= flat->mesh_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u out of range (the scene has %u)", m, nm);
+		if (listed[m]) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u listed twice", m);
+		listed[m] = 1u;
+		const crs_mesh &a = s->meshes[m], &b = flat->meshes[m];
+		if (a.poly_offset != b.poly_offset || a.poly_count != b.poly_count || a.material_offset != b.material_offset || a.material_count != b.material_count ||
+		    a.texcoord_count != b.texcoord_count || a.bvh != b.bvh)
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its record differs from the uploaded one (the topology cannot change)", m);
+		if (a.bvh >= s->bvh_prims.size() || s->bvh_prims[a.bvh] != a.poly_count)
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its uploaded BVH does not cover exactly its polys", m);
+		if ((uint64_t)b.poly_offset + b.poly_count > flat->poly_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u ranges out of bounds", m);
+		if (a.poly_count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: %u polys (the device builder's limit is 4194304)", m, a.poly_count);
+		MeshEdit e;
+		memset(&e, 0, sizeof e);
+		e.mesh = m; e.bvh = a.bvh; e.n = a.poly_count;
+		int rc = check_mesh_polys(flat, b, e);
+		if (rc) return rc;
+		if (e.n) edits.push_back(e);
 	}
+	int rc = drain(s);
+	if (rc) return rc;
+	if (edits.empty()) return CRGPU_OK;
+	rc = ensure_edit(s);
+	if (rc) return rc;
+
+	/* the mesh scratch: every listed mesh's inputs and records, then the builder's scratch for the largest */
+	size_t total = 0;
+	uint32_t nmax = 0;
+	auto take = [&](size_t bytes) { const size_t o = total; total += align256(bytes); return o; };
+	for (MeshEdit &e : edits) {
+		e.o_polys = take((size_t)e.n * sizeof(crs_poly));
+		e.o_verts = take((size_t)(e.vhi - e.vlo) * 12u); e.o_norms = take((size_t)(e.nhi - e.nlo) * 12u); e.o_uvs = take((size_t)(e.thi - e.tlo) * 8u);
+		e.o_bb = take((size_t)e.n * 24u); e.o_ctr = take((size_t)e.n * 12u);
+		e.o_pairs = take((size_t)(e.n > 1u ? e.n - 1u : 1u) * sizeof(PairNode)); e.o_prims = take((size_t)e.n * 4u);
+		e.o_tris = take((size_t)e.n * sizeof(PackedTri)); e.o_slot = take((size_t)e.n * 4u); e.o_keys = take(e.n);
+		e.o_spolys = take((size_t)e.n * sizeof(ShadePoly));
+		if (e.n > nmax) nmax = e.n;
+	}
+	const size_t o_build = take(crg_bvh_scratch_bytes(nmax));
+	if (total > s->mesh_scratch_bytes) {
+		void *q = nullptr;
+		rc = ctx_alloc(s->device, total, &q);
+		if (rc) return rc;
+		ctx_free(s->device, s->mesh_scratch, s->mesh_scratch_bytes);
+		s->mesh_scratch = q; s->mesh_scratch_bytes = total;
+	}
+	uint8_t *sc = static_cast<uint8_t *>(s->mesh_scratch);
+	cudaStream_t st = s->stream;
+	for (MeshEdit &e : edits) {
+		const crs_mesh &mesh = flat->meshes[e.mesh];
+		CU(cudaMemcpyAsync(sc + e.o_polys, flat->polys + mesh.poly_offset, (size_t)e.n * sizeof(crs_poly), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(sc + e.o_verts, flat->vertices + 3 * (size_t)e.vlo, (size_t)(e.vhi - e.vlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.nhi > e.nlo) CU(cudaMemcpyAsync(sc + e.o_norms, flat->normals + 3 * (size_t)e.nlo, (size_t)(e.nhi - e.nlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.thi > e.tlo) CU(cudaMemcpyAsync(sc + e.o_uvs, flat->texcoords + 2 * (size_t)e.tlo, (size_t)(e.thi - e.tlo) * 8u, cudaMemcpyHostToDevice, st));
+		const crs_poly *polys = reinterpret_cast<const crs_poly *>(sc + e.o_polys);
+		float *bb = reinterpret_cast<float *>(sc + e.o_bb), *ctr = reinterpret_cast<float *>(sc + e.o_ctr);
+		crg_launch_poly_boxes(polys, reinterpret_cast<const float *>(sc + e.o_verts), e.vlo, e.n, bb, ctr, st);
+		CU(cudaGetLastError());
+		int32_t *prims = reinterpret_cast<int32_t *>(sc + e.o_prims);
+		rc = crg_bvh_build_pairs(bb, ctr, e.n, sc + o_build, st, reinterpret_cast<PairNode *>(sc + e.o_pairs), prims, &e.res);
+		if (rc) return rc;
+		if (e.res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: BVH deeper than 64 levels", e.mesh);
+		const CrgMeshRepack r = { polys, reinterpret_cast<const float *>(sc + e.o_verts), reinterpret_cast<const float *>(sc + e.o_norms),
+		                          reinterpret_cast<const float *>(sc + e.o_uvs), e.vlo, e.nlo, e.tlo, e.n, mesh.poly_offset, mesh.material_offset,
+		                          mesh.texcoord_count };
+		crg_launch_mesh_repack(r, prims, reinterpret_cast<PackedTri *>(sc + e.o_tris), reinterpret_cast<uint32_t *>(sc + e.o_slot), sc + e.o_keys,
+		                       reinterpret_cast<ShadePoly *>(sc + e.o_spolys), st);
+		CU(cudaGetLastError());
+	}
+
+	/* the top level over the new mesh roots, built from the roots in the instance scratch (restored if anything below fails) */
+	const uint32_t ninst = (uint32_t)s->inst_kind.size();
+	std::vector<float> roots = s->bvh_root;
+	for (const MeshEdit &e : edits) memcpy(&roots[6 * (size_t)e.bvh], e.res.bounds, 6 * sizeof(float));
+	const EditLayout L = edit_layout(s);
+	float *droots = reinterpret_cast<float *>(static_cast<uint8_t *>(s->edit_scratch) + L.so[ES_ROOTS]);
+	auto undo = [&](int code) {
+		cudaMemcpyAsync(droots, s->bvh_root.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st);
+		cudaStreamSynchronize(st);
+		return code;
+	};
+	CU(cudaMemcpyAsync(droots, roots.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st));
+	CrgBuildResult top;
+	memset(&top, 0, sizeof top);
+	if (ninst) {
+		rc = build_top(s, nullptr, &top);
+		if (rc) return undo(rc);
+	}
+	uint32_t add = 0;
+	for (const MeshEdit &e : edits) if (s->mesh_region[e.mesh] == 0xffffffffu) add += e.n > 1u ? e.n - 1u : 1u;
+	if (add) {
+		const uint32_t first = s->edit_pairs;
+		if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return undo(fail(CRGPU_ERR_UNSUPPORTED, "set_meshes: more pair nodes than the scene can address"));
+		rc = grow_edit(s, add);
+		if (rc) return undo(rc);
+		uint32_t next = first;
+		for (const MeshEdit &e : edits)
+			if (s->mesh_region[e.mesh] == 0xffffffffu) { s->mesh_region[e.mesh] = next; next += e.n > 1u ? e.n - 1u : 1u; }
+	}
+
+	/* commit: each mesh's region, slot and poly ranges, BVH record and staged prefix, then the instances and the top level */
+	PairNode *pairs = static_cast<PairNode *>(s->edit);
+	for (const MeshEdit &e : edits) {
+		const crs_mesh &mesh = s->meshes[e.mesh];
+		DevBvh &b = s->bvhs[e.bvh];
+		const PairNode *staged = reinterpret_cast<const PairNode *>(sc + e.o_pairs);
+		const uint32_t region = s->mesh_region[e.mesh];
+		if (e.res.pairs) CU(cudaMemcpyAsync(pairs + region, staged, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<PackedTri *>(s->dev.tris) + b.slot_offset, sc + e.o_tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<uint32_t *>(s->dev.slot_poly) + b.slot_offset, sc + e.o_slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.slot_key) + b.slot_offset, sc + e.o_keys, e.n, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<ShadePoly *>(s->dev.spolys) + mesh.poly_offset, sc + e.o_spolys, (size_t)e.n * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
+		const uint32_t slot_offset = b.slot_offset, stage_base = b.stage_base;
+		memset(&b, 0, sizeof b);
+		b.pair_offset = region;
+		b.pair_end = region + e.res.pairs;
+		b.node_count = e.res.node_count;
+		b.slot_offset = slot_offset;
+		if (e.res.node_count == 1u) { memcpy(b.root_bounds, e.res.bounds, sizeof b.root_bounds); b.root_first = e.res.root_first; b.root_count = e.res.root_count; }
+		b.stage_base = stage_base;
+		b.stage_count = e.res.pairs < s->stage_cap[e.bvh] ? e.res.pairs : s->stage_cap[e.bvh];
+		CU(cudaMemcpyAsync(const_cast<DevBvh *>(s->dev.bvhs) + e.bvh, &b, sizeof b, cudaMemcpyHostToDevice, st));
+		if (b.stage_count)
+			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, staged, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	}
+	s->bvh_root = roots;
+	if (ninst) return commit_top(s, top);
+	s->dev.pairs = pairs;
 	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
 	CU(cudaStreamSynchronize(st));
 	return CRGPU_OK;

@@ -357,11 +357,11 @@ __global__ void k_scan_add(unsigned long long *out, const unsigned long long *__
 	if (i < n && blk > 0u) out[i] += sums_incl[blk - 1u];
 }
 
-/* ---- the pair layout of an edited scene's top level (crgpu_api.cu build_pairs, on the device) ----------------------------------------
+/* ---- the pair layout of an edited scene's BVHs, top level or mesh (crgpu_api.cu build_pairs, on the device) ------------------------
  * build_pairs numbers internal nodes in BFS order, children left before right.  Records are created level by level, but in atomic
  * order within a level, so one block walks the levels in BFS order: per level, an exclusive block scan of the internal-child counts
  * of the level's internal nodes (in their BFS order) places their internal children in the next level. */
-__global__ void __launch_bounds__(1024) k_top_bfs(const Rec *__restrict__ recs, uint32_t *order, uint32_t *bfs_of, uint32_t *info) {
+__global__ void __launch_bounds__(1024) k_pair_bfs(const Rec *__restrict__ recs, uint32_t *order, uint32_t *bfs_of, uint32_t *info) {
 	__shared__ uint32_t s_warp[32];
 	const unsigned lane = threadIdx.x & 31u, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
 	if (threadIdx.x == 0) { order[0] = 0u; bfs_of[0] = 0u; }
@@ -393,7 +393,7 @@ __global__ void __launch_bounds__(1024) k_top_bfs(const Rec *__restrict__ recs, 
 	}
 	if (threadIdx.x == 0) { info[0] = tail; info[1] = levels; }
 }
-__global__ void k_top_pairs(const Rec *__restrict__ recs, const uint32_t *__restrict__ order, const uint32_t *__restrict__ bfs_of, uint32_t count,
+__global__ void k_pairs(const Rec *__restrict__ recs, const uint32_t *__restrict__ order, const uint32_t *__restrict__ bfs_of, uint32_t count,
 							PairNode *pairs) {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= count) return;
@@ -536,8 +536,8 @@ static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scrat
 
 size_t crg_bvh_scratch_bytes(uint32_t n) { Scratch s; return carve(nullptr, n, &s); }
 
-int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, void *scratch, cudaStream_t st, PairNode *pairs_out, int32_t *prims_out,
-					  CrgTopResult *out) {
+int crg_bvh_build_pairs(const float *bb, const float *ctr, uint32_t n, void *scratch, cudaStream_t st, PairNode *pairs_out, int32_t *prims_out,
+					  CrgBuildResult *out) {
 	memset(out, 0, sizeof *out);
 	if (n == 0u) return CRGPU_OK;
 	if (n > 4194304u) return crg_fail(CRGPU_ERR_UNSUPPORTED, "crgpu_bvh_build: %u primitives (limit 4194304 per call)", n);
@@ -552,9 +552,9 @@ int crg_bvh_build_top(const float *bb, const float *ctr, uint32_t n, void *scrat
 		return crg_fail(CRGPU_ERR_UNSUPPORTED, "crgpu_bvh_build: the tree of %u primitives needs %u nodes, more than 2n - 1", n, nrec);
 	uint32_t info[2] = { 0u, 0u };
 	if (nrec > 1u) {
-		k_top_bfs<<<1, 1024, 0, st>>>(rs.recs, s.order, s.bfs_of, s.info);
+		k_pair_bfs<<<1, 1024, 0, st>>>(rs.recs, s.order, s.bfs_of, s.info);
 		const uint32_t internal = (nrec - 1u) / 2u;                   /* a full binary tree */
-		k_top_pairs<<<(internal + 255u) / 256u, 256, 0, st>>>(rs.recs, s.order, s.bfs_of, internal, pairs_out);
+		k_pairs<<<(internal + 255u) / 256u, 256, 0, st>>>(rs.recs, s.order, s.bfs_of, internal, pairs_out);
 		CUB(cudaMemcpyAsync(info, s.info, sizeof info, cudaMemcpyDeviceToHost, st));
 	}
 	CUB(cudaMemcpyAsync(prims_out, s.prims, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
@@ -627,10 +627,9 @@ __global__ void k_instance_boxes(const crs_instance *__restrict__ inst, DevInsta
 								 float *bb, float *ctr, float *offs) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
-	const crs_instance &s = inst[i];
 	DevInstance &d = insts[i];
-	for (int k = 0; k < 12; ++k) { d.A[k] = s.A[k]; d.Ainv[k] = s.Ainv[k]; }
-	const float *m = s.A;                                                     /* row-major 4x4: m[4 * row + col] */
+	if (inst) for (int k = 0; k < 12; ++k) { d.A[k] = inst[i].A[k]; d.Ainv[k] = inst[i].Ainv[k]; }
+	const float *m = d.A;                                                     /* rows 0-2 of the row-major 4x4: m[4 * row + col] */
 	float mn[3], mx[3];
 	if (d.kind == CRS_INST_MESH) {
 		const float *b = bvh_root + 6 * (size_t)d.bvh;
@@ -666,7 +665,8 @@ void crg_launch_instance_boxes(const crs_instance *inst, DevInstance *insts, con
 	k_instance_offsets<<<(n + 255u) / 256u, 256, 0, st>>>(insts, last, offs, n);
 }
 
-/* the edit's item records, from the committed instances' new state and the mesh BVHs (which an instance edit never moves) */
+/* the edit's item records, from the committed instances' new state and the committed mesh BVH records (a mesh edit moves the pair
+ * nodes of the meshes it rebuilds, and may change their node counts and staged prefixes, so those records are written first) */
 __global__ void k_top_items(const int32_t *__restrict__ prims, const DevInstance *__restrict__ insts, const DevBvh *__restrict__ bvhs, uint32_t n,
                             DevTopItem *__restrict__ items) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -674,4 +674,78 @@ __global__ void k_top_items(const int32_t *__restrict__ prims, const DevInstance
 }
 void crg_launch_top_items(const int32_t *prims, const DevInstance *insts, const DevBvh *bvhs, uint32_t n, DevTopItem *items, cudaStream_t st) {
 	if (n) k_top_items<<<(n + 255u) / 256u, 256, 0, st>>>(prims, insts, bvhs, n, items);
+}
+
+/* ---- a mesh edit's bottom level: poly_bbox, then the records crgpu_prepare packs, in the new leaf order ---------------------------
+ * Plain fp32 operations in the loader's / crgpu_prepare's order; -fmad=false keeps the products unfused. */
+__global__ void k_poly_boxes(const crs_poly *__restrict__ polys, const float *__restrict__ verts, uint32_t vbase, uint32_t n, float *bb, float *ctr) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const crs_poly &p = polys[i];
+	const float *v0 = verts + 3 * (size_t)((uint32_t)p.v[0] - vbase), *v1 = verts + 3 * (size_t)((uint32_t)p.v[1] - vbase),
+	            *v2 = verts + 3 * (size_t)((uint32_t)p.v[2] - vbase);
+	for (int k = 0; k < 3; ++k) {
+		bb[6 * (size_t)i + k] = MACRO_MIN(v0[k], MACRO_MIN(v1[k], v2[k]));
+		bb[6 * (size_t)i + 3 + k] = MACRO_MAX(v0[k], MACRO_MAX(v1[k], v2[k]));
+		ctr[3 * (size_t)i + k] = ((v0[k] + v1[k]) + v2[k]) * (1.0f / 3.0f);
+	}
+}
+void crg_launch_poly_boxes(const crs_poly *polys, const float *verts, uint32_t vbase, uint32_t n, float *bb, float *ctr, cudaStream_t st) {
+	if (n) k_poly_boxes<<<(n + 255u) / 256u, 256, 0, st>>>(polys, verts, vbase, n, bb, ctr);
+}
+
+__device__ __forceinline__ void cross_unfused(const float *a, const float *b, float *out) {            /* poly.c:22 */
+	out[0] = a[1] * b[2] - a[2] * b[1]; out[1] = a[2] * b[0] - a[0] * b[2]; out[2] = a[0] * b[1] - a[1] * b[0];
+}
+__device__ __forceinline__ void edges(const CrgMeshRepack &m, const crs_poly &p, float *v0, float *e1, float *e2) {   /* poly.c:20-21 */
+	const float *a = m.verts + 3 * (size_t)((uint32_t)p.v[0] - m.vbase), *b = m.verts + 3 * (size_t)((uint32_t)p.v[1] - m.vbase),
+	            *c = m.verts + 3 * (size_t)((uint32_t)p.v[2] - m.vbase);
+	for (int k = 0; k < 3; ++k) { v0[k] = a[k]; e1[k] = a[k] - b[k]; e2[k] = c[k] - a[k]; }
+}
+/* slot i of the mesh: crgpu_prepare step (2) and the shading key */
+__global__ void k_mesh_slots(const CrgMeshRepack m, const int32_t *__restrict__ prims, PackedTri *tris, uint32_t *slot_poly, uint8_t *keys) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= m.n) return;
+	const uint32_t local = (uint32_t)prims[i];
+	const crs_poly &p = m.polys[local];
+	PackedTri t;
+	edges(m, p, t.v0, t.e1, t.e2);
+	cross_unfused(t.e1, t.e2, t.n);
+	tris[i] = t;
+	slot_poly[i] = m.poly_offset + local;
+	const uint32_t material = m.material_offset + p.material;
+	keys[i] = (uint8_t)(material + 1u < 255u ? material + 1u : 255u);
+}
+/* poly j of the mesh: crgpu_prepare step (3) */
+__global__ void k_mesh_spolys(const CrgMeshRepack m, ShadePoly *spolys) {
+	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= m.n) return;
+	const crs_poly &p = m.polys[j];
+	ShadePoly sp;
+	memset(&sp, 0, sizeof sp);
+	const bool has_n = p.has_normals != 0;
+	if (has_n) {
+		float *dst[3] = { sp.n0, sp.n1, sp.n2 };
+		for (int v = 0; v < 3; ++v)
+			for (int k = 0; k < 3; ++k) dst[v][k] = m.normals[3 * (size_t)((uint32_t)p.n[v] - m.nbase) + k];
+	} else {                                                                  /* geometric normal e1 x e2 (poly.c:22,46) */
+		float v0[3], e1[3], e2[3];
+		edges(m, p, v0, e1, e2);
+		cross_unfused(e1, e2, sp.n0);
+	}
+	const bool has_uv = m.texcoord_count != 0u && p.t[0] != -1;                 /* instance.c:151-153 */
+	if (has_uv) {
+		float *dst[3] = { sp.t0, sp.t1, sp.t2 };
+		for (int v = 0; v < 3; ++v)
+			for (int k = 0; k < 2; ++k) dst[v][k] = m.uvs[2 * (size_t)((uint32_t)p.t[v] - m.tbase) + k];
+	}
+	sp.material = m.material_offset + p.material;
+	sp.flags = (has_n ? 1u : 0u) | (has_uv ? 2u : 0u);
+	spolys[j] = sp;
+}
+void crg_launch_mesh_repack(const CrgMeshRepack &m, const int32_t *prims, PackedTri *tris, uint32_t *slot_poly, uint8_t *keys, ShadePoly *spolys,
+                            cudaStream_t st) {
+	if (!m.n) return;
+	k_mesh_slots<<<(m.n + 255u) / 256u, 256, 0, st>>>(m, prims, tris, slot_poly, keys);
+	k_mesh_spolys<<<(m.n + 255u) / 256u, 256, 0, st>>>(m, spolys);
 }

@@ -177,10 +177,26 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *                              room for any top level of `count` instances); later calls reuse it.  A top level that needs more
  *                              than count - 1 pair nodes (a tree of more than 2 count - 1 nodes, which only instances whose boxes no
  *                              split separates make: see crloader_build_bvh in crloader.h) is refused with CRGPU_ERR_UNSUPPORTED.
+ *   crgpu_scene_set_meshes     deforms meshes (crTransformMesh, "recompute kd-tree"): every mesh listed in `meshes` takes its polys,
+ *                              flat->polys[poly_offset .. + poly_count), and the vertices, normals and texture coordinates they
+ *                              index from `flat`; positions, normals, uvs and each poly's material (within the mesh's material
+ *                              range) may change.  Nothing else in `flat` is read: its BVHs and ray offsets are ignored and rebuilt.
+ *                              Exactly the listed meshes are rebuilt: a vertex shared with an unlisted mesh does not move that mesh.
+ *                              Each listed mesh's record must equal the uploaded one in poly_offset, poly_count, material_offset,
+ *                              material_count, texcoord_count and bvh, and its uploaded BVH must cover exactly its polys; a mesh
+ *                              out of range, a mesh listed twice, an index out of range or a material outside the mesh's range is
+ *                              refused with CRGPU_ERR_BAD_ARGUMENT, as crgpu_prepare refuses them.  On the device, each mesh's
+ *                              triangle boxes, BVH (the tree the scene loader builds), leaf-ordered triangles and shading records are
+ *                              rebuilt, then every instance's box and ray offset under its current transform (an earlier
+ *                              crgpu_scene_set_instances included) and the top level.  A mesh tree of more than 2n - 1 nodes
+ *                              (crloader_build_bvh), deeper than 64 levels, or of more than 4,194,304 polys is refused with
+ *                              CRGPU_ERR_UNSUPPORTED.  The first edit of a mesh gives it its own region of max(1, n - 1) pair nodes
+ *                              behind the scene's other pairs; later edits reuse it.
  * Edits apply to this device scene only: the crgpu_prepared it was created from, and any scene created from that later, are
  * unedited. */
 int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam);
 int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
+int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count);
 
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
