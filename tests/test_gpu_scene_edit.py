@@ -71,21 +71,22 @@ def scene_json(name):
     return json.load(open(path))
 
 
-def load(doc):
-    """A FlatScene from JSON text, with assets resolved as the bundled scenes are (oracle_lib.bundled_scene)."""
-    cwd = os.getcwd()
-    os.chdir(REFDIR)
+def load(doc, cwd=REFDIR, asset_path="input"):
+    """A FlatScene from JSON text, with assets resolved as the bundled scenes are (oracle_lib.bundled_scene) unless the scene's own
+    working directory and mesh directory are given."""
+    here = os.getcwd()
+    os.chdir(cwd)
     try:
-        return crscene.load_json_buf(json.dumps(doc), "input")
+        return crscene.load_json_buf(json.dumps(doc), asset_path)
     finally:
-        os.chdir(cwd)
+        os.chdir(here)
 
 
 class Loaded:
     """A flat scene configured at W x H x spp, bounces, with its camera and instances kept for edits."""
 
-    def __init__(self, doc, W, H, spp, b):
-        self.flat = load(doc)
+    def __init__(self, doc, W, H, spp, b, cwd=REFDIR, asset_path="input"):
+        self.flat = load(doc, cwd, asset_path)
         crgpu.lib().crscene_set_config(C.byref(self.flat), W, H, spp, b)
         self.cfg = (W, H, spp, b)
         self.camera = crgpu.Camera.from_buffer_copy(self.flat.camera)
