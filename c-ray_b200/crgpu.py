@@ -142,6 +142,10 @@ def lib():
         if hasattr(L, "crgpu_scene_set_meshes"):   # absent from libraries built before mesh edits
             L.crgpu_scene_set_meshes.argtypes = [P, C.POINTER(FlatScene), P, C.c_uint32]
             L.crgpu_scene_set_meshes.restype = C.c_int
+        if hasattr(L, "crgpu_scene_set_shading"):  # absent from libraries built before shading edits
+            L.crgpu_scene_set_shading.argtypes = [P, C.POINTER(FlatScene)]
+            L.crgpu_scene_shading.argtypes = [P, P, P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
+            L.crgpu_scene_set_shading.restype = L.crgpu_scene_shading.restype = C.c_int
         _lib = L
     return _lib
 
@@ -276,6 +280,20 @@ class GpuScene:
         idx = np.ascontiguousarray(meshes, dtype=np.uint32).reshape(-1)
         _check(lib().crgpu_scene_set_meshes(self.handle, C.byref(flat), idx.ctypes.data if len(idx) else None, len(idx)),
                "crgpu_scene_set_meshes")
+
+    def set_shading(self, flat):
+        """Replace the materials, node graph, textures, texel data and background of the resident scene with those of the FlatScene
+        `flat` (crgpu_scene_set_shading): same material count, everything else of `flat` is ignored."""
+        _check(lib().crgpu_scene_set_shading(self.handle, C.byref(flat)), "crgpu_scene_set_shading")
+
+    def shading(self):
+        """How the shading kernels sample the live scene (crgpu_scene_shading): dict of kinds and flags (uint32 per material, as
+        crgpu_prepared_materials gives them), background_kind and complete_interpreter."""
+        n, bg, x = C.c_uint32(0), C.c_uint32(0), C.c_int(0)
+        _check(lib().crgpu_scene_shading(self.handle, None, None, 0, C.byref(n), C.byref(bg), C.byref(x)), "crgpu_scene_shading")
+        kinds, flags = np.zeros(n.value, np.uint32), np.zeros(n.value, np.uint32)
+        _check(lib().crgpu_scene_shading(self.handle, kinds.ctypes.data, flags.ctypes.data, n.value, None, None, None), "crgpu_scene_shading")
+        return {"kinds": kinds, "flags": flags, "background_kind": bg.value, "complete_interpreter": bool(x.value)}
 
     def set_stream(self, cuda_stream_ptr):
         """Enqueue on a caller-owned cudaStream_t (int pointer, e.g. torch.cuda.current_stream().cuda_stream)."""

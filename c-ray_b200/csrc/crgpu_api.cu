@@ -220,6 +220,10 @@ struct crgpu_scene {
 	std::vector<uint32_t> stage_cap;           /* staged pairs reserved for each BVH at upload */
 	std::vector<uint32_t> mesh_region;         /* first pair of a mesh's own region in the edit block (UINT32_MAX: none yet) */
 	void *mesh_scratch; size_t mesh_scratch_bytes;   /* a mesh edit's inputs, its rebuilt records and the builder's scratch */
+	/* shading edits (crgpu_scene_set_shading) */
+	uint32_t material_count;   /* as uploaded: an edit must keep it */
+	void *shade; size_t shade_bytes;           /* NULL until the first shading edit: the node graph, texture table and texel data the
+	                                              kernels read in place of the slab's */
 };
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
@@ -442,6 +446,80 @@ static DevFlatBg fold_background(const crs_scene *f, int root) {
 	return b;
 }
 
+/* ---- the shading fold: everything the kernels read about materials, the node graph, textures and the background --------------
+ * crgpu_prepare and crgpu_scene_set_shading both take these records from here, so an edited scene holds the bytes a fresh prepare
+ * of the same arrays would.  Reads material_count, materials, node_count, nodes, texture_count, textures, texdata_bytes and
+ * background of `f`; validates them as an upload must (the error is the one crgpu_prepare returns). */
+struct ShadingFold {
+	bool xnodes;                       /* some node is of a kind only the complete interpreter (NodeX) evaluates */
+	DevFlatBg bg;
+	std::vector<DevMaterial> mats;
+	std::vector<DevFlat> flat;
+	std::vector<DevTexture> texs;      /* data = byte offset into texdata (patched with a device address at upload) */
+	std::vector<uint8_t> order;        /* K4's bucket order, 256 keys */
+	uint32_t flat_keys;
+};
+
+static int fold_shading(const crs_scene *f, ShadingFold &out) {
+	if (!node_ok(f, f->background) || f->nodes[f->background].kind != CRS_BSDF_BACKGROUND)
+		return fail(CRGPU_ERR_UNSUPPORTED, "scene background must be a background node");
+	out.xnodes = false;
+	for (uint32_t i = 0; i < f->node_count; ++i) {
+		const int k = f->nodes[i].kind;
+		if (k == CRS_COLOR_VECTOCOLOR || k == CRS_COLOR_COMBINE_VALUE || k == CRS_COLOR_COMBINE_RGB || k == CRS_VALUE_MATH || k == CRS_VALUE_FRESNEL ||
+			k == CRS_VALUE_RAYLENGTH || k == CRS_VECTOR_CONSTANT || k == CRS_VECTOR_NORMAL || k == CRS_VECTOR_VECMATH) out.xnodes = true;
+	}
+	out.bg = fold_background(f, f->background);
+	int rc;
+	{
+		bool uv = false;
+		if ((rc = check_bsdf(f, f->background, 0, 0, &uv))) return rc;
+	}
+	out.mats.resize(f->material_count);
+	out.flat.resize(f->material_count);
+	for (uint32_t i = 0; i < f->material_count; ++i) {
+		const crs_material &m = f->materials[i];
+		bool uv = false;
+		if ((rc = check_bsdf(f, m.bsdf, 0, 0, &uv))) return rc;
+		DevMaterial d;
+		memset(&d, 0, sizeof d);
+		d.emission[0] = m.emission[0]; d.emission[1] = m.emission[1]; d.emission[2] = m.emission[2];
+		d.IOR = m.IOR; d.bsdf = m.bsdf;
+		/* x + w*0 == x bit-for-bit for finite w, so only non-zero (or non-finite) emission needs the add */
+		const bool emits = !(m.emission[0] == 0.0f && m.emission[1] == 0.0f && m.emission[2] == 0.0f);
+		d.flags = (uv ? 1u : 0u) | (emits ? 2u : 0u);
+		out.mats[i] = d;
+		out.flat[i] = fold_flat(f, m.bsdf);
+	}
+	out.texs.resize(f->texture_count);
+	for (uint32_t i = 0; i < f->texture_count; ++i) {
+		const crs_texture &t = f->textures[i];
+		const uint64_t bytes = (uint64_t)t.width * t.height * t.channels * (t.is_float ? 4u : 1u);
+		if (t.width == 0 || t.height == 0 || t.channels == 0 || t.channels > 4 || t.width > 65536u || t.height > 65536u ||
+			t.data_offset > f->texdata_bytes || bytes > f->texdata_bytes - t.data_offset) {
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "texture %u malformed", i);
+		}
+		DevTexture d;
+		d.width = t.width; d.height = t.height; d.channels = t.channels; d.is_float = t.is_float; d.has_alpha = t.has_alpha; d.pad = 0;
+		d.wmask = (t.width & (t.width - 1u)) == 0u ? t.width - 1u : 0u;
+		d.hmask = (t.height & (t.height - 1u)) == 0u ? t.height - 1u : 0u;
+		d.data = reinterpret_cast<const uint8_t *>((uintptr_t)t.data_offset);
+		out.texs[i] = d;
+	}
+	for (uint32_t i = 0; i < f->node_count; ++i)
+		if (f->nodes[i].kind == CRS_COLOR_IMAGE && (f->nodes[i].tex >= (int32_t)f->texture_count || f->nodes[i].tex < -1))
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "node %u texture index out of range", i);
+	/* K4's bucket order for the flat launch: the misses, the keys of flat materials (1..254, one material each), then the rest —
+	 * the generic keys and the overflow key 255, which materials 254 and up share */
+	auto is_flat = [&](uint32_t k) { return k < 255u && k - 1u < f->material_count && out.flat[k - 1u].kind != CRG_FLAT_NONE; };
+	out.order.clear();
+	out.order.push_back(0);
+	for (uint32_t k = 1; k < 256; ++k) if (is_flat(k)) out.order.push_back((uint8_t)k);
+	out.flat_keys = (uint32_t)out.order.size() - 1u;
+	for (uint32_t k = 1; k < 256; ++k) if (!is_flat(k)) out.order.push_back((uint8_t)k);
+	return CRGPU_OK;
+}
+
 /* ---- BVH re-layout: reference nodes (bvh.c:37-42) -> BFS-ordered PairNodes ---------------------------------------- */
 /* errors raised on worker threads (fail() writes a thread-local buffer): first one wins, reported by the caller */
 struct HostError {
@@ -581,6 +659,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->edit, s->edit_bytes);
 	ctx_free(s->device, s->edit_scratch, s->edit_scratch_bytes);
 	ctx_free(s->device, s->mesh_scratch, s->mesh_scratch_bytes);
+	ctx_free(s->device, s->shade, s->shade_bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -650,37 +729,20 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	crgpu_prepared *p = new crgpu_prepared();
 	p->slab = nullptr; p->pinned = false; p->slab_bytes = 0;
 	p->prefs = f->prefs; p->camera = f->camera; p->background = f->background; p->instance_count = f->instance_count;
-	p->xnodes = false;
-	for (uint32_t i = 0; i < f->node_count; ++i) {
-		const int k = f->nodes[i].kind;
-		if (k == CRS_COLOR_VECTOCOLOR || k == CRS_COLOR_COMBINE_VALUE || k == CRS_COLOR_COMBINE_RGB || k == CRS_VALUE_MATH || k == CRS_VALUE_FRESNEL ||
-			k == CRS_VALUE_RAYLENGTH || k == CRS_VECTOR_CONSTANT || k == CRS_VECTOR_NORMAL || k == CRS_VECTOR_VECMATH) p->xnodes = true;
-	}
-	p->bg = fold_background(f, f->background);
 	p->texture_count = f->texture_count;
 #define PFAIL(x) do { int rc_ = (x); if (rc_) return pfail(p, rc_); } while (0)
 
-	/* materials + graph validation */
-	std::vector<DevMaterial> mats(f->material_count);
-	std::vector<DevFlat> flat(f->material_count);
-	{
-		bool uv = false;
-		PFAIL(check_bsdf(f, f->background, 0, 0, &uv));
-	}
-	for (uint32_t i = 0; i < f->material_count; ++i) {
-		const crs_material &m = f->materials[i];
-		bool uv = false;
-		PFAIL(check_bsdf(f, m.bsdf, 0, 0, &uv));
-		DevMaterial d;
-		memset(&d, 0, sizeof d);
-		d.emission[0] = m.emission[0]; d.emission[1] = m.emission[1]; d.emission[2] = m.emission[2];
-		d.IOR = m.IOR; d.bsdf = m.bsdf;
-		/* x + w*0 == x bit-for-bit for finite w, so only non-zero (or non-finite) emission needs the add */
-		const bool emits = !(m.emission[0] == 0.0f && m.emission[1] == 0.0f && m.emission[2] == 0.0f);
-		d.flags = (uv ? 1u : 0u) | (emits ? 2u : 0u);
-		mats[i] = d;
-		flat[i] = fold_flat(f, m.bsdf);
-	}
+	/* materials, node graph, textures, background (their checks come before the geometry's: a scene malformed in both reports
+	 * its shading error) */
+	ShadingFold sh;
+	PFAIL(fold_shading(f, sh));
+	p->xnodes = sh.xnodes;
+	p->bg = sh.bg;
+	const std::vector<DevMaterial> &mats = sh.mats;
+	const std::vector<DevFlat> &flat = sh.flat;
+	const std::vector<DevTexture> &texs = sh.texs;
+	const std::vector<uint8_t> &order = sh.order;
+	p->flat_keys = sh.flat_keys;
 
 	/* BVHs → pair nodes; triangles in leaf order; per-poly shading records.  The three products are independent once the
 	 * slot offsets are known, and every element is computed from the flat scene alone, so they are filled by index on a
@@ -836,26 +898,6 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	p->bvh_prims.resize(f->bvh_count);
 	for (uint32_t b = 0; b < f->bvh_count; ++b) p->bvh_prims[b] = f->bvhs[b].prim_count;
 
-	/* textures (data pointers are byte offsets into the texture section here; patched per device at upload) */
-	std::vector<DevTexture> texs(f->texture_count);
-	for (uint32_t i = 0; i < f->texture_count; ++i) {
-		const crs_texture &t = f->textures[i];
-		const uint64_t bytes = (uint64_t)t.width * t.height * t.channels * (t.is_float ? 4u : 1u);
-		if (t.width == 0 || t.height == 0 || t.channels == 0 || t.channels > 4 || t.width > 65536u || t.height > 65536u ||
-			t.data_offset > f->texdata_bytes || bytes > f->texdata_bytes - t.data_offset) {
-			return pfail(p, fail(CRGPU_ERR_BAD_ARGUMENT, "texture %u malformed", i));
-		}
-		DevTexture d;
-		d.width = t.width; d.height = t.height; d.channels = t.channels; d.is_float = t.is_float; d.has_alpha = t.has_alpha; d.pad = 0;
-		d.wmask = (t.width & (t.width - 1u)) == 0u ? t.width - 1u : 0u;
-		d.hmask = (t.height & (t.height - 1u)) == 0u ? t.height - 1u : 0u;
-		d.data = reinterpret_cast<const uint8_t *>((uintptr_t)t.data_offset);
-		texs[i] = d;
-	}
-	for (uint32_t i = 0; i < f->node_count; ++i)
-		if (f->nodes[i].kind == CRS_COLOR_IMAGE && (f->nodes[i].tex >= (int32_t)f->texture_count || f->nodes[i].tex < -1))
-			return pfail(p, fail(CRGPU_ERR_BAD_ARGUMENT, "node %u texture index out of range", i));
-
 	std::vector<crs_node> nodes(f->nodes, f->nodes + f->node_count);
 
 	/* staging image: top-of-tree pair nodes (BFS prefix) of every BVH, the top level first, then the meshes
@@ -913,16 +955,6 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 			if (insts[i].kind == CRS_INST_SPHERE) keys[(size_t)total_slots + i] = key_of(insts[i].material);
 	}
 	p->key_inst_off = (size_t)total_slots;
-	/* K4's bucket order for the flat launch: the misses, the keys of flat materials (1..254, one material each), then the rest —
-	 * the generic keys and the overflow key 255, which materials 254 and up share */
-	std::vector<uint8_t> order;
-	{
-		auto is_flat = [&](uint32_t k) { return k < 255u && k - 1u < f->material_count && flat[k - 1u].kind != CRG_FLAT_NONE; };
-		order.push_back(0);
-		for (uint32_t k = 1; k < 256; ++k) if (is_flat(k)) order.push_back((uint8_t)k);
-		p->flat_keys = (uint32_t)order.size() - 1u;
-		for (uint32_t k = 1; k < 256; ++k) if (!is_flat(k)) order.push_back((uint8_t)k);
-	}
 	p->material_count = f->material_count;
 	std::vector<float> lut(256);
 	for (int i = 0; i < 256; ++i) { volatile float num = (float)i, den = 255.0f; lut[i] = num / den; }   /* IEEE divss == __fdiv_rn */
@@ -985,6 +1017,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	for (size_t b = 0; b < s->bvhs.size(); ++b) s->stage_cap[b] = s->bvhs[b].stage_count;
 	s->mesh_region.assign(p->meshes.size(), 0xffffffffu);
 	s->mesh_scratch = nullptr; s->mesh_scratch_bytes = 0;
+	s->material_count = p->material_count; s->shade = nullptr; s->shade_bytes = 0;
 	s->device = device; s->xnodes = p->xnodes; s->dev_copy = nullptr; s->fb = nullptr; s->fb8 = nullptr; s->stream = nullptr; s->own_stream = nullptr; s->cap_paths = 0;
 	s->slab = nullptr; s->slab_bytes = 0; s->small = nullptr; s->small_bytes = 0; s->wave = nullptr; s->wave_bytes = 0; s->fb_floats = 0;
 	memset(s->fetched, 0, sizeof s->fetched);
@@ -1780,6 +1813,72 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	s->dev.pairs = pairs;
 	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
 	CU(cudaStreamSynchronize(st));
+	return CRGPU_OK;
+}
+
+/* ---- shading edits ------------------------------------------------------------------------------------------------------------------
+ * The records whose size the material count fixes (materials, flat records, K4's key order) are rewritten in the slab; the node graph,
+ * texture table and texel data, whose sizes may change, go into a new shading block that replaces the previous one.  Every check and
+ * the fold run first and the block is filled before anything the kernels read changes. */
+extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat) {
+	if (!s || !flat) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (flat->material_count != s->material_count)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "%u materials given, the scene has %u", flat->material_count, s->material_count);
+	ShadingFold sh;
+	int rc = fold_shading(flat, sh);
+	if (rc) return rc;
+	rc = drain(s);
+	if (rc) return rc;
+	const size_t node_bytes = (size_t)flat->node_count * sizeof(crs_node), tex_bytes = sh.texs.size() * sizeof(DevTexture);
+	const size_t o_texs = align256(node_bytes), o_data = o_texs + align256(tex_bytes), bytes = o_data + align256((size_t)flat->texdata_bytes);
+	void *blk = nullptr;
+	rc = ctx_alloc(s->device, bytes, &blk);
+	if (rc) return rc;
+	uint8_t *base = static_cast<uint8_t *>(blk);
+	for (DevTexture &t : sh.texs) t.data = base + o_data + (uintptr_t)t.data;
+	cudaStream_t st = s->stream;
+	cudaError_t ce = cudaSuccess;
+	if (node_bytes) ce = cudaMemcpyAsync(base, flat->nodes, node_bytes, cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && tex_bytes) ce = cudaMemcpyAsync(base + o_texs, sh.texs.data(), tex_bytes, cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(base + o_data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (ce != cudaSuccess) { ctx_free(s->device, blk, bytes); return fail(CRGPU_ERR_CUDA, "set_shading: %s", cudaGetErrorString(ce)); }
+
+	/* commit */
+	const size_t nm = s->material_count;
+	if (nm) {
+		CU(cudaMemcpyAsync(const_cast<DevMaterial *>(s->dev.materials), sh.mats.data(), nm * sizeof(DevMaterial), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<DevFlat *>(s->dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
+	}
+	CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
+	s->dev.nodes = reinterpret_cast<const crs_node *>(base);
+	s->dev.textures = reinterpret_cast<const DevTexture *>(base + o_texs);
+	s->dev.bg = sh.bg;
+	s->dev.flat_keys = sh.flat_keys;
+	s->dev.background = flat->background;
+	s->xnodes = sh.xnodes;
+	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
+	CU(cudaStreamSynchronize(st));
+	ctx_free(s->device, s->shade, s->shade_bytes);
+	s->shade = blk; s->shade_bytes = bytes;
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,
+                                   uint32_t *background_kind, int *complete_interpreter) {
+	if (!s || (count && (!kinds || !flags))) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	const uint32_t n = count < s->material_count ? count : s->material_count;
+	if (n) {
+		int rc = drain(s);
+		if (rc) return rc;
+		std::vector<DevFlat> fl(n);
+		CU(cudaMemcpyAsync(fl.data(), s->dev.flat, (size_t)n * sizeof(DevFlat), cudaMemcpyDeviceToHost, s->stream));
+		CU(cudaStreamSynchronize(s->stream));
+		for (uint32_t i = 0; i < n; ++i) { kinds[i] = fl[i].kind; flags[i] = fl[i].flags; }
+	}
+	if (material_count) *material_count = s->material_count;
+	if (background_kind) *background_kind = s->dev.bg.kind;
+	if (complete_interpreter) *complete_interpreter = s->xnodes ? 1 : 0;
 	return CRGPU_OK;
 }
 

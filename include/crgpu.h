@@ -166,8 +166,8 @@ int crgpu_progress(crgpu_scene *s, int *passes_done, int *busy);
 int crgpu_request_snapshot(crgpu_scene *s);
 int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
 
-/* Editing a resident scene between renders (c-ray's crMoveCamera / crTransformMesh, src/c-ray.h:95-103): the edited scene renders
- * the same bits as the scene loaded fresh from the edited JSON.  Both calls first wait for the work queued on the scene's streams,
+/* Editing a resident scene between renders (c-ray's crMoveCamera / crTransformMesh / crSetHDR, src/c-ray.h:95-103): the edited scene
+ * renders the same bits as the scene loaded fresh from the edited JSON.  Every call first waits for the work queued on the scene's streams,
  * never touch the framebuffer (clear it before rendering the edited frame) and leave the scene unchanged when they fail.
  *   crgpu_scene_set_camera     copies every field of `cam` bit for bit; its width and height must be the scene's image size.
  *   crgpu_scene_set_instances  takes A and Ainv of each instance bit for bit (Ainv is not recomputed); `count`, and each instance's
@@ -192,11 +192,28 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *                              (crloader_build_bvh), deeper than 64 levels, or of more than 4,194,304 polys is refused with
  *                              CRGPU_ERR_UNSUPPORTED.  The first edit of a mesh gives it its own region of max(1, n - 1) pair nodes
  *                              behind the scene's other pairs; later edits reuse it.
+ *   crgpu_scene_set_shading    replaces the materials, the node graph, the textures, the texel data and the background root
+ *                              (crSetHDR, and recolouring, re-bsdf'ing or lighting surfaces) with those of `flat`, reading only its
+ *                              material_count, materials, node_count, nodes, texture_count, textures, texdata_bytes, texdata and
+ *                              background.  material_count must be the uploaded count (else CRGPU_ERR_BAD_ARGUMENT): material i of
+ *                              `flat` becomes material i of the scene, and which material each poly and sphere uses does not change
+ *                              (crgpu_scene_set_meshes changes a poly's).  Node count, texture count and texel bytes may grow or
+ *                              shrink.  The arrays are validated and folded as crgpu_prepare does it, and a refusal returns the code
+ *                              crgpu_prepare returns for them.  Materials, flat records and K4's key order are rewritten in place; the
+ *                              nodes, texture table and all texel data are uploaded on every call into a new block that replaces the
+ *                              previous edit's (the upload's node and texel sections stay allocated, unread).
+ *   crgpu_scene_shading        the live scene's counterpart of crgpu_prepared_materials and crgpu_prepared_background (same kinds and
+ *                              flags, read back from the device: min(count, material count) entries), and whether the shading kernels
+ *                              run the complete node interpreter.  kinds and flags may be NULL when count is 0, the other outputs
+ *                              always.
  * Edits apply to this device scene only: the crgpu_prepared it was created from, and any scene created from that later, are
  * unedited. */
 int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam);
 int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
 int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count);
+int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat);
+int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,
+                        uint32_t *background_kind, int *complete_interpreter);
 
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
