@@ -16,7 +16,6 @@
 #include <cstring>
 #include <cstdarg>
 #include <vector>
-#include <unordered_map>
 #include <queue>
 #include <thread>
 #include <mutex>
@@ -58,7 +57,7 @@ extern "C" int crgpu_device_count(int *n) {
  * back to a per-device cache and the next scene on that device takes it from there (best fit within 2x); a cudaMalloc that
  * fails trims the cache and retries.  crgpu_device_trim() hands everything back to the driver. */
 #define CRG_MAX_DEVICES 64
-struct DevBlock { void *p; size_t bytes; };
+struct DevBlock { void *p = nullptr; size_t bytes = 0; };
 struct DevCtx {
 	std::mutex lock;
 	std::vector<DevBlock> cache;
@@ -142,6 +141,16 @@ extern "C" void crgpu_host_free(void *p) { if (p) cudaFreeHost(p); }
  * pointer-carrying tables.  A host that renders many frames of one scene, or one frame on many GPUs, prepares once. */
 enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_ITEMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_FLAT, SEC_ORDER, SEC_NODES, SEC_TEXS, SEC_LUT,
        SEC_TEXDATA, SEC_COUNT };
+/* What the geometry edits (crgpu_scene_set_instances, crgpu_scene_set_meshes) need beyond the slab: the records they check an edit
+ * against, and the BVH root bounds they build the top level from. */
+struct EditRecord {
+	std::vector<uint32_t> inst_kind, inst_object;   /* kind and object of every instance: an edit must keep them */
+	std::vector<uint32_t> last;                      /* the last instance of each instance's object: all of them take its ray offset */
+	std::vector<float> bvh_root;                     /* root bounds of every BVH as stored, 6 floats each (the slab keeps only pair
+	                                                    nodes, whose roots' own boxes are not in it); an edited scene keeps them current */
+	std::vector<crs_mesh> meshes;                    /* every mesh record: an edit must keep each */
+	std::vector<uint32_t> bvh_prims;                 /* primitives of each BVH */
+};
 struct crgpu_prepared {
 	crs_prefs prefs;
 	crs_camera camera;
@@ -160,71 +169,67 @@ struct crgpu_prepared {
 	bool pinned;
 	size_t slab_bytes;
 	size_t off[SEC_COUNT], len[SEC_COUNT];
-	/* what crgpu_scene_set_instances needs beyond the slab: kind and object of every instance, and the root bounds of every BVH
-	 * as stored (6 floats each; the slab keeps only pair nodes, whose roots' own boxes are not in it) */
-	std::vector<uint32_t> inst_kind, inst_object;
-	std::vector<float> bvh_root;
-	/* what crgpu_scene_set_meshes checks an edit against: every mesh record and the primitive count of every BVH */
-	std::vector<crs_mesh> meshes;
-	std::vector<uint32_t> bvh_prims;
+	EditRecord rec;
 };
 
 struct crgpu_scene {
-	int device;
-	int sm_count;
-	bool xnodes;               /* crgpu_prepared::xnodes: selects the K3 / tail kernels with the complete node interpreter */
-	cudaStream_t stream;       /* the stream work is enqueued on (own_stream unless crgpu_set_stream) */
-	cudaStream_t own_stream;
-	unsigned long long fetched[8];   /* device counters at the previous stats fetch */
-	uint64_t pend_paths, pend_launches;
-	float pend_trace_ms, pend_shade_ms, pend_total_ms;
-	DevScene dev;
-	DevScene *dev_copy;        /* the same descriptor in HBM, for kernels that call noinline device functions */
-	void *slab; size_t slab_bytes;   /* the scene arrays + dev_copy */
-	void *small; size_t small_bytes; /* hist, counts, stats */
-	float *fb;                 /* W*H*3 fp32, row H-1-y */
-	uint8_t *fb8;              /* lazily allocated sRGB8 staging */
-	size_t fb_floats;
-	uint64_t max_paths;
-	uint64_t cap_paths;        /* capacity of the wavefront buffers */
-	void *wave; size_t wave_bytes;
-	int wave_sets;             /* 1, or 2 when batches are overlapped on two streams (each set holds cap_paths paths) */
-	WaveBuffers wb;            /* set 0 */
-	WaveBuffers wb2;           /* set 1: own ray / hit / radiance buffers and own hist + counts; stats shared */
-	cudaStream_t stream2;      /* the second stream of overlapped batches */
-	cudaEvent_t ev[4];
-	cudaEvent_t evAcc[2], evFork;   /* accumulate-order chain between the two streams */
-	uint32_t *pixels;          /* device pixel list of the last crgpu_render_tiles tile set */
-	size_t pixel_cap;
+	int device = 0;
+	int sm_count = 0;
+	bool xnodes = false;       /* crgpu_prepared::xnodes: selects the K3 / tail kernels with the complete node interpreter */
+	cudaStream_t stream = nullptr;   /* the stream work is enqueued on (own_stream unless crgpu_set_stream) */
+	cudaStream_t own_stream = nullptr;
+	unsigned long long fetched[8] = {};   /* device counters at the previous stats fetch */
+	uint64_t pend_paths = 0, pend_launches = 0;
+	float pend_trace_ms = 0.f, pend_shade_ms = 0.f, pend_total_ms = 0.f;
+	DevScene dev = {};
+	DevScene *dev_copy = nullptr;    /* the same descriptor in HBM, for kernels that call noinline device functions */
+	void *slab = nullptr; size_t slab_bytes = 0;     /* the scene arrays + dev_copy */
+	void *small = nullptr; size_t small_bytes = 0;   /* hist, counts, stats */
+	float *fb = nullptr;             /* W*H*3 fp32, row H-1-y */
+	uint8_t *fb8 = nullptr;          /* lazily allocated sRGB8 staging */
+	size_t fb_floats = 0;
+	uint64_t max_paths = 0;
+	uint64_t cap_paths = 0;          /* capacity of the wavefront buffers */
+	void *wave = nullptr; size_t wave_bytes = 0;
+	int wave_sets = 0;               /* 1, or 2 when batches are overlapped on two streams (each set holds cap_paths paths) */
+	WaveBuffers wb = {};             /* set 0 */
+	WaveBuffers wb2 = {};            /* set 1: own ray / hit / radiance buffers and own hist + counts; stats shared */
+	cudaStream_t stream2 = nullptr;  /* the second stream of overlapped batches */
+	cudaEvent_t ev[4] = {};
+	cudaEvent_t evAcc[2] = {}, evFork = nullptr;   /* accumulate-order chain between the two streams */
+	uint32_t *pixels = nullptr;      /* device pixel list of the last crgpu_render_tiles tile set */
+	size_t pixel_cap = 0;
 	std::vector<int> pixel_key;
-	bool armed;                /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
-	unsigned *stop_host;       /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight, [3] snapshot state
-	                              (0 idle, 1 requested, 2 staged), [4] its pass index (NULL until armed once) */
-	unsigned *stop_ctl;        /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets,
-	                              [3] the next publish step stages a snapshot, [4] its block count (crgpu_wave.cuh) */
-	uint8_t *snap8;            /* W*H*3 sRGB8 snapshot staged by a publish step (allocated by the first armed call) */
-	cudaStream_t snap_stream;  /* crgpu_take_snapshot's copies: never behind the render (created when first armed) */
-	/* instance edits (crgpu_scene_set_instances) */
-	std::vector<uint32_t> inst_kind, inst_object;    /* as uploaded: an edit must keep them */
-	std::vector<float> bvh_root;                     /* crgpu_prepared::bvh_root */
-	uint32_t pair_count;       /* pair nodes uploaded (the edit block starts with a copy of them) */
-	uint32_t top_stage_cap;    /* staged top-level pairs reserved at upload */
-	void *edit; size_t edit_bytes;             /* NULL until the first edit of instances or meshes: edit_pairs pair nodes (the
-	                                              uploaded pairs, the top region, the edited meshes' regions), then top_items */
-	uint32_t edit_pairs;
-	void *edit_scratch; size_t edit_scratch_bytes;   /* instance inputs, boxes, the new top level and the builder's scratch */
-	/* mesh edits (crgpu_scene_set_meshes) */
-	std::vector<crs_mesh> meshes;              /* as uploaded: an edit must keep each record */
-	std::vector<uint32_t> bvh_prims;           /* primitives of each BVH as uploaded */
-	std::vector<DevBvh> bvhs;                  /* the committed BVH records (the slab's copy is what the kernels read) */
-	std::vector<uint32_t> stage_cap;           /* staged pairs reserved for each BVH at upload */
-	std::vector<uint32_t> mesh_region;         /* first pair of a mesh's own region in the edit block (UINT32_MAX: none yet) */
-	void *mesh_scratch; size_t mesh_scratch_bytes;   /* a mesh edit's inputs, its rebuilt records and the builder's scratch */
-	/* shading edits (crgpu_scene_set_shading) */
-	uint32_t material_count;   /* as uploaded: an edit must keep it */
-	void *shade; size_t shade_bytes;           /* NULL until the first shading edit: the node graph, texture table and texel data the
-	                                              kernels read in place of the slab's */
+	bool armed = false;              /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
+	unsigned *stop_host = nullptr;   /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight, [3] snapshot
+	                                    state (0 idle, 1 requested, 2 staged), [4] its pass index (NULL until armed once) */
+	unsigned *stop_ctl = nullptr;    /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets,
+	                                    [3] the next publish step stages a snapshot, [4] its block count (crgpu_wave.cuh) */
+	uint8_t *snap8 = nullptr;        /* W*H*3 sRGB8 snapshot staged by a publish step (allocated by the first armed call) */
+	cudaStream_t snap_stream = nullptr;   /* crgpu_take_snapshot's copies: never behind the render (created when first armed) */
+	/* scene edits */
+	EditRecord rec;                  /* crgpu_prepared::rec */
+	std::vector<DevBvh> bvhs;        /* the committed BVH records (the slab's copy is what the kernels read) */
+	std::vector<uint32_t> stage_cap; /* staged pairs reserved for each BVH at upload */
+	std::vector<uint32_t> mesh_region;   /* first pair of a mesh's own region in the pairs block (UINT32_MAX: none yet) */
+	uint32_t pair_count = 0;         /* pair nodes uploaded */
+	uint32_t pair_cap = 0;           /* pair nodes dev.pairs holds: pair_count until the first geometry edit, then the pairs block's */
+	uint32_t top_stage_cap = 0;      /* staged top-level pairs reserved at upload */
+	uint32_t material_count = 0;     /* as uploaded: a shading edit must keep it */
+	DevBlock pairs;                  /* NULL until the first geometry edit: the uploaded pairs, the top region, the edited meshes' regions */
+	DevBlock insts;                  /* NULL until the first geometry edit: EditRecord::last, then the top level's item records */
+	DevBlock scratch;                /* a geometry edit's inputs, records and builder scratch; grows only, and nothing in it outlives a call */
+	DevBlock shade;                  /* NULL until the first shading edit: the node graph, texture table and texel data the kernels read in
+	                                    place of the slab's */
 };
+
+/* K1 and K2 take the host descriptor s->dev by value; K3, the tail kernel and the KAT read its HBM copy s->dev_copy.  Writes the
+ * copy and waits for it (and for everything queued before it on the scene's stream). */
+static int publish(crgpu_scene *s) {
+	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
 static bool node_ok(const crs_scene *f, int idx) { return idx >= 0 && (uint32_t)idx < f->node_count; }
@@ -610,6 +615,24 @@ static int build_pairs(const crs_scene *f, const crs_bvh &b, std::vector<PairNod
 
 static inline void f3(float *dst, const float *src, size_t idx) { dst[0] = src[3 * idx]; dst[1] = src[3 * idx + 1]; dst[2] = src[3 * idx + 2]; }
 
+/* The world box the kernels normalise hit points by: the top-level root's bounds b (minx,maxx,miny,maxy,minz,maxz). */
+static void world_box(const float b[6], float lo[3], float inv[3]) {
+	for (int k = 0; k < 3; ++k) {
+		const float e = b[2 * k + 1] - b[2 * k];
+		lo[k] = b[2 * k];
+		inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
+	}
+}
+
+static DevCamera dev_camera(const crs_camera &c) {
+	DevCamera d;
+	d.sensor_x = c.sensor_x; d.sensor_y = c.sensor_y; d.aperture = c.aperture; d.focal_distance = c.focal_distance;
+	memcpy(d.forward, c.forward, 12); memcpy(d.right, c.right, 12); memcpy(d.up, c.up, 12);
+	d.width = c.width; d.height = c.height;
+	memcpy(d.A, c.A, sizeof d.A);
+	return d;
+}
+
 /* all wavefront buffers of a scene are carved from ONE device block (one cudaMalloc / one cache hit per frame) */
 static int alloc_wave(crgpu_scene *s, uint64_t paths, int sets) {
 	if (paths <= s->cap_paths && sets <= s->wave_sets) return CRGPU_OK;
@@ -656,10 +679,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->fb8, s->fb_floats);
 	ctx_free(s->device, s->snap8, s->fb_floats);
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
-	ctx_free(s->device, s->edit, s->edit_bytes);
-	ctx_free(s->device, s->edit_scratch, s->edit_scratch_bytes);
-	ctx_free(s->device, s->mesh_scratch, s->mesh_scratch_bytes);
-	ctx_free(s->device, s->shade, s->shade_bytes);
+	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade }) ctx_free(s->device, b->p, b->bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -888,15 +908,20 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 		} else { return pfail(p, fail(CRGPU_ERR_UNSUPPORTED, "instance kind %u (volumes are not reachable from the scene loader)", src.kind)); }
 		insts[i] = d;
 	}
-	p->inst_kind.resize(f->instance_count);
-	p->inst_object.resize(f->instance_count);
-	for (uint32_t i = 0; i < f->instance_count; ++i) { p->inst_kind[i] = f->instances[i].kind; p->inst_object[i] = f->instances[i].object; }
-	p->bvh_root.assign(6 * (size_t)f->bvh_count, 0.0f);
-	for (uint32_t b = 0; b < f->bvh_count; ++b)
-		if (f->bvhs[b].node_count) memcpy(&p->bvh_root[6 * (size_t)b], f->bvh_nodes[f->bvhs[b].node_offset].bounds, 6 * sizeof(float));
-	p->meshes.assign(f->meshes, f->meshes + f->mesh_count);
-	p->bvh_prims.resize(f->bvh_count);
-	for (uint32_t b = 0; b < f->bvh_count; ++b) p->bvh_prims[b] = f->bvhs[b].prim_count;
+	EditRecord &rec = p->rec;
+	std::vector<uint32_t> last_of[2] = { std::vector<uint32_t>(f->mesh_count), std::vector<uint32_t>(f->sphere_count) };   /* by kind, object */
+	for (uint32_t i = 0; i < f->instance_count; ++i) {
+		rec.inst_kind.push_back(f->instances[i].kind);
+		rec.inst_object.push_back(f->instances[i].object);
+		last_of[f->instances[i].kind == CRS_INST_SPHERE][f->instances[i].object] = i;
+	}
+	for (uint32_t i = 0; i < f->instance_count; ++i) rec.last.push_back(last_of[rec.inst_kind[i] == CRS_INST_SPHERE][rec.inst_object[i]]);
+	rec.bvh_root.assign(6 * (size_t)f->bvh_count, 0.0f);
+	for (uint32_t b = 0; b < f->bvh_count; ++b) {
+		if (f->bvhs[b].node_count) memcpy(&rec.bvh_root[6 * (size_t)b], f->bvh_nodes[f->bvhs[b].node_offset].bounds, 6 * sizeof(float));
+		rec.bvh_prims.push_back(f->bvhs[b].prim_count);
+	}
+	rec.meshes.assign(f->meshes, f->meshes + f->mesh_count);
 
 	std::vector<crs_node> nodes(f->nodes, f->nodes + f->node_count);
 
@@ -931,18 +956,10 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	/* the instance step's record of every top-level leaf item (the staging above has set every stage_count) */
 	std::vector<DevTopItem> items(top_prims.size());
 	for (size_t i = 0; i < top_prims.size(); ++i) items[i] = crg_top_item(insts[top_prims[i]], bvhs.data(), (uint32_t)top_prims[i]);
-	{	/* world bounds = bounds of the top-level BVH root (both children of pair 0, or the single leaf's box) */
-		float lo[3] = { 0.f, 0.f, 0.f }, hi[3] = { 1.f, 1.f, 1.f };
+	{
+		static const float unit[6] = { 0.f, 1.f, 0.f, 1.f, 0.f, 1.f };
 		const crs_bvh &tb = f->bvhs[f->top_bvh];
-		if (tb.node_count >= 1) {
-			const float *b = f->bvh_nodes[tb.node_offset].bounds;          /* minx,maxx,miny,maxy,minz,maxz */
-			for (int k = 0; k < 3; ++k) { lo[k] = b[2 * k]; hi[k] = b[2 * k + 1]; }
-		}
-		for (int k = 0; k < 3; ++k) {
-			const float e = hi[k] - lo[k];
-			p->world_lo[k] = lo[k];
-			p->world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
-		}
+		world_box(tb.node_count ? f->bvh_nodes[tb.node_offset].bounds : unit, p->world_lo, p->world_inv);
 	}
 	/* shading keys (K4's buckets): min(material + 1, 255) per prim slot from its poly, then per instance for spheres */
 	std::vector<uint8_t> keys((size_t)total_slots + f->instance_count, 0u);
@@ -1001,29 +1018,15 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	CU(cudaSetDevice(device));
 
 	crgpu_scene *s = new crgpu_scene();
-	memset(&s->dev, 0, sizeof s->dev);
-	memset(&s->wb, 0, sizeof s->wb);
-	memset(&s->wb2, 0, sizeof s->wb2);
-	s->wave_sets = 0; s->stream2 = nullptr; s->evAcc[0] = s->evAcc[1] = nullptr; s->evFork = nullptr;
-	s->pixels = nullptr; s->pixel_cap = 0;
-	s->armed = false; s->stop_host = nullptr; s->stop_ctl = nullptr; s->snap8 = nullptr; s->snap_stream = nullptr;
-	s->inst_kind = p->inst_kind; s->inst_object = p->inst_object; s->bvh_root = p->bvh_root;
-	s->pair_count = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode)); s->top_stage_cap = p->top.stage_count;
-	s->edit = nullptr; s->edit_bytes = 0; s->edit_pairs = 0; s->edit_scratch = nullptr; s->edit_scratch_bytes = 0;
-	s->meshes = p->meshes; s->bvh_prims = p->bvh_prims;
-	s->bvhs.resize(p->len[SEC_BVHS] / sizeof(DevBvh));
-	memcpy(s->bvhs.data(), p->slab + p->off[SEC_BVHS], p->len[SEC_BVHS]);
-	s->stage_cap.resize(s->bvhs.size());
-	for (size_t b = 0; b < s->bvhs.size(); ++b) s->stage_cap[b] = s->bvhs[b].stage_count;
-	s->mesh_region.assign(p->meshes.size(), 0xffffffffu);
-	s->mesh_scratch = nullptr; s->mesh_scratch_bytes = 0;
-	s->material_count = p->material_count; s->shade = nullptr; s->shade_bytes = 0;
-	s->device = device; s->xnodes = p->xnodes; s->dev_copy = nullptr; s->fb = nullptr; s->fb8 = nullptr; s->stream = nullptr; s->own_stream = nullptr; s->cap_paths = 0;
-	s->slab = nullptr; s->slab_bytes = 0; s->small = nullptr; s->small_bytes = 0; s->wave = nullptr; s->wave_bytes = 0; s->fb_floats = 0;
-	memset(s->fetched, 0, sizeof s->fetched);
-	s->pend_paths = s->pend_launches = 0; s->pend_trace_ms = s->pend_shade_ms = s->pend_total_ms = 0.f;
-	s->max_paths = 0;   /* set below from the free device memory */
-	for (auto &e : s->ev) e = nullptr;
+	s->device = device; s->xnodes = p->xnodes;
+	s->rec = p->rec;
+	const DevBvh *bvhs = reinterpret_cast<const DevBvh *>(p->slab + p->off[SEC_BVHS]);
+	s->bvhs.assign(bvhs, bvhs + p->len[SEC_BVHS] / sizeof(DevBvh));
+	for (const DevBvh &b : s->bvhs) s->stage_cap.push_back(b.stage_count);
+	s->mesh_region.assign(p->rec.meshes.size(), 0xffffffffu);
+	s->pair_count = s->pair_cap = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode));
+	s->top_stage_cap = p->top.stage_count;
+	s->material_count = p->material_count;
 #define FAIL_IF(x) do { int rc_ = (x); if (rc_) { crgpu_scene_destroy(s); return rc_; } } while (0)
 #define CUS(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { int rc_ = fail(CRGPU_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); crgpu_scene_destroy(s); return rc_; } } while (0)
 	CUS(cudaDeviceGetAttribute(&s->sm_count, cudaDevAttrMultiProcessorCount, device));
@@ -1047,11 +1050,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 		CUS(cudaStreamSynchronize(s->stream));   /* texs is a local pageable buffer */
 	}
 	DevScene &d = s->dev;
-	d.cam.sensor_x = p->camera.sensor_x; d.cam.sensor_y = p->camera.sensor_y;
-	d.cam.aperture = p->camera.aperture; d.cam.focal_distance = p->camera.focal_distance;
-	memcpy(d.cam.forward, p->camera.forward, 12); memcpy(d.cam.right, p->camera.right, 12); memcpy(d.cam.up, p->camera.up, 12);
-	d.cam.width = p->camera.width; d.cam.height = p->camera.height;
-	memcpy(d.cam.A, p->camera.A, sizeof d.cam.A);
+	d.cam = dev_camera(p->camera);
 	d.image_width = p->prefs.image_width; d.image_height = p->prefs.image_height;
 	d.sample_count = p->prefs.sample_count; d.bounces = p->prefs.bounces;
 	d.background = p->background;
@@ -1079,7 +1078,6 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	d.u8_to_unit = reinterpret_cast<const float *>(base + p->off[SEC_LUT]);
 	static_assert(sizeof(DevScene) <= 512, "DevScene must fit the descriptor slot behind the scene arrays");
 	s->dev_copy = reinterpret_cast<DevScene *>(base + p->slab_bytes - 512);
-	CUS(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, s->stream));
 
 	s->fb_floats = (size_t)d.image_width * d.image_height * 3u;
 	{ void *q = nullptr; FAIL_IF(ctx_alloc(device, s->fb_floats * sizeof(float), &q)); s->fb = static_cast<float *>(q); }
@@ -1111,7 +1109,7 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 		if (fit < (1ull << 20)) fit = 1ull << 20;
 		s->max_paths = fit;
 	}
-	CUS(cudaStreamSynchronize(s->stream));
+	FAIL_IF(publish(s));
 #undef FAIL_IF
 #undef CUS
 	*out = s;
@@ -1457,130 +1455,145 @@ extern "C" int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *pass
 	return CRGPU_OK;
 }
 
-/* ---- scene edits between renders ----------------------------------------------------------------------------------------------------
- * K1 and K2 take the host descriptor s->dev by value; K3, the tail kernel and the KAT read its HBM copy s->dev_copy: both change. */
+/* ---- scene edits between renders -------------------------------------------------------------------------------------------------- */
 extern "C" int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam) {
 	if (!s || !cam) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (cam->width != (int32_t)s->dev.image_width || cam->height != (int32_t)s->dev.image_height)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "camera is %dx%d, the scene renders %ux%u", cam->width, cam->height, s->dev.image_width, s->dev.image_height);
 	int rc = drain(s);
 	if (rc) return rc;
-	DevCamera &c = s->dev.cam;
-	c.sensor_x = cam->sensor_x; c.sensor_y = cam->sensor_y; c.aperture = cam->aperture; c.focal_distance = cam->focal_distance;
-	memcpy(c.forward, cam->forward, 12); memcpy(c.right, cam->right, 12); memcpy(c.up, cam->up, 12);
-	c.width = cam->width; c.height = cam->height;
-	memcpy(c.A, cam->A, sizeof c.A);
-	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, s->stream));
-	CU(cudaStreamSynchronize(s->stream));
-	return CRGPU_OK;
+	s->dev.cam = dev_camera(*cam);
+	return publish(s);
 }
 
 static size_t align256(size_t b) { return (b + 255u) & ~(size_t)255u; }
 
-/* The instance scratch of an edit that rebuilds the top level: the caller's instances, last instance of each object, BVH roots,
- * boxes, centres, offsets, new instance records, new top pairs and prims, then the builder's own scratch. */
-enum { ES_INST, ES_LAST, ES_ROOTS, ES_BB, ES_CTR, ES_OFFS, ES_NEW_INSTS, ES_PAIRS, ES_PRIMS, ES_BUILD, ES_COUNT };
-struct EditLayout { size_t sz[ES_COUNT], so[ES_COUNT], total; };
-static EditLayout edit_layout(const crgpu_scene *s) {
-	const uint32_t n = (uint32_t)s->inst_kind.size();
-	const size_t top_cap = n > 1u ? n - 1u : 1u;
-	EditLayout L;
-	const size_t sz[ES_COUNT] = { (size_t)n * sizeof(crs_instance), (size_t)n * 4u, s->bvh_root.size() * sizeof(float), (size_t)n * 24u, (size_t)n * 12u,
-	                              (size_t)n * 4u, (size_t)n * sizeof(DevInstance), top_cap * sizeof(PairNode), (size_t)n * 4u, crg_bvh_scratch_bytes(n) };
-	L.total = 0;
-	for (int k = 0; k < ES_COUNT; ++k) { L.sz[k] = sz[k]; L.so[k] = L.total; L.total += align256(sz[k]); }
-	return L;
-}
-static DevTopItem *edit_items(const crgpu_scene *s) {
-	return reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->edit) + align256((size_t)s->edit_pairs * sizeof(PairNode)));
-}
+/* Pair nodes a BVH of n primitives may need: the room of a top region or of a mesh region. */
+static uint32_t region_pairs(uint32_t n) { return n > 1u ? n - 1u : 1u; }
 
-/* The first edit of instances or meshes gives the scene its own pairs block: the uploaded pairs (unedited meshes' pair offsets do not
- * move), then a top region that holds any top level of n instances, then its n item records; the uploaded top level keeps rendering
- * until an edit is committed.  It also allocates the instance scratch. */
-static int ensure_edit(crgpu_scene *s) {
-	if (s->edit) return CRGPU_OK;
-	const uint32_t n = (uint32_t)s->inst_kind.size();
-	const uint32_t top_cap = n > 1u ? n - 1u : 1u;
-	const EditLayout L = edit_layout(s);
-	const size_t edit_bytes = align256((size_t)(s->pair_count + top_cap) * sizeof(PairNode)) + (size_t)n * sizeof(DevTopItem);
-	cudaStream_t st = s->stream;
-	void *e = nullptr, *q = nullptr;
-	int rc = ctx_alloc(s->device, edit_bytes, &e);
-	if (!rc) rc = ctx_alloc(s->device, L.total, &q);
-	std::vector<uint32_t> last(n);
-	std::unordered_map<uint64_t, uint32_t> last_of;                  /* (kind, object) -> its last instance */
-	for (uint32_t i = n; i-- > 0;) {
-		const uint64_t key = ((uint64_t)s->inst_kind[i] << 32) | s->inst_object[i];
-		last[i] = last_of.emplace(key, i).first->second;
+/* Parts of one device block, 256-byte aligned, in the order they are taken.  A layout runs twice: over base 0 to size the block,
+ * then over the block. */
+struct Carve {
+	uintptr_t base;
+	size_t bytes;
+	template <class T> T *take(size_t count) { T *q = reinterpret_cast<T *>(base + bytes); bytes += align256(count * sizeof(T)); return q; }
+};
+/* Lays layout's parts out over blk.  When they need more than blk holds, blk first goes back to the per-device cache (nothing in it
+ * may be read any more) and a large enough block takes its place. */
+template <class F> static int carve(int device, DevBlock &blk, F layout) {
+	Carve c = { 0, 0 };
+	layout(c);
+	if (c.bytes > blk.bytes) {
+		ctx_free(device, blk.p, blk.bytes);
+		blk = DevBlock();
+		int rc = ctx_alloc(device, c.bytes, &blk.p);
+		if (rc) return rc;
+		blk.bytes = c.bytes;
 	}
-	cudaError_t ce = cudaSuccess;
-	if (!rc) ce = cudaMemcpyAsync(e, s->dev.pairs, (size_t)s->pair_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st);
-	if (!rc && ce == cudaSuccess && n) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + L.so[ES_LAST], last.data(), L.sz[ES_LAST], cudaMemcpyHostToDevice, st);
-	if (!rc && ce == cudaSuccess) ce = cudaMemcpyAsync(static_cast<uint8_t *>(q) + L.so[ES_ROOTS], s->bvh_root.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st);
-	if (!rc && ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (!rc && ce != cudaSuccess) rc = fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
-	if (rc) { ctx_free(s->device, e, edit_bytes); ctx_free(s->device, q, L.total); return rc; }
-	s->edit = e; s->edit_bytes = edit_bytes; s->edit_pairs = s->pair_count + top_cap;
-	s->edit_scratch = q; s->edit_scratch_bytes = L.total;
+	c = { reinterpret_cast<uintptr_t>(blk.p), 0 };
+	layout(c);
 	return CRGPU_OK;
 }
 
-/* Instance boxes, ray offsets and the top-level BVH into the instance scratch: A and Ainv from inst (device, in the scratch), or the
- * scene's current instance records when inst is NULL; mesh boxes from the BVH roots in the scratch. */
-static int build_top(crgpu_scene *s, const crs_instance *inst, CrgBuildResult *res) {
-	const uint32_t n = (uint32_t)s->inst_kind.size();
-	const EditLayout L = edit_layout(s);
-	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
+/* The top-level build's part of an edit call's scratch: the BVH roots it reads, the instance boxes, centres and ray offsets, the new
+ * instance records, and the new top level's pairs and primitive order. */
+struct TopParts {
+	float *roots, *bb, *ctr, *offs;
+	DevInstance *insts;
+	PairNode *pairs;
+	int32_t *prims;
+};
+static TopParts take_top(Carve &c, const crgpu_scene *s) {
+	const size_t n = s->rec.inst_kind.size();
+	TopParts t;
+	t.roots = c.take<float>(s->rec.bvh_root.size());
+	t.bb = c.take<float>(6 * n); t.ctr = c.take<float>(3 * n); t.offs = c.take<float>(n);
+	t.insts = c.take<DevInstance>(n);
+	t.pairs = c.take<PairNode>(region_pairs((uint32_t)n));
+	t.prims = c.take<int32_t>(n);
+	return t;
+}
+
+/* The DevBvh record of a device build whose pairs sit at pair_offset; it stages at most stage_cap of them at stage_base. */
+static DevBvh bvh_record(const CrgBuildResult &res, uint32_t pair_offset, uint32_t slot_offset, uint32_t stage_base, uint32_t stage_cap) {
+	DevBvh b;
+	memset(&b, 0, sizeof b);
+	b.pair_offset = pair_offset;
+	b.pair_end = pair_offset + res.pairs;
+	b.node_count = res.node_count;
+	b.slot_offset = slot_offset;
+	if (res.node_count == 1u) { memcpy(b.root_bounds, res.bounds, sizeof b.root_bounds); b.root_first = res.root_first; b.root_count = res.root_count; }
+	b.stage_base = stage_base;
+	b.stage_count = res.pairs < stage_cap ? res.pairs : stage_cap;
+	return b;
+}
+
+/* Gives the scene a pairs block of `count` pair nodes that starts with a copy of the live ones (the uploaded pairs until the first
+ * geometry edit; unedited meshes' pair offsets do not move) and swaps it in.  The block it replaces goes back to the per-device cache
+ * after the publish that stops the descriptor from pointing at it. */
+static int reserve_pairs(crgpu_scene *s, uint32_t count) {
+	DevBlock blk;
+	int rc = ctx_alloc(s->device, (size_t)count * sizeof(PairNode), &blk.p);
+	if (rc) return rc;
+	blk.bytes = (size_t)count * sizeof(PairNode);
+	cudaError_t ce = cudaMemcpyAsync(blk.p, s->dev.pairs, (size_t)s->pair_cap * sizeof(PairNode), cudaMemcpyDeviceToDevice, s->stream);
+	if (ce != cudaSuccess) { ctx_free(s->device, blk.p, blk.bytes); return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce)); }
+	const DevBlock old = s->pairs;
+	s->pairs = blk;
+	s->pair_cap = count;
+	s->dev.pairs = static_cast<const PairNode *>(blk.p);
+	rc = publish(s);
+	if (!rc) ctx_free(s->device, old.p, old.bytes);
+	return rc;
+}
+
+/* The first geometry edit of a scene with instances gives it its instance block: EditRecord::last, which never changes, then room
+ * for the top level's item records. */
+static int alloc_insts(crgpu_scene *s) {
+	if (s->insts.p) return CRGPU_OK;
+	const size_t n = s->rec.last.size();
+	const size_t bytes = align256(n * 4u) + n * sizeof(DevTopItem);
+	int rc = ctx_alloc(s->device, bytes, &s->insts.p);
+	if (rc) return rc;
+	s->insts.bytes = bytes;
+	cudaError_t ce = cudaMemcpyAsync(s->insts.p, s->rec.last.data(), n * 4u, cudaMemcpyHostToDevice, s->stream);
+	if (ce == cudaSuccess) return CRGPU_OK;
+	ctx_free(s->device, s->insts.p, s->insts.bytes);
+	s->insts = DevBlock();
+	return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
+}
+
+/* Instance boxes, ray offsets and the top-level BVH into the scratch parts t: A and Ainv from inst (device), or the scene's current
+ * instance records when inst is NULL; mesh boxes from t.roots. */
+static int build_top(crgpu_scene *s, const crs_instance *inst, const TopParts &t, void *build, CrgBuildResult *res) {
+	const uint32_t n = (uint32_t)s->rec.inst_kind.size();
 	cudaStream_t st = s->stream;
-	DevInstance *new_insts = reinterpret_cast<DevInstance *>(sc + L.so[ES_NEW_INSTS]);
-	CU(cudaMemcpyAsync(new_insts, s->dev.instances, L.sz[ES_NEW_INSTS], cudaMemcpyDeviceToDevice, st));
-	crg_launch_instance_boxes(inst, new_insts, reinterpret_cast<const float *>(sc + L.so[ES_ROOTS]), reinterpret_cast<const uint32_t *>(sc + L.so[ES_LAST]), n,
-	                          reinterpret_cast<float *>(sc + L.so[ES_BB]), reinterpret_cast<float *>(sc + L.so[ES_CTR]), reinterpret_cast<float *>(sc + L.so[ES_OFFS]), st);
+	CU(cudaMemcpyAsync(t.insts, s->dev.instances, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
+	crg_launch_instance_boxes(inst, t.insts, t.roots, static_cast<const uint32_t *>(s->insts.p), n, t.bb, t.ctr, t.offs, st);
 	CU(cudaGetLastError());
-	int rc = crg_bvh_build_pairs(reinterpret_cast<const float *>(sc + L.so[ES_BB]), reinterpret_cast<const float *>(sc + L.so[ES_CTR]), n, sc + L.so[ES_BUILD], st,
-	                             reinterpret_cast<PairNode *>(sc + L.so[ES_PAIRS]), reinterpret_cast<int32_t *>(sc + L.so[ES_PRIMS]), res);
+	int rc = crg_bvh_build_pairs(t.bb, t.ctr, n, build, st, t.pairs, t.prims, res);
 	if (rc) return rc;
 	if (res->levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "BVH deeper than 64 levels");
 	return CRGPU_OK;
 }
 
-/* Copies a built top level over the scene's instances, top region, item records and staged prefix, and the new descriptor to HBM.
+/* Copies a built top level over the scene's instances, top region, item records and staged prefix, and publishes the descriptor.
  * The BVH records the items read must already be committed. */
-static int commit_top(crgpu_scene *s, const CrgBuildResult &res) {
-	const uint32_t n = (uint32_t)s->inst_kind.size();
-	const EditLayout L = edit_layout(s);
-	uint8_t *sc = static_cast<uint8_t *>(s->edit_scratch);
+static int commit_top(crgpu_scene *s, const TopParts &t, const CrgBuildResult &res) {
+	const uint32_t n = (uint32_t)s->rec.inst_kind.size();
 	cudaStream_t st = s->stream;
-	const DevInstance *new_insts = reinterpret_cast<const DevInstance *>(sc + L.so[ES_NEW_INSTS]);
-	const PairNode *new_pairs = reinterpret_cast<const PairNode *>(sc + L.so[ES_PAIRS]);
-	DevBvh t;
-	memset(&t, 0, sizeof t);
-	t.pair_offset = s->pair_count;
-	t.pair_end = s->pair_count + res.pairs;
-	t.node_count = res.node_count;
-	if (res.node_count == 1u) { memcpy(t.root_bounds, res.bounds, sizeof t.root_bounds); t.root_first = res.root_first; t.root_count = res.root_count; }
-	t.stage_base = s->dev.top.stage_base;
-	t.stage_count = res.pairs < s->top_stage_cap ? res.pairs : s->top_stage_cap;
-	PairNode *top_pairs = static_cast<PairNode *>(s->edit) + s->pair_count;          /* = pairs + t.pair_offset */
-	DevTopItem *top_items = edit_items(s);
-	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), new_insts, L.sz[ES_NEW_INSTS], cudaMemcpyDeviceToDevice, st));
-	if (res.pairs) CU(cudaMemcpyAsync(top_pairs, new_pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	crg_launch_top_items(reinterpret_cast<const int32_t *>(sc + L.so[ES_PRIMS]), new_insts, s->dev.bvhs, n, top_items, st);
+	const DevBvh top = bvh_record(res, s->pair_count, 0u, s->dev.top.stage_base, s->top_stage_cap);
+	DevTopItem *items = reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->insts.p) + align256((size_t)n * 4u));
+	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), t.insts, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
+	if (res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + top.pair_offset, t.pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	crg_launch_top_items(t.prims, t.insts, s->dev.bvhs, n, items, st);
 	CU(cudaGetLastError());
-	if (t.stage_count)
-		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + t.stage_base, new_pairs, (size_t)t.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	s->dev.top = t;
-	s->dev.pairs = reinterpret_cast<const PairNode *>(s->edit);
-	s->dev.top_items = top_items;
-	for (int k = 0; k < 3; ++k) {            /* as crgpu_prepare: the root's bounds */
-		const float lo = res.bounds[2 * k], e = res.bounds[2 * k + 1] - lo;
-		s->dev.world_lo[k] = lo;
-		s->dev.world_inv[k] = (e > 0.f && e < 3.0e38f) ? 1.0f / e : 0.f;
-	}
-	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
-	CU(cudaStreamSynchronize(st));
-	return CRGPU_OK;
+	if (top.stage_count)
+		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + top.stage_base, t.pairs, (size_t)top.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	s->dev.top = top;
+	s->dev.top_items = items;
+	world_box(res.bounds, s->dev.world_lo, s->dev.world_inv);
+	return publish(s);
 }
 
 /* Instance boxes, ray offsets and the top-level BVH of the edited instances are computed on the device, into scratch; only once the
@@ -1588,32 +1601,44 @@ static int commit_top(crgpu_scene *s, const CrgBuildResult &res) {
  * item records rebuilt from them. */
 extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
 	if (!s || !inst) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	const uint32_t n = (uint32_t)s->inst_kind.size();
+	const uint32_t n = (uint32_t)s->rec.inst_kind.size();
 	if (count != n) return fail(CRGPU_ERR_BAD_ARGUMENT, "%u instances given, the scene has %u", count, n);
 	for (uint32_t i = 0; i < n; ++i)
-		if (inst[i].kind != s->inst_kind[i] || inst[i].object != s->inst_object[i])
+		if (inst[i].kind != s->rec.inst_kind[i] || inst[i].object != s->rec.inst_object[i])
 			return fail(CRGPU_ERR_BAD_ARGUMENT, "instance %u changes its kind or object", i);
 	int rc = drain(s);
 	if (rc) return rc;
 	if (n == 0) return CRGPU_OK;
-	rc = ensure_edit(s);
+	crs_instance *dinst = nullptr;
+	TopParts t;
+	void *build = nullptr;
+	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
+	if (!rc) rc = alloc_insts(s);
 	if (rc) return rc;
-	const EditLayout L = edit_layout(s);
-	crs_instance *dinst = reinterpret_cast<crs_instance *>(static_cast<uint8_t *>(s->edit_scratch) + L.so[ES_INST]);
-	CU(cudaMemcpyAsync(dinst, inst, L.sz[ES_INST], cudaMemcpyHostToDevice, s->stream));
+	/* the roots in a copy of their own: packing them behind the caller's instances would cost a host copy of every instance */
+	CU(cudaMemcpyAsync(dinst, inst, (size_t)n * sizeof(crs_instance), cudaMemcpyHostToDevice, s->stream));
+	CU(cudaMemcpyAsync(t.roots, s->rec.bvh_root.data(), s->rec.bvh_root.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
 	CrgBuildResult res;
-	rc = build_top(s, dinst, &res);
+	rc = build_top(s, dinst, t, build, &res);
+	if (!rc && !s->pairs.p) rc = reserve_pairs(s, s->pair_count + region_pairs(n));
 	if (rc) return rc;
-	return commit_top(s, res);
+	return commit_top(s, t, res);
 }
 
 /* ---- mesh edits ---------------------------------------------------------------------------------------------------------------------
  * What one listed mesh reads from the caller's flat scene: its polys and the index ranges of vertices, normals and texcoords they use
- * (checked as crgpu_prepare checks them), and where its inputs and rebuilt records sit in the mesh scratch. */
+ * (checked as crgpu_prepare checks them), and its parts of the scratch: inputs and rebuilt records. */
 struct MeshEdit {
 	uint32_t mesh, bvh, n;
 	uint32_t vlo, vhi, nlo, nhi, tlo, thi;          /* [lo, hi) index ranges; hi == lo: none */
-	size_t o_polys, o_verts, o_norms, o_uvs, o_bb, o_ctr, o_pairs, o_prims, o_tris, o_slot, o_keys, o_spolys;
+	crs_poly *polys;
+	float *verts, *norms, *uvs, *bb, *ctr;
+	PairNode *pairs;
+	int32_t *prims;
+	PackedTri *tris;
+	uint32_t *slot;
+	uint8_t *keys;
+	ShadePoly *spolys;
 	CrgBuildResult res;
 };
 
@@ -1653,33 +1678,11 @@ static int check_mesh_polys(const crs_scene *f, const crs_mesh &mesh, MeshEdit &
 	return CRGPU_OK;
 }
 
-/* Gives the edit block room for `add` more pair nodes behind its current ones (the queued work has been drained). */
-static int grow_edit(crgpu_scene *s, uint32_t add) {
-	const uint32_t n = (uint32_t)s->inst_kind.size();
-	const uint32_t pairs = s->edit_pairs + add;
-	const size_t bytes = align256((size_t)pairs * sizeof(PairNode)) + (size_t)n * sizeof(DevTopItem);
-	void *e = nullptr;
-	int rc = ctx_alloc(s->device, bytes, &e);
-	if (rc) return rc;
-	cudaStream_t st = s->stream;
-	const DevTopItem *old_items = edit_items(s);
-	cudaError_t ce = cudaMemcpyAsync(e, s->edit, (size_t)s->edit_pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st);
-	if (ce == cudaSuccess && n)
-		ce = cudaMemcpyAsync(static_cast<uint8_t *>(e) + align256((size_t)pairs * sizeof(PairNode)), old_items, (size_t)n * sizeof(DevTopItem), cudaMemcpyDeviceToDevice, st);
-	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) { ctx_free(s->device, e, bytes); return fail(CRGPU_ERR_CUDA, "set_meshes: %s", cudaGetErrorString(ce)); }
-	ctx_free(s->device, s->edit, s->edit_bytes);
-	const bool live = s->dev.pairs == s->edit;
-	s->edit = e; s->edit_bytes = bytes; s->edit_pairs = pairs;
-	if (live) { s->dev.pairs = static_cast<const PairNode *>(e); s->dev.top_items = edit_items(s); }
-	return CRGPU_OK;
-}
-
 /* Each listed mesh's triangle boxes, BVH, triangles, slot records and shading records, then the instances and the top level, are
  * rebuilt on the device into scratch; only once every build has passed the upload's checks are they copied over the scene. */
 extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count) {
 	if (!s || !flat || (count && !meshes)) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	const uint32_t nm = (uint32_t)s->meshes.size();
+	const uint32_t nm = (uint32_t)s->rec.meshes.size();
 	std::vector<uint8_t> listed(nm, 0u);
 	std::vector<MeshEdit> edits;
 	for (uint32_t k = 0; k < count; ++k) {
@@ -1687,11 +1690,11 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 		if (m >= nm || m >= flat->mesh_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u out of range (the scene has %u)", m, nm);
 		if (listed[m]) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u listed twice", m);
 		listed[m] = 1u;
-		const crs_mesh &a = s->meshes[m], &b = flat->meshes[m];
+		const crs_mesh &a = s->rec.meshes[m], &b = flat->meshes[m];
 		if (a.poly_offset != b.poly_offset || a.poly_count != b.poly_count || a.material_offset != b.material_offset || a.material_count != b.material_count ||
 		    a.texcoord_count != b.texcoord_count || a.bvh != b.bvh)
 			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its record differs from the uploaded one (the topology cannot change)", m);
-		if (a.bvh >= s->bvh_prims.size() || s->bvh_prims[a.bvh] != a.poly_count)
+		if (a.bvh >= s->rec.bvh_prims.size() || s->rec.bvh_prims[a.bvh] != a.poly_count)
 			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its uploaded BVH does not cover exactly its polys", m);
 		if ((uint64_t)b.poly_offset + b.poly_count > flat->poly_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u ranges out of bounds", m);
 		if (a.poly_count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: %u polys (the device builder's limit is 4194304)", m, a.poly_count);
@@ -1705,115 +1708,84 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	int rc = drain(s);
 	if (rc) return rc;
 	if (edits.empty()) return CRGPU_OK;
-	rc = ensure_edit(s);
-	if (rc) return rc;
 
-	/* the mesh scratch: every listed mesh's inputs and records, then the builder's scratch for the largest */
-	size_t total = 0;
-	uint32_t nmax = 0;
-	auto take = [&](size_t bytes) { const size_t o = total; total += align256(bytes); return o; };
-	for (MeshEdit &e : edits) {
-		e.o_polys = take((size_t)e.n * sizeof(crs_poly));
-		e.o_verts = take((size_t)(e.vhi - e.vlo) * 12u); e.o_norms = take((size_t)(e.nhi - e.nlo) * 12u); e.o_uvs = take((size_t)(e.thi - e.tlo) * 8u);
-		e.o_bb = take((size_t)e.n * 24u); e.o_ctr = take((size_t)e.n * 12u);
-		e.o_pairs = take((size_t)(e.n > 1u ? e.n - 1u : 1u) * sizeof(PairNode)); e.o_prims = take((size_t)e.n * 4u);
-		e.o_tris = take((size_t)e.n * sizeof(PackedTri)); e.o_slot = take((size_t)e.n * 4u); e.o_keys = take(e.n);
-		e.o_spolys = take((size_t)e.n * sizeof(ShadePoly));
-		if (e.n > nmax) nmax = e.n;
-	}
-	const size_t o_build = take(crg_bvh_scratch_bytes(nmax));
-	if (total > s->mesh_scratch_bytes) {
-		void *q = nullptr;
-		rc = ctx_alloc(s->device, total, &q);
-		if (rc) return rc;
-		ctx_free(s->device, s->mesh_scratch, s->mesh_scratch_bytes);
-		s->mesh_scratch = q; s->mesh_scratch_bytes = total;
-	}
-	uint8_t *sc = static_cast<uint8_t *>(s->mesh_scratch);
+	/* the scratch: every listed mesh's inputs and records, the top level's parts, then the builder's scratch for the largest build */
+	const uint32_t ninst = (uint32_t)s->rec.inst_kind.size();
+	uint32_t nmax = ninst;
+	for (const MeshEdit &e : edits) nmax = e.n > nmax ? e.n : nmax;
+	TopParts t;
+	void *build = nullptr;
+	rc = carve(s->device, s->scratch, [&](Carve &c) {
+		for (MeshEdit &e : edits) {
+			e.polys = c.take<crs_poly>(e.n);
+			e.verts = c.take<float>(3 * (size_t)(e.vhi - e.vlo)); e.norms = c.take<float>(3 * (size_t)(e.nhi - e.nlo)); e.uvs = c.take<float>(2 * (size_t)(e.thi - e.tlo));
+			e.bb = c.take<float>(6 * (size_t)e.n); e.ctr = c.take<float>(3 * (size_t)e.n);
+			e.pairs = c.take<PairNode>(region_pairs(e.n)); e.prims = c.take<int32_t>(e.n);
+			e.tris = c.take<PackedTri>(e.n); e.slot = c.take<uint32_t>(e.n); e.keys = c.take<uint8_t>(e.n); e.spolys = c.take<ShadePoly>(e.n);
+		}
+		t = take_top(c, s);
+		build = c.take<uint8_t>(crg_bvh_scratch_bytes(nmax));
+	});
+	if (rc) return rc;
 	cudaStream_t st = s->stream;
 	for (MeshEdit &e : edits) {
 		const crs_mesh &mesh = flat->meshes[e.mesh];
-		CU(cudaMemcpyAsync(sc + e.o_polys, flat->polys + mesh.poly_offset, (size_t)e.n * sizeof(crs_poly), cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(sc + e.o_verts, flat->vertices + 3 * (size_t)e.vlo, (size_t)(e.vhi - e.vlo) * 12u, cudaMemcpyHostToDevice, st));
-		if (e.nhi > e.nlo) CU(cudaMemcpyAsync(sc + e.o_norms, flat->normals + 3 * (size_t)e.nlo, (size_t)(e.nhi - e.nlo) * 12u, cudaMemcpyHostToDevice, st));
-		if (e.thi > e.tlo) CU(cudaMemcpyAsync(sc + e.o_uvs, flat->texcoords + 2 * (size_t)e.tlo, (size_t)(e.thi - e.tlo) * 8u, cudaMemcpyHostToDevice, st));
-		const crs_poly *polys = reinterpret_cast<const crs_poly *>(sc + e.o_polys);
-		float *bb = reinterpret_cast<float *>(sc + e.o_bb), *ctr = reinterpret_cast<float *>(sc + e.o_ctr);
-		crg_launch_poly_boxes(polys, reinterpret_cast<const float *>(sc + e.o_verts), e.vlo, e.n, bb, ctr, st);
+		CU(cudaMemcpyAsync(e.polys, flat->polys + mesh.poly_offset, (size_t)e.n * sizeof(crs_poly), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(e.verts, flat->vertices + 3 * (size_t)e.vlo, (size_t)(e.vhi - e.vlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.nhi > e.nlo) CU(cudaMemcpyAsync(e.norms, flat->normals + 3 * (size_t)e.nlo, (size_t)(e.nhi - e.nlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.thi > e.tlo) CU(cudaMemcpyAsync(e.uvs, flat->texcoords + 2 * (size_t)e.tlo, (size_t)(e.thi - e.tlo) * 8u, cudaMemcpyHostToDevice, st));
+		crg_launch_poly_boxes(e.polys, e.verts, e.vlo, e.n, e.bb, e.ctr, st);
 		CU(cudaGetLastError());
-		int32_t *prims = reinterpret_cast<int32_t *>(sc + e.o_prims);
-		rc = crg_bvh_build_pairs(bb, ctr, e.n, sc + o_build, st, reinterpret_cast<PairNode *>(sc + e.o_pairs), prims, &e.res);
+		rc = crg_bvh_build_pairs(e.bb, e.ctr, e.n, build, st, e.pairs, e.prims, &e.res);
 		if (rc) return rc;
 		if (e.res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: BVH deeper than 64 levels", e.mesh);
-		const CrgMeshRepack r = { polys, reinterpret_cast<const float *>(sc + e.o_verts), reinterpret_cast<const float *>(sc + e.o_norms),
-		                          reinterpret_cast<const float *>(sc + e.o_uvs), e.vlo, e.nlo, e.tlo, e.n, mesh.poly_offset, mesh.material_offset,
-		                          mesh.texcoord_count };
-		crg_launch_mesh_repack(r, prims, reinterpret_cast<PackedTri *>(sc + e.o_tris), reinterpret_cast<uint32_t *>(sc + e.o_slot), sc + e.o_keys,
-		                       reinterpret_cast<ShadePoly *>(sc + e.o_spolys), st);
+		const CrgMeshRepack r = { e.polys, e.verts, e.norms, e.uvs, e.vlo, e.nlo, e.tlo, e.n, mesh.poly_offset, mesh.material_offset, mesh.texcoord_count };
+		crg_launch_mesh_repack(r, e.prims, e.tris, e.slot, e.keys, e.spolys, st);
 		CU(cudaGetLastError());
 	}
 
-	/* the top level over the new mesh roots, built from the roots in the instance scratch (restored if anything below fails) */
-	const uint32_t ninst = (uint32_t)s->inst_kind.size();
-	std::vector<float> roots = s->bvh_root;
+	/* the top level over the new mesh roots */
+	std::vector<float> roots = s->rec.bvh_root;
 	for (const MeshEdit &e : edits) memcpy(&roots[6 * (size_t)e.bvh], e.res.bounds, 6 * sizeof(float));
-	const EditLayout L = edit_layout(s);
-	float *droots = reinterpret_cast<float *>(static_cast<uint8_t *>(s->edit_scratch) + L.so[ES_ROOTS]);
-	auto undo = [&](int code) {
-		cudaMemcpyAsync(droots, s->bvh_root.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st);
-		cudaStreamSynchronize(st);
-		return code;
-	};
-	CU(cudaMemcpyAsync(droots, roots.data(), L.sz[ES_ROOTS], cudaMemcpyHostToDevice, st));
 	CrgBuildResult top;
 	memset(&top, 0, sizeof top);
 	if (ninst) {
-		rc = build_top(s, nullptr, &top);
-		if (rc) return undo(rc);
+		CU(cudaMemcpyAsync(t.roots, roots.data(), roots.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+		rc = alloc_insts(s);
+		if (!rc) rc = build_top(s, nullptr, t, build, &top);
+		if (rc) return rc;
 	}
+	/* the first geometry edit reserves the top region behind the uploaded pairs, and the first edit of a mesh its own region */
+	const uint32_t first = s->pairs.p ? s->pair_cap : s->pair_count + region_pairs(ninst);
 	uint32_t add = 0;
-	for (const MeshEdit &e : edits) if (s->mesh_region[e.mesh] == 0xffffffffu) add += e.n > 1u ? e.n - 1u : 1u;
-	if (add) {
-		const uint32_t first = s->edit_pairs;
-		if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return undo(fail(CRGPU_ERR_UNSUPPORTED, "set_meshes: more pair nodes than the scene can address"));
-		rc = grow_edit(s, add);
-		if (rc) return undo(rc);
+	for (const MeshEdit &e : edits) if (s->mesh_region[e.mesh] == 0xffffffffu) add += region_pairs(e.n);
+	if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "set_meshes: more pair nodes than the scene can address");
+	if (first + add > s->pair_cap) {
+		rc = reserve_pairs(s, first + add);
+		if (rc) return rc;
 		uint32_t next = first;
 		for (const MeshEdit &e : edits)
-			if (s->mesh_region[e.mesh] == 0xffffffffu) { s->mesh_region[e.mesh] = next; next += e.n > 1u ? e.n - 1u : 1u; }
+			if (s->mesh_region[e.mesh] == 0xffffffffu) { s->mesh_region[e.mesh] = next; next += region_pairs(e.n); }
 	}
 
 	/* commit: each mesh's region, slot and poly ranges, BVH record and staged prefix, then the instances and the top level */
-	PairNode *pairs = static_cast<PairNode *>(s->edit);
 	for (const MeshEdit &e : edits) {
-		const crs_mesh &mesh = s->meshes[e.mesh];
+		const crs_mesh &mesh = s->rec.meshes[e.mesh];
 		DevBvh &b = s->bvhs[e.bvh];
-		const PairNode *staged = reinterpret_cast<const PairNode *>(sc + e.o_pairs);
 		const uint32_t region = s->mesh_region[e.mesh];
-		if (e.res.pairs) CU(cudaMemcpyAsync(pairs + region, staged, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<PackedTri *>(s->dev.tris) + b.slot_offset, sc + e.o_tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<uint32_t *>(s->dev.slot_poly) + b.slot_offset, sc + e.o_slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.slot_key) + b.slot_offset, sc + e.o_keys, e.n, cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<ShadePoly *>(s->dev.spolys) + mesh.poly_offset, sc + e.o_spolys, (size_t)e.n * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
-		const uint32_t slot_offset = b.slot_offset, stage_base = b.stage_base;
-		memset(&b, 0, sizeof b);
-		b.pair_offset = region;
-		b.pair_end = region + e.res.pairs;
-		b.node_count = e.res.node_count;
-		b.slot_offset = slot_offset;
-		if (e.res.node_count == 1u) { memcpy(b.root_bounds, e.res.bounds, sizeof b.root_bounds); b.root_first = e.res.root_first; b.root_count = e.res.root_count; }
-		b.stage_base = stage_base;
-		b.stage_count = e.res.pairs < s->stage_cap[e.bvh] ? e.res.pairs : s->stage_cap[e.bvh];
+		if (e.res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + region, e.pairs, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<PackedTri *>(s->dev.tris) + b.slot_offset, e.tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<uint32_t *>(s->dev.slot_poly) + b.slot_offset, e.slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.slot_key) + b.slot_offset, e.keys, e.n, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<ShadePoly *>(s->dev.spolys) + mesh.poly_offset, e.spolys, (size_t)e.n * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
+		b = bvh_record(e.res, region, b.slot_offset, b.stage_base, s->stage_cap[e.bvh]);
 		CU(cudaMemcpyAsync(const_cast<DevBvh *>(s->dev.bvhs) + e.bvh, &b, sizeof b, cudaMemcpyHostToDevice, st));
 		if (b.stage_count)
-			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, staged, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, e.pairs, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	}
-	s->bvh_root = roots;
-	if (ninst) return commit_top(s, top);
-	s->dev.pairs = pairs;
-	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
-	CU(cudaStreamSynchronize(st));
-	return CRGPU_OK;
+	s->rec.bvh_root = roots;
+	if (ninst) return commit_top(s, t, top);
+	return publish(s);
 }
 
 /* ---- shading edits ------------------------------------------------------------------------------------------------------------------
@@ -1829,20 +1801,20 @@ extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *f
 	if (rc) return rc;
 	rc = drain(s);
 	if (rc) return rc;
-	const size_t node_bytes = (size_t)flat->node_count * sizeof(crs_node), tex_bytes = sh.texs.size() * sizeof(DevTexture);
-	const size_t o_texs = align256(node_bytes), o_data = o_texs + align256(tex_bytes), bytes = o_data + align256((size_t)flat->texdata_bytes);
-	void *blk = nullptr;
-	rc = ctx_alloc(s->device, bytes, &blk);
+	DevBlock blk;
+	crs_node *nodes = nullptr;
+	DevTexture *texs = nullptr;
+	uint8_t *data = nullptr;
+	rc = carve(s->device, blk, [&](Carve &c) { nodes = c.take<crs_node>(flat->node_count); texs = c.take<DevTexture>(sh.texs.size()); data = c.take<uint8_t>(flat->texdata_bytes); });
 	if (rc) return rc;
-	uint8_t *base = static_cast<uint8_t *>(blk);
-	for (DevTexture &t : sh.texs) t.data = base + o_data + (uintptr_t)t.data;
+	for (DevTexture &t : sh.texs) t.data = data + (uintptr_t)t.data;
 	cudaStream_t st = s->stream;
 	cudaError_t ce = cudaSuccess;
-	if (node_bytes) ce = cudaMemcpyAsync(base, flat->nodes, node_bytes, cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && tex_bytes) ce = cudaMemcpyAsync(base + o_texs, sh.texs.data(), tex_bytes, cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(base + o_data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
+	if (flat->node_count) ce = cudaMemcpyAsync(nodes, flat->nodes, (size_t)flat->node_count * sizeof(crs_node), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && !sh.texs.empty()) ce = cudaMemcpyAsync(texs, sh.texs.data(), sh.texs.size() * sizeof(DevTexture), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
 	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) { ctx_free(s->device, blk, bytes); return fail(CRGPU_ERR_CUDA, "set_shading: %s", cudaGetErrorString(ce)); }
+	if (ce != cudaSuccess) { ctx_free(s->device, blk.p, blk.bytes); return fail(CRGPU_ERR_CUDA, "set_shading: %s", cudaGetErrorString(ce)); }
 
 	/* commit */
 	const size_t nm = s->material_count;
@@ -1851,17 +1823,17 @@ extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *f
 		CU(cudaMemcpyAsync(const_cast<DevFlat *>(s->dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
 	}
 	CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
-	s->dev.nodes = reinterpret_cast<const crs_node *>(base);
-	s->dev.textures = reinterpret_cast<const DevTexture *>(base + o_texs);
+	s->dev.nodes = nodes;
+	s->dev.textures = texs;
 	s->dev.bg = sh.bg;
 	s->dev.flat_keys = sh.flat_keys;
 	s->dev.background = flat->background;
 	s->xnodes = sh.xnodes;
-	CU(cudaMemcpyAsync(s->dev_copy, &s->dev, sizeof(DevScene), cudaMemcpyHostToDevice, st));
-	CU(cudaStreamSynchronize(st));
-	ctx_free(s->device, s->shade, s->shade_bytes);
-	s->shade = blk; s->shade_bytes = bytes;
-	return CRGPU_OK;
+	const DevBlock old = s->shade;
+	s->shade = blk;
+	rc = publish(s);
+	if (!rc) ctx_free(s->device, old.p, old.bytes);   /* the descriptor no longer points at it */
+	return rc;
 }
 
 extern "C" int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,

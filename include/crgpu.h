@@ -173,10 +173,11 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *   crgpu_scene_set_instances  takes A and Ainv of each instance bit for bit (Ainv is not recomputed); `count`, and each instance's
  *                              kind and object, must be those uploaded (instances cannot be added or removed).  The instance
  *                              boxes, ray offsets and the top-level BVH are rebuilt on the device, the tree that the scene loader
- *                              builds.  The first call gives the scene its own copy of the BVH pair nodes (the uploaded pairs plus
- *                              room for any top level of `count` instances); later calls reuse it.  A top level that needs more
- *                              than count - 1 pair nodes (a tree of more than 2 count - 1 nodes, which only instances whose boxes no
- *                              split separates make: see crloader_build_bvh in crloader.h) is refused with CRGPU_ERR_UNSUPPORTED.
+ *                              builds.  The first instance or mesh edit gives the scene its own copy of the BVH pair nodes (the
+ *                              uploaded pairs plus room for any top level of `count` instances) and its own top-level item records;
+ *                              later edits reuse them.  A top level that needs more than count - 1 pair nodes (a tree of more than
+ *                              2 count - 1 nodes, which only instances whose boxes no split separates make: see crloader_build_bvh
+ *                              in crloader.h) is refused with CRGPU_ERR_UNSUPPORTED.
  *   crgpu_scene_set_meshes     deforms meshes (crTransformMesh, "recompute kd-tree"): every mesh listed in `meshes` takes its polys,
  *                              flat->polys[poly_offset .. + poly_count), and the vertices, normals and texture coordinates they
  *                              index from `flat`; positions, normals, uvs and each poly's material (within the mesh's material

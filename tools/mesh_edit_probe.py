@@ -7,12 +7,12 @@ Cases (tests/test_gpu_mesh_edit.py builds the same deformations):
   grid      a generated 1,002,528-triangle grid mesh
   reload    crloader_load_json_buf of the deformed scene + crgpu_prepare + crgpu_scene_create_prepared (what the edit costs without
             set_meshes)
-  first     the first set_meshes of the mesh (it also creates the scene's edit block and the mesh's region)
+  first     the first set_meshes of the mesh (it also creates the scene's pairs and instance blocks and the mesh's region)
   later     later set_meshes calls (alternating the deformed and the original geometry)
 Each edit is also checked against a fresh upload of the deformed scene at a small size (frame and traced records, bit for bit).
 Then bench.py runs once on the unedited default workload and its frame CRC is printed.  Times are host wall clock around calls that
-end in a device synchronise; medians of --reps.  The bytes are the edit block (uploaded pairs, top region, mesh regions, item
-records) and the mesh edit's staged inputs and records, from crgpu_api.cu's layout (the builder's own scratch comes on top).
+end in a device synchronise; medians of --reps.  The bytes are the pairs block (uploaded pairs, top region, mesh regions) plus the
+instance block (last-instance table, item records), and the call's scratch without the builder's own, from crgpu_api.cu's layout.
 
     python tools/mesh_edit_probe.py [--reps 10] [--out results.json]
 """
@@ -43,13 +43,14 @@ def a256(b):
 
 
 def layout_bytes(flat, meshes):
-    """(edit block, mesh edit inputs + records) bytes of a first set_meshes of `meshes` on a scene uploaded from `flat`."""
+    """(pairs block + instance block, scratch without the builder's own) bytes of a first set_meshes of `meshes` on a scene uploaded
+    from `flat`."""
     A = crscene.arrays(flat)
     internal = sum((int(b["node_count"]) - 1) // 2 for i, b in enumerate(A["bvhs"]) if b["node_count"] > 1)
     n_inst = len(A["instances"])
     regions = sum(max(1, int(A["meshes"][m]["poly_count"]) - 1) for m in meshes)
-    edit = a256((internal + max(1, n_inst - 1) + regions) * 64) + n_inst * 64
-    staged = 0
+    blocks = (internal + max(1, n_inst - 1) + regions) * 64 + (a256(n_inst * 4) + n_inst * 64 if n_inst else 0)
+    scratch = 0
     for m in meshes:
         mesh = A["meshes"][m]
         n = int(mesh["poly_count"])
@@ -58,9 +59,11 @@ def layout_bytes(flat, meshes):
         nn = polys["n"][polys["has_normals"] != 0].ravel()
         t = polys["t"][(polys["t"][:, 0] != -1)].ravel() if mesh["texcoord_count"] else np.zeros(0, np.int32)
         rng = lambda x, w: a256((int(x.max()) - int(x.min()) + 1) * w if len(x) else 0)
-        staged += (a256(n * 44) + rng(v, 12) + rng(nn, 12) + rng(t, 8) + a256(n * 24) + a256(n * 12) + a256(max(1, n - 1) * 64)
-                   + a256(n * 4) + a256(n * 48) + a256(n * 4) + a256(n) + a256(n * 80))
-    return edit, staged
+        scratch += (a256(n * 44) + rng(v, 12) + rng(nn, 12) + rng(t, 8) + a256(n * 24) + a256(n * 12) + a256(max(1, n - 1) * 64)
+                    + a256(n * 4) + a256(n * 48) + a256(n * 4) + a256(n) + a256(n * 80))
+    scratch += (a256(len(A["bvhs"]) * 24) + a256(n_inst * 24) + a256(n_inst * 12) + a256(n_inst * 4) + a256(n_inst * 128)
+                + a256(max(1, n_inst - 1) * 64) + a256(n_inst * 4))
+    return blocks, scratch
 
 
 def docs(case):
@@ -108,7 +111,7 @@ def probe(case, reps):
     ch = M.changed_meshes(a, b)
     n_inst = len(a.instances)
     polys = int(sum(crscene.arrays(a.flat)["meshes"]["poly_count"][ch]))
-    edit_bytes, staged_bytes = layout_bytes(a.flat, ch)
+    block_bytes, scratch_bytes = layout_bytes(a.flat, ch)
     g = a.upload()
     first = wall(lambda: g.set_meshes(b.flat, ch))
     later = [wall(lambda k=k: g.set_meshes((a if k % 2 == 0 else b).flat, ch)) for k in range(reps)]
@@ -128,7 +131,7 @@ def probe(case, reps):
     sb.close()
     return dict(case=case, meshes=ch, triangles=polys, instances=n_inst, size=cfg[:2],
                 set_meshes_first_ms=first, set_meshes_ms=float(np.median(later)), reload_prepare_create_ms=float(np.median(reload)),
-                edit_block_bytes=edit_bytes, mesh_inputs_records_bytes=staged_bytes, checked=True)
+                pairs_instance_blocks_bytes=block_bytes, scratch_bytes=scratch_bytes, checked=True)
 
 
 def main():
