@@ -142,6 +142,9 @@ def lib():
         if hasattr(L, "crgpu_scene_set_meshes"):   # absent from libraries built before mesh edits
             L.crgpu_scene_set_meshes.argtypes = [P, C.POINTER(FlatScene), P, C.c_uint32]
             L.crgpu_scene_set_meshes.restype = C.c_int
+        if hasattr(L, "crgpu_scene_set_instance_list"):   # absent from libraries built before instance-list edits
+            L.crgpu_scene_set_instance_list.argtypes = [P, P, C.c_uint32]
+            L.crgpu_scene_set_instance_list.restype = C.c_int
         if hasattr(L, "crgpu_scene_set_shading"):  # absent from libraries built before shading edits
             L.crgpu_scene_set_shading.argtypes = [P, C.POINTER(FlatScene)]
             L.crgpu_scene_shading.argtypes = [P, P, P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
@@ -272,6 +275,15 @@ class GpuScene:
         import crscene
         arr = np.ascontiguousarray(instances, dtype=crscene.INSTANCE)
         _check(lib().crgpu_scene_set_instances(self.handle, arr.ctypes.data, len(arr)), "crgpu_scene_set_instances")
+
+    def set_instance_list(self, instances):
+        """Replace the whole instance list (crgpu_scene_set_instance_list): an array of struct crs_instance (crscene.INSTANCE) of any
+        length up to 4,194,304, each a sphere or mesh the scene was uploaded with; A and Ainv are taken bit for bit and the top-level
+        BVH is rebuilt on the device."""
+        import crscene
+        arr = np.ascontiguousarray(instances, dtype=crscene.INSTANCE)
+        _check(lib().crgpu_scene_set_instance_list(self.handle, arr.ctypes.data if len(arr) else None, len(arr)),
+               "crgpu_scene_set_instance_list")
 
     def set_meshes(self, flat, meshes):
         """Deform meshes of the resident scene (crgpu_scene_set_meshes): each mesh index in `meshes` takes its polys and the

@@ -141,14 +141,16 @@ extern "C" void crgpu_host_free(void *p) { if (p) cudaFreeHost(p); }
  * pointer-carrying tables.  A host that renders many frames of one scene, or one frame on many GPUs, prepares once. */
 enum { SEC_STAGE, SEC_PAIRS, SEC_TRIS, SEC_SLOT_POLY, SEC_KEYS, SEC_SPOLYS, SEC_TOP_ITEMS, SEC_BVHS, SEC_INSTS, SEC_MATS, SEC_FLAT, SEC_ORDER, SEC_NODES, SEC_TEXS, SEC_LUT,
        SEC_TEXDATA, SEC_COUNT };
-/* What the geometry edits (crgpu_scene_set_instances, crgpu_scene_set_meshes) need beyond the slab: the records they check an edit
- * against, and the BVH root bounds they build the top level from. */
+/* What the geometry edits (crgpu_scene_set_instances, crgpu_scene_set_meshes, crgpu_scene_set_instance_list) need beyond the slab:
+ * the records they check an edit against, the BVH root bounds they build the top level from, and the objects a new instance list
+ * may instance. */
 struct EditRecord {
-	std::vector<uint32_t> inst_kind, inst_object;   /* kind and object of every instance: an edit must keep them */
+	std::vector<uint32_t> inst_kind, inst_object;   /* kind and object of every instance of the current list */
 	std::vector<uint32_t> last;                      /* the last instance of each instance's object: all of them take its ray offset */
 	std::vector<float> bvh_root;                     /* root bounds of every BVH as stored, 6 floats each (the slab keeps only pair
 	                                                    nodes, whose roots' own boxes are not in it); an edited scene keeps them current */
 	std::vector<crs_mesh> meshes;                    /* every mesh record: an edit must keep each */
+	std::vector<crs_sphere> spheres;                 /* every sphere record: radius and material of its instances */
 	std::vector<uint32_t> bvh_prims;                 /* primitives of each BVH */
 };
 struct crgpu_prepared {
@@ -170,6 +172,16 @@ struct crgpu_prepared {
 	size_t slab_bytes;
 	size_t off[SEC_COUNT], len[SEC_COUNT];
 	EditRecord rec;
+};
+
+/* The parts of an edited scene's instance block: the last-instance table and the top level's item records, then, from the first
+ * instance-list edit on, the scene's own instance records and instance keys (DevScene::instances and inst_key point at them in place
+ * of the slab's SEC_INSTS and key tail). */
+struct InstParts {
+	uint32_t *last;
+	DevTopItem *items;
+	DevInstance *recs;         /* NULL before the first list edit */
+	uint8_t *keys;             /* NULL before the first list edit */
 };
 
 struct crgpu_scene {
@@ -214,10 +226,14 @@ struct crgpu_scene {
 	std::vector<uint32_t> mesh_region;   /* first pair of a mesh's own region in the pairs block (UINT32_MAX: none yet) */
 	uint32_t pair_count = 0;         /* pair nodes uploaded */
 	uint32_t pair_cap = 0;           /* pair nodes dev.pairs holds: pair_count until the first geometry edit, then the pairs block's */
+	uint32_t top_off = 0, top_cap = 0;   /* the top region in the pairs block: first pair and room, at least max(1, n - 1) for the current
+	                                        n instances (reserved behind the uploaded pairs until a list outgrows it) */
 	uint32_t top_stage_cap = 0;      /* staged top-level pairs reserved at upload */
 	uint32_t material_count = 0;     /* as uploaded: a shading edit must keep it */
 	DevBlock pairs;                  /* NULL until the first geometry edit: the uploaded pairs, the top region, the edited meshes' regions */
-	DevBlock insts;                  /* NULL until the first geometry edit: EditRecord::last, then the top level's item records */
+	DevBlock insts;                  /* NULL until the first geometry edit: the instance block (InstParts) */
+	InstParts ip = {};               /* its parts */
+	uint32_t inst_cap = 0;           /* instances it has room for */
 	DevBlock scratch;                /* a geometry edit's inputs, records and builder scratch; grows only, and nothing in it outlives a call */
 	DevBlock shade;                  /* NULL until the first shading edit: the node graph, texture table and texel data the kernels read in
 	                                    place of the slab's */
@@ -549,6 +565,59 @@ static void host_parallel_for(uint32_t n, F fn) {
 		pool.emplace_back(fn, (uint32_t)((uint64_t)n * k / threads), (uint32_t)((uint64_t)n * (k + 1) / threads));
 	fn(0u, (uint32_t)((uint64_t)n / threads));
 	for (auto &t : pool) t.join();
+}
+
+/* ---- instance packing: the DevInstance records, the sphere instances' shading keys and the last-instance table of a list ----------
+ * crgpu_prepare and crgpu_scene_set_instance_list both take them from here.  An instance of another kind is refused with `bad_kind`
+ * (crgpu_prepare: CRGPU_ERR_UNSUPPORTED, volumes; an edit: CRGPU_ERR_BAD_ARGUMENT), an object or a sphere material out of range with
+ * CRGPU_ERR_BAD_ARGUMENT.  ray_offset is the object's as loaded; the top-level build on the device recomputes it. */
+struct InstancePack {
+	std::vector<DevInstance> recs;
+	std::vector<uint8_t> keys;         /* min(material + 1, 255) of a sphere instance, 0 for a mesh instance */
+	std::vector<uint32_t> last;
+};
+static uint8_t shade_key(uint32_t material) { return (uint8_t)(material + 1u < 255u ? material + 1u : 255u); }
+
+static int pack_instances(const crs_instance *inst, uint32_t n, const crs_sphere *spheres, uint32_t sphere_count, const crs_mesh *meshes,
+                          uint32_t mesh_count, uint32_t material_count, int bad_kind, InstancePack &out) {
+	std::vector<uint32_t> last_of[2] = { std::vector<uint32_t>(mesh_count), std::vector<uint32_t>(sphere_count) };   /* by kind, object */
+	for (uint32_t i = 0; i < n; ++i) {
+		const crs_instance &src = inst[i];
+		if (src.kind == CRS_INST_MESH) {
+			if (src.object >= mesh_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "instance mesh index out of range");
+		} else if (src.kind == CRS_INST_SPHERE) {
+			if (src.object >= sphere_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "instance sphere index out of range");
+			if (spheres[src.object].material >= material_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "sphere material out of range");
+		} else {
+			return fail(bad_kind, "instance %u has kind %u (volumes are not reachable from the scene loader)", i, src.kind);
+		}
+		last_of[src.kind == CRS_INST_SPHERE][src.object] = i;
+	}
+	out.recs.resize(n);
+	out.keys.assign(n, 0u);
+	out.last.resize(n);
+	host_parallel_for(n, [&](uint32_t lo, uint32_t hi) {
+		for (uint32_t i = lo; i < hi; ++i) {
+			const crs_instance &src = inst[i];
+			DevInstance d;
+			memset(&d, 0, sizeof d);
+			memcpy(d.Ainv, src.Ainv, sizeof d.Ainv);
+			memcpy(d.A, src.A, sizeof d.A);
+			d.kind = src.kind;
+			if (src.kind == CRS_INST_MESH) {
+				d.bvh = meshes[src.object].bvh;
+				d.ray_offset = meshes[src.object].ray_offset;
+			} else {
+				d.ray_offset = spheres[src.object].ray_offset;
+				d.radius = spheres[src.object].radius;
+				d.material = spheres[src.object].material;
+				out.keys[i] = shade_key(d.material);
+			}
+			out.recs[i] = d;
+			out.last[i] = last_of[src.kind == CRS_INST_SPHERE][src.object];
+		}
+	});
+	return CRGPU_OK;
 }
 
 static int build_pairs(const crs_scene *f, const crs_bvh &b, std::vector<PairNode> &pairs, DevBvh &out, uint32_t slot_offset, HostError *err) {
@@ -887,41 +956,23 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 
 	/* instances */
 	if (f->instance_count > CRG_ITEM_INDEX + 1u) { return pfail(p, fail(CRGPU_ERR_UNSUPPORTED, "more than 2^30 instances")); }
-	std::vector<DevInstance> insts(f->instance_count);
-	for (uint32_t i = 0; i < f->instance_count; ++i) {
-		const crs_instance &src = f->instances[i];
-		DevInstance d;
-		memset(&d, 0, sizeof d);
-		memcpy(d.Ainv, src.Ainv, sizeof d.Ainv);
-		memcpy(d.A, src.A, sizeof d.A);
-		d.kind = src.kind;
-		if (src.kind == CRS_INST_MESH) {
-			if (src.object >= f->mesh_count) { return pfail(p, fail(CRGPU_ERR_BAD_ARGUMENT, "instance mesh index out of range")); }
-			d.bvh = f->meshes[src.object].bvh;
-			d.ray_offset = f->meshes[src.object].ray_offset;
-		} else if (src.kind == CRS_INST_SPHERE) {
-			if (src.object >= f->sphere_count) { return pfail(p, fail(CRGPU_ERR_BAD_ARGUMENT, "instance sphere index out of range")); }
-			d.ray_offset = f->spheres[src.object].ray_offset;
-			d.radius = f->spheres[src.object].radius;
-			d.material = f->spheres[src.object].material;
-			if (d.material >= f->material_count) { return pfail(p, fail(CRGPU_ERR_BAD_ARGUMENT, "sphere material out of range")); }
-		} else { return pfail(p, fail(CRGPU_ERR_UNSUPPORTED, "instance kind %u (volumes are not reachable from the scene loader)", src.kind)); }
-		insts[i] = d;
-	}
+	InstancePack pk;
+	PFAIL(pack_instances(f->instances, f->instance_count, f->spheres, f->sphere_count, f->meshes, f->mesh_count, f->material_count,
+	                     CRGPU_ERR_UNSUPPORTED, pk));
+	const std::vector<DevInstance> &insts = pk.recs;
 	EditRecord &rec = p->rec;
-	std::vector<uint32_t> last_of[2] = { std::vector<uint32_t>(f->mesh_count), std::vector<uint32_t>(f->sphere_count) };   /* by kind, object */
 	for (uint32_t i = 0; i < f->instance_count; ++i) {
 		rec.inst_kind.push_back(f->instances[i].kind);
 		rec.inst_object.push_back(f->instances[i].object);
-		last_of[f->instances[i].kind == CRS_INST_SPHERE][f->instances[i].object] = i;
 	}
-	for (uint32_t i = 0; i < f->instance_count; ++i) rec.last.push_back(last_of[rec.inst_kind[i] == CRS_INST_SPHERE][rec.inst_object[i]]);
+	rec.last = pk.last;
 	rec.bvh_root.assign(6 * (size_t)f->bvh_count, 0.0f);
 	for (uint32_t b = 0; b < f->bvh_count; ++b) {
 		if (f->bvhs[b].node_count) memcpy(&rec.bvh_root[6 * (size_t)b], f->bvh_nodes[f->bvhs[b].node_offset].bounds, 6 * sizeof(float));
 		rec.bvh_prims.push_back(f->bvhs[b].prim_count);
 	}
 	rec.meshes.assign(f->meshes, f->meshes + f->mesh_count);
+	rec.spheres.assign(f->spheres, f->spheres + f->sphere_count);
 
 	std::vector<crs_node> nodes(f->nodes, f->nodes + f->node_count);
 
@@ -963,14 +1014,10 @@ extern "C" int crgpu_prepare(const struct crs_scene *f, crgpu_prepared **out) {
 	}
 	/* shading keys (K4's buckets): min(material + 1, 255) per prim slot from its poly, then per instance for spheres */
 	std::vector<uint8_t> keys((size_t)total_slots + f->instance_count, 0u);
-	{
-		auto key_of = [](uint32_t material) { return (uint8_t)(material + 1u < 255u ? material + 1u : 255u); };
-		host_parallel_for((uint32_t)total_slots, [&](uint32_t lo, uint32_t hi) {
-			for (uint32_t i = lo; i < hi; ++i) keys[i] = key_of(spolys[slot_poly[i]].material);
-		});
-		for (uint32_t i = 0; i < f->instance_count; ++i)
-			if (insts[i].kind == CRS_INST_SPHERE) keys[(size_t)total_slots + i] = key_of(insts[i].material);
-	}
+	host_parallel_for((uint32_t)total_slots, [&](uint32_t lo, uint32_t hi) {
+		for (uint32_t i = lo; i < hi; ++i) keys[i] = shade_key(spolys[slot_poly[i]].material);
+	});
+	std::copy(pk.keys.begin(), pk.keys.end(), keys.begin() + (ptrdiff_t)total_slots);
 	p->key_inst_off = (size_t)total_slots;
 	p->material_count = f->material_count;
 	std::vector<float> lut(256);
@@ -1025,6 +1072,8 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	for (const DevBvh &b : s->bvhs) s->stage_cap.push_back(b.stage_count);
 	s->mesh_region.assign(p->rec.meshes.size(), 0xffffffffu);
 	s->pair_count = s->pair_cap = (uint32_t)(p->len[SEC_PAIRS] / sizeof(PairNode));
+	s->top_off = s->pair_count;
+	s->top_cap = p->instance_count > 1u ? p->instance_count - 1u : 1u;
 	s->top_stage_cap = p->top.stage_count;
 	s->material_count = p->material_count;
 #define FAIL_IF(x) do { int rc_ = (x); if (rc_) { crgpu_scene_destroy(s); return rc_; } } while (0)
@@ -1496,22 +1545,36 @@ template <class F> static int carve(int device, DevBlock &blk, F layout) {
 }
 
 /* The top-level build's part of an edit call's scratch: the BVH roots it reads, the instance boxes, centres and ray offsets, the new
- * instance records, and the new top level's pairs and primitive order. */
+ * instance records, and the new top level's pairs and primitive order, for n instances.  A list edit also stages its last-instance
+ * table and instance keys there; the other edits read the instance block's table. */
 struct TopParts {
 	float *roots, *bb, *ctr, *offs;
 	DevInstance *insts;
 	PairNode *pairs;
 	int32_t *prims;
+	uint32_t *last;
+	uint8_t *keys;
 };
-static TopParts take_top(Carve &c, const crgpu_scene *s) {
-	const size_t n = s->rec.inst_kind.size();
+static TopParts take_top(Carve &c, const crgpu_scene *s, uint32_t n, bool list = false) {
 	TopParts t;
 	t.roots = c.take<float>(s->rec.bvh_root.size());
-	t.bb = c.take<float>(6 * n); t.ctr = c.take<float>(3 * n); t.offs = c.take<float>(n);
+	t.bb = c.take<float>(6 * (size_t)n); t.ctr = c.take<float>(3 * (size_t)n); t.offs = c.take<float>(n);
 	t.insts = c.take<DevInstance>(n);
-	t.pairs = c.take<PairNode>(region_pairs((uint32_t)n));
+	t.pairs = c.take<PairNode>(region_pairs(n));
 	t.prims = c.take<int32_t>(n);
+	t.last = list ? c.take<uint32_t>(n) : nullptr;
+	t.keys = list ? c.take<uint8_t>(n) : nullptr;
 	return t;
+}
+
+/* The instance block's parts for cap instances; `own`: with the scene's own instance records and keys. */
+static InstParts take_insts(Carve &c, uint32_t cap, bool own) {
+	InstParts q;
+	q.last = c.take<uint32_t>(cap);
+	q.items = c.take<DevTopItem>(cap);
+	q.recs = own ? c.take<DevInstance>(cap) : nullptr;
+	q.keys = own ? c.take<uint8_t>(cap) : nullptr;
+	return q;
 }
 
 /* The DevBvh record of a device build whose pairs sit at pair_offset; it stages at most stage_cap of them at stage_base. */
@@ -1547,29 +1610,33 @@ static int reserve_pairs(crgpu_scene *s, uint32_t count) {
 	return rc;
 }
 
-/* The first geometry edit of a scene with instances gives it its instance block: EditRecord::last, which never changes, then room
- * for the top level's item records. */
+/* The first instance or mesh edit of a scene with instances gives it its instance block for the uploaded list: EditRecord::last,
+ * then room for the top level's item records.  The slab's instance records and keys stay in use until a list edit. */
 static int alloc_insts(crgpu_scene *s) {
 	if (s->insts.p) return CRGPU_OK;
-	const size_t n = s->rec.last.size();
-	const size_t bytes = align256(n * 4u) + n * sizeof(DevTopItem);
-	int rc = ctx_alloc(s->device, bytes, &s->insts.p);
+	const uint32_t n = (uint32_t)s->rec.last.size();
+	InstParts q = {};
+	int rc = carve(s->device, s->insts, [&](Carve &c) { q = take_insts(c, n, false); });
 	if (rc) return rc;
-	s->insts.bytes = bytes;
-	cudaError_t ce = cudaMemcpyAsync(s->insts.p, s->rec.last.data(), n * 4u, cudaMemcpyHostToDevice, s->stream);
-	if (ce == cudaSuccess) return CRGPU_OK;
-	ctx_free(s->device, s->insts.p, s->insts.bytes);
-	s->insts = DevBlock();
-	return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
+	cudaError_t ce = cudaMemcpyAsync(q.last, s->rec.last.data(), (size_t)n * 4u, cudaMemcpyHostToDevice, s->stream);
+	if (ce != cudaSuccess) {
+		ctx_free(s->device, s->insts.p, s->insts.bytes);
+		s->insts = DevBlock();
+		return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
+	}
+	s->ip = q;
+	s->inst_cap = n;
+	return CRGPU_OK;
 }
 
-/* Instance boxes, ray offsets and the top-level BVH into the scratch parts t: A and Ainv from inst (device), or the scene's current
- * instance records when inst is NULL; mesh boxes from t.roots. */
-static int build_top(crgpu_scene *s, const crs_instance *inst, const TopParts &t, void *build, CrgBuildResult *res) {
-	const uint32_t n = (uint32_t)s->rec.inst_kind.size();
+/* Instance boxes, ray offsets and the top-level BVH of n instances into the scratch parts t, mesh boxes from t.roots.  The records
+ * start from `from` (the scene's current ones), or from what t.insts already holds when it is NULL; A and Ainv from inst (device)
+ * when it is not NULL.  The offsets follow t.last, or the instance block's table when it is NULL. */
+static int build_top(crgpu_scene *s, uint32_t n, const DevInstance *from, const crs_instance *inst, const TopParts &t, void *build,
+                     CrgBuildResult *res) {
 	cudaStream_t st = s->stream;
-	CU(cudaMemcpyAsync(t.insts, s->dev.instances, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
-	crg_launch_instance_boxes(inst, t.insts, t.roots, static_cast<const uint32_t *>(s->insts.p), n, t.bb, t.ctr, t.offs, st);
+	if (from && n) CU(cudaMemcpyAsync(t.insts, from, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
+	crg_launch_instance_boxes(inst, t.insts, t.roots, t.last ? t.last : s->ip.last, n, t.bb, t.ctr, t.offs, st);
 	CU(cudaGetLastError());
 	int rc = crg_bvh_build_pairs(t.bb, t.ctr, n, build, st, t.pairs, t.prims, res);
 	if (rc) return rc;
@@ -1577,22 +1644,21 @@ static int build_top(crgpu_scene *s, const crs_instance *inst, const TopParts &t
 	return CRGPU_OK;
 }
 
-/* Copies a built top level over the scene's instances, top region, item records and staged prefix, and publishes the descriptor.
- * The BVH records the items read must already be committed. */
-static int commit_top(crgpu_scene *s, const TopParts &t, const CrgBuildResult &res) {
-	const uint32_t n = (uint32_t)s->rec.inst_kind.size();
+/* Copies a built top level of n instances over the scene's instance records, top region, item records and staged prefix, and
+ * publishes the descriptor.  The BVH records the items read, the instance block and the top region must already be committed. */
+static int commit_top(crgpu_scene *s, uint32_t n, const TopParts &t, const CrgBuildResult &res) {
 	cudaStream_t st = s->stream;
-	const DevBvh top = bvh_record(res, s->pair_count, 0u, s->dev.top.stage_base, s->top_stage_cap);
-	DevTopItem *items = reinterpret_cast<DevTopItem *>(static_cast<uint8_t *>(s->insts.p) + align256((size_t)n * 4u));
-	CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), t.insts, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
+	const DevBvh top = bvh_record(res, s->top_off, 0u, s->dev.top.stage_base, s->top_stage_cap);
+	if (n) CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), t.insts, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
 	if (res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + top.pair_offset, t.pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	crg_launch_top_items(t.prims, t.insts, s->dev.bvhs, n, items, st);
+	crg_launch_top_items(t.prims, t.insts, s->dev.bvhs, n, s->ip.items, st);
 	CU(cudaGetLastError());
 	if (top.stage_count)
 		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + top.stage_base, t.pairs, (size_t)top.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	s->dev.top = top;
-	s->dev.top_items = items;
-	world_box(res.bounds, s->dev.world_lo, s->dev.world_inv);
+	s->dev.top_items = s->ip.items;
+	static const float unit[6] = { 0.f, 1.f, 0.f, 1.f, 0.f, 1.f };  /* crgpu_prepare's box of an empty top level */
+	world_box(res.node_count ? res.bounds : unit, s->dev.world_lo, s->dev.world_inv);
 	return publish(s);
 }
 
@@ -1612,17 +1678,99 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	crs_instance *dinst = nullptr;
 	TopParts t;
 	void *build = nullptr;
-	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
+	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s, n); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
 	if (!rc) rc = alloc_insts(s);
 	if (rc) return rc;
 	/* the roots in a copy of their own: packing them behind the caller's instances would cost a host copy of every instance */
 	CU(cudaMemcpyAsync(dinst, inst, (size_t)n * sizeof(crs_instance), cudaMemcpyHostToDevice, s->stream));
 	CU(cudaMemcpyAsync(t.roots, s->rec.bvh_root.data(), s->rec.bvh_root.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
 	CrgBuildResult res;
-	rc = build_top(s, dinst, t, build, &res);
-	if (!rc && !s->pairs.p) rc = reserve_pairs(s, s->pair_count + region_pairs(n));
+	rc = build_top(s, n, s->dev.instances, dinst, t, build, &res);
+	if (!rc && !s->pairs.p) rc = reserve_pairs(s, s->top_off + s->top_cap);
 	if (rc) return rc;
-	return commit_top(s, t, res);
+	return commit_top(s, n, t, res);
+}
+
+/* ---- instance-list edits ------------------------------------------------------------------------------------------------------------
+ * The new list is validated and packed on the host (pack_instances, as crgpu_prepare packs it), and its boxes, ray offsets and top level
+ * are built on the device into scratch.  Only once the build has passed the upload's checks do the blocks change: the pairs block
+ * grows when the top region cannot hold a top level of the new count, and the instance block is replaced when it has no records of
+ * its own or no room for the new count.  Then the records, keys, last table, top region, item records and staged prefix are
+ * committed and published, and the replaced instance block goes back to the per-device cache. */
+extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
+	if (!s || (count && !inst)) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "%u instances (the device builder's limit is 4194304)", count);
+	InstancePack pk;
+	int rc = pack_instances(inst, count, s->rec.spheres.data(), (uint32_t)s->rec.spheres.size(), s->rec.meshes.data(), (uint32_t)s->rec.meshes.size(),
+	                        s->material_count, CRGPU_ERR_BAD_ARGUMENT, pk);
+	if (rc) return rc;
+	rc = drain(s);
+	if (rc) return rc;
+	const uint32_t n = count;
+	TopParts t;
+	void *build = nullptr;
+	rc = carve(s->device, s->scratch, [&](Carve &c) { t = take_top(c, s, n, true); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
+	if (rc) return rc;
+	cudaStream_t st = s->stream;
+	if (n) {
+		CU(cudaMemcpyAsync(t.insts, pk.recs.data(), (size_t)n * sizeof(DevInstance), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(t.last, pk.last.data(), (size_t)n * 4u, cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(t.keys, pk.keys.data(), n, cudaMemcpyHostToDevice, st));
+	}
+	CU(cudaMemcpyAsync(t.roots, s->rec.bvh_root.data(), s->rec.bvh_root.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+	CrgBuildResult res;
+	rc = build_top(s, n, nullptr, nullptr, t, build, &res);
+	if (rc) return rc;
+
+	/* the top region: the current one while it holds any top level of n instances (region_pairs(n)), else a new one behind every pair
+	 * of the block; mesh regions never move.  A region that has to move grows by half at least, so that adding instances a few at a
+	 * time does not leave a trail of abandoned regions. */
+	uint32_t top_off = s->top_off, top_cap = s->top_cap;
+	if (region_pairs(n) > top_cap) {
+		const uint64_t want = (uint64_t)top_cap + top_cap / 2u;
+		top_cap = want > region_pairs(n) ? (uint32_t)want : region_pairs(n);
+		if (s->pairs.p) top_off = s->pair_cap;            /* before the first geometry edit the reserved region is simply larger */
+	}
+	const uint64_t need = (uint64_t)top_off + top_cap;
+	if (need > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "set_instance_list: more pair nodes than the scene can address");
+	if (!s->pairs.p || need > s->pair_cap) {
+		rc = reserve_pairs(s, (uint32_t)(need > s->pair_cap ? need : s->pair_cap));
+		if (rc) return rc;
+	}
+	/* the instance block: kept while it has records of its own and room for n, else a new one (growing by half at least) */
+	DevBlock old;
+	if (!s->ip.recs || n > s->inst_cap) {
+		const uint64_t grown = (uint64_t)s->inst_cap + s->inst_cap / 2u;
+		const uint32_t cap = s->ip.recs && grown > n ? (uint32_t)(grown < 4194304u ? grown : 4194304u) : n;
+		DevBlock blk;
+		InstParts q = {};
+		rc = carve(s->device, blk, [&](Carve &c) { q = take_insts(c, cap, true); });
+		if (rc) return rc;
+		old = s->insts;
+		s->insts = blk;
+		s->ip = q;
+		s->inst_cap = cap;
+	}
+
+	/* commit */
+	if (n) {
+		CU(cudaMemcpyAsync(s->ip.last, t.last, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(s->ip.keys, t.keys, n, cudaMemcpyDeviceToDevice, st));
+	}
+	s->dev.instances = s->ip.recs;
+	s->dev.inst_key = s->ip.keys;
+	s->dev.instance_count = n;
+	s->top_off = top_off;
+	s->top_cap = top_cap;
+	rc = commit_top(s, n, t, res);
+	if (rc) return rc;
+	ctx_free(s->device, old.p, old.bytes);                   /* the descriptor no longer points at it */
+	EditRecord &r = s->rec;
+	r.inst_kind.resize(n);
+	r.inst_object.resize(n);
+	for (uint32_t i = 0; i < n; ++i) { r.inst_kind[i] = inst[i].kind; r.inst_object[i] = inst[i].object; }
+	r.last = pk.last;
+	return CRGPU_OK;
 }
 
 /* ---- mesh edits ---------------------------------------------------------------------------------------------------------------------
@@ -1723,7 +1871,7 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 			e.pairs = c.take<PairNode>(region_pairs(e.n)); e.prims = c.take<int32_t>(e.n);
 			e.tris = c.take<PackedTri>(e.n); e.slot = c.take<uint32_t>(e.n); e.keys = c.take<uint8_t>(e.n); e.spolys = c.take<ShadePoly>(e.n);
 		}
-		t = take_top(c, s);
+		t = take_top(c, s, ninst);
 		build = c.take<uint8_t>(crg_bvh_scratch_bytes(nmax));
 	});
 	if (rc) return rc;
@@ -1752,11 +1900,12 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	if (ninst) {
 		CU(cudaMemcpyAsync(t.roots, roots.data(), roots.size() * sizeof(float), cudaMemcpyHostToDevice, st));
 		rc = alloc_insts(s);
-		if (!rc) rc = build_top(s, nullptr, t, build, &top);
+		if (!rc) rc = build_top(s, ninst, s->dev.instances, nullptr, t, build, &top);
 		if (rc) return rc;
 	}
-	/* the first geometry edit reserves the top region behind the uploaded pairs, and the first edit of a mesh its own region */
-	const uint32_t first = s->pairs.p ? s->pair_cap : s->pair_count + region_pairs(ninst);
+	/* the first geometry edit reserves the top region behind the uploaded pairs, and the first edit of a mesh its own region behind
+	 * every pair of the block */
+	const uint32_t first = s->pairs.p ? s->pair_cap : s->top_off + s->top_cap;
 	uint32_t add = 0;
 	for (const MeshEdit &e : edits) if (s->mesh_region[e.mesh] == 0xffffffffu) add += region_pairs(e.n);
 	if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "set_meshes: more pair nodes than the scene can address");
@@ -1784,7 +1933,7 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, e.pairs, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	}
 	s->rec.bvh_root = roots;
-	if (ninst) return commit_top(s, t, top);
+	if (ninst) return commit_top(s, ninst, t, top);
 	return publish(s);
 }
 

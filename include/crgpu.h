@@ -171,13 +171,26 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  * never touch the framebuffer (clear it before rendering the edited frame) and leave the scene unchanged when they fail.
  *   crgpu_scene_set_camera     copies every field of `cam` bit for bit; its width and height must be the scene's image size.
  *   crgpu_scene_set_instances  takes A and Ainv of each instance bit for bit (Ainv is not recomputed); `count`, and each instance's
- *                              kind and object, must be those uploaded (instances cannot be added or removed).  The instance
- *                              boxes, ray offsets and the top-level BVH are rebuilt on the device, the tree that the scene loader
- *                              builds.  The first instance or mesh edit gives the scene its own copy of the BVH pair nodes (the
- *                              uploaded pairs plus room for any top level of `count` instances) and its own top-level item records;
- *                              later edits reuse them.  A top level that needs more than count - 1 pair nodes (a tree of more than
- *                              2 count - 1 nodes, which only instances whose boxes no split separates make: see crloader_build_bvh
- *                              in crloader.h) is refused with CRGPU_ERR_UNSUPPORTED.
+ *                              kind and object, must be those of the scene's current list (crgpu_scene_set_instance_list changes
+ *                              them).  The instance boxes, ray offsets and the top-level BVH are rebuilt on the device, the tree that
+ *                              the scene loader builds.  The first instance or mesh edit gives the scene its own copy of the BVH pair
+ *                              nodes (the uploaded pairs plus room for any top level of `count` instances) and its own top-level item
+ *                              records; later edits reuse them.  A top level that needs more than count - 1 pair nodes (a tree of more
+ *                              than 2 count - 1 nodes, which only instances whose boxes no split separates make: see
+ *                              crloader_build_bvh in crloader.h) or is deeper than 64 levels is refused with CRGPU_ERR_UNSUPPORTED.
+ *   crgpu_scene_set_instance_list  replaces the whole instance list: instance i of `inst` becomes instance i of the scene, `count`
+ *                              from 0 to 4,194,304 (the device builder's limit; above it CRGPU_ERR_UNSUPPORTED before any instance is
+ *                              read).  Each instance is a CRS_INST_SPHERE or CRS_INST_MESH of an uploaded sphere or mesh, also one
+ *                              that had no instance; no object is created.  A sphere instance takes its sphere's uploaded radius and
+ *                              material, a mesh instance its mesh's current BVH (crgpu_scene_set_meshes included), and every object
+ *                              the ray offset of its last instance, as the scene loader gives them.  A and Ainv are taken bit for bit.
+ *                              A NULL `inst` with count > 0, another kind or an object out of range is refused with
+ *                              CRGPU_ERR_BAD_ARGUMENT; a top level of more than 2 count - 1 nodes or deeper than 64 levels with
+ *                              CRGPU_ERR_UNSUPPORTED.  With count 0 every ray misses.  The instance records, instance keys,
+ *                              last-instance table and item records then live in an instance block that only grows (the upload's
+ *                              instance sections stay allocated, unread); a top level that no longer fits the top region gets a
+ *                              larger region at the end of the pairs block, and mesh regions never move.  Later calls of
+ *                              crgpu_scene_set_instances and crgpu_scene_set_meshes work on the new list.
  *   crgpu_scene_set_meshes     deforms meshes (crTransformMesh, "recompute kd-tree"): every mesh listed in `meshes` takes its polys,
  *                              flat->polys[poly_offset .. + poly_count), and the vertices, normals and texture coordinates they
  *                              index from `flat`; positions, normals, uvs and each poly's material (within the mesh's material
@@ -211,6 +224,7 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  * unedited. */
 int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam);
 int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
+int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
 int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count);
 int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat);
 int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,
