@@ -113,6 +113,7 @@ def lib():
         L.crgpu_trace_rays.argtypes = [P, P, C.c_uint32, C.POINTER(TraceOpts), P, P, C.POINTER(C.c_uint32), C.POINTER(Stats)]
         L.crgpu_shade_rays.argtypes = [P, P, C.c_uint32, C.POINTER(ShadeOpts), P, P, C.POINTER(C.c_uint32), P]
         L.crgpu_libm_eval.argtypes = [C.c_int, C.c_int, P, P, P, C.c_uint32]
+        L.crgpu_path_order_map.argtypes = [C.c_int, C.c_uint32, C.c_uint32, P, P, P, C.c_uint32, C.c_uint32, P]
         L.crgpu_prepared_background.argtypes = [P, C.POINTER(C.c_uint32)]
         L.crgpu_scene_create_prepared.argtypes = [P, C.c_int, C.POINTER(P)]
         L.crgpu_scene_info.argtypes = [P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
@@ -129,7 +130,7 @@ def lib():
         for f in ("crgpu_device_count", "crgpu_scene_create", "crgpu_scene_destroy", "crgpu_set_max_paths_in_flight",
                   "crgpu_render_tile", "crgpu_render_tiles", "crgpu_set_stream", "crgpu_use_own_stream", "crgpu_get_stats", "crgpu_framebuffer_clear", "crgpu_framebuffer_read", "crgpu_framebuffer_write",
                   "crgpu_framebuffer_to_srgb8", "crgpu_framebuffer_device_ptr", "crgpu_trace_kat", "crgpu_trace_rays", "crscene_load",
-                  "crgpu_shade_rays", "crgpu_libm_eval", "crgpu_prepared_background",
+                  "crgpu_shade_rays", "crgpu_libm_eval", "crgpu_path_order_map", "crgpu_prepared_background",
                   "crgpu_scene_create_prepared", "crgpu_scene_info", "crgpu_device_trim",
                   "crgpu_stop_enable", "crgpu_request_stop", "crgpu_clear_stop", "crgpu_progress",
 

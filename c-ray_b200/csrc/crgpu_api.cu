@@ -1313,6 +1313,7 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 		const WaveBuffers &wb = set ? s->wb2 : s->wb;
 		TileDesc td = base;
 		td.npix = (unsigned)tile_pixels;
+		td.order = crg_path_order();
 		td.pass_begin = pb;
 		td.pass_count = (pass_begin + pass_count - pb) < (int)batch ? (pass_begin + pass_count - pb) : (int)batch;
 		if (timing) times.mark(times.k1, st);
@@ -2052,7 +2053,8 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 		CU(cudaMemcpyAsync(tab, rects, (size_t)nrects * 16u, cudaMemcpyHostToDevice, s->stream));
 		CU(cudaMemcpyAsync(tab + (size_t)nrects * 16u, offs.data(), (size_t)nrects * 4u, cudaMemcpyHostToDevice, s->stream));
 		CU(cudaStreamSynchronize(s->stream));           /* offs is a local; costs ~20 us, once per tile set */
-		crg_launch_pixel_list(s->pixels, reinterpret_cast<const int4 *>(tab), reinterpret_cast<const unsigned *>(tab + (size_t)nrects * 16u), nrects, s->stream);
+		crg_launch_pixel_list(s->pixels, reinterpret_cast<const int4 *>(tab), reinterpret_cast<const unsigned *>(tab + (size_t)nrects * 16u), nrects,
+		                      crg_path_order().blocked, s->stream);
 		CU(cudaGetLastError());
 		s->pixel_key.swap(key);
 	}
@@ -2356,6 +2358,28 @@ extern "C" int crgpu_shade_rays(crgpu_scene *s, const struct crgpu_path_state *s
 	*survivors_out = surv;
 	if (box_out) memcpy(box_out, box, sizeof box);
 	return crgpu_get_stats(s, nullptr);
+}
+
+extern "C" int crgpu_path_order_map(int order, uint32_t npix, uint32_t pass_count, uint32_t *pass_out, uint32_t *pixel_out, uint32_t *id_out,
+                                    uint32_t w, uint32_t h, uint32_t *xy_out) {
+	if (order < 0 || order >= CRG_PATH_ORDERS || (uint64_t)npix * pass_count > 0xffffffffull || (uint64_t)w * h > 0xffffffffull || w > 65535u || h > 65535u)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "bad argument");
+	const PathOrder o = crg_path_order_of(order);
+	const uint32_t n = npix * pass_count;
+	for (uint32_t id = 0; id < n; ++id) {
+		unsigned pl, px;
+		crg_path_pass_pixel(id, npix, pass_count, o.p, o.q, pl, px);
+		if (pass_out) pass_out[id] = pl;
+		if (pixel_out) pixel_out[id] = px;
+		if (id_out) id_out[id] = crg_path_id(id / npix, id % npix, npix, pass_count, o.p, o.q);
+	}
+	const uint32_t m = w * h;
+	for (uint32_t i = 0; xy_out && i < m; ++i) {
+		unsigned x = i % w, y = i / w;
+		if (o.blocked) crg_block_xy(i, w, h, x, y);
+		xy_out[i] = x | y << 16;
+	}
+	return CRGPU_OK;
 }
 
 extern "C" int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *out, uint32_t n) {

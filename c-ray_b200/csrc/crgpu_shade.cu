@@ -332,18 +332,29 @@ __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, cons
 													 const unsigned *__restrict__ snap_host) {
 	if (ARMED && snap_host && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = crg_ld_sys(snap_host + 3) == 1u ? 1u : 0u;
 	if (ARMED && (gate[1 + set] != 0u || gate[0] != (unsigned)td.pass_begin)) return;
-	const unsigned tile_pixels = td.npix;
+	const unsigned tile_pixels = td.npix, npass = (unsigned)td.pass_count, P = td.order.p, Q = td.order.q, h = tile_pixels / Q;
 	for (unsigned px = blockIdx.x * blockDim.x + threadIdx.x; px < tile_pixels; px += gridDim.x * blockDim.x) {
 		int x, y;
 		crg_pixel_xy(td, px, x, y);
 		float *dst = fb + ((size_t)x + (size_t)(image_height - (y + 1)) * (size_t)image_width) * 3u;  /* texture.c:24-28 */
 		float r = dst[0], g = dst[1], b = dst[2];
-		for (int pl = 0; pl < td.pass_count; ++pl) {
-			const float4 s = L[(size_t)pl * tile_pixels + px];
-			const int completed = td.pass_begin + pl + 1;                                     /* renderer.c:288-291 */
-			const float k = (float)(completed - 1);
-			const float t = cr_div(1.0f, (float)completed);
-			r = (r * k + s.x) * t; g = (g * k + s.y) * t; b = (b * k + s.z) * t;
+		/* the pixel's passes in pass order (crg_path_pass_pixel): within a pass group its paths are `step` apart, and the whole groups
+		 * start P * tile_pixels apart, so only the first group and a last, shorter one need the map.  With P = 1 this is the
+		 * pass-major walk L[pass * tile_pixels + px]; with Q = 4 the quarter-warps of a block read 64 contiguous bytes per pass. */
+		const unsigned step = px < Q * h ? Q : tile_pixels - Q * h;
+		unsigned c0 = 0u, pc = P <= npass ? P : npass, id = crg_path_id(0u, px, tile_pixels, npass, P, Q);
+		while (true) {
+			for (unsigned j = 0u; j < pc; ++j) {
+				const float4 s = L[id + j * step];
+				const int completed = td.pass_begin + (int)(c0 + j) + 1;                      /* renderer.c:288-291 */
+				const float k = (float)(completed - 1);
+				const float t = cr_div(1.0f, (float)completed);
+				r = (r * k + s.x) * t; g = (g * k + s.y) * t; b = (b * k + s.z) * t;
+			}
+			c0 += pc;
+			if (c0 >= npass) break;
+			if (npass - c0 >= P) id += P * tile_pixels;                                     /* the next group is whole */
+			else { pc = npass - c0; id = crg_path_id(c0, px, tile_pixels, npass, P, Q); }
 		}
 		dst[0] = r; dst[1] = g; dst[2] = b;
 	}

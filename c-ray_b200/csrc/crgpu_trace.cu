@@ -8,21 +8,37 @@
 #include "crgpu_trace.cuh"
 #include <cstdlib>
 
-/* ---- pixel list of a tile set: blockIdx.y = tile, the block's threads walk its pixels row by row (crgpu_render_tiles) ---------------- */
-__global__ void __launch_bounds__(256) k_pixel_list(uint32_t *__restrict__ pixels, const int4 *__restrict__ rects, const unsigned *__restrict__ offs) {
+/* ---- pixel list of a tile set: blockIdx.y = tile, the block's threads walk its pixels row by row, or in 8x4 blocks (blocked,
+ *      crg_block_xy) (crgpu_render_tiles) ------------------------------------------------------------------------------------------- */
+__global__ void __launch_bounds__(256) k_pixel_list(uint32_t *__restrict__ pixels, const int4 *__restrict__ rects, const unsigned *__restrict__ offs, int blocked) {
 	const int4 r = rects[blockIdx.y];
-	const unsigned w = (unsigned)(r.z - r.x), n = w * (unsigned)(r.w - r.y);
+	const unsigned w = (unsigned)(r.z - r.x), h = (unsigned)(r.w - r.y), n = w * h;
 	uint32_t *out = pixels + offs[blockIdx.y];
 	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-		const unsigned y = i / w, x = i - y * w;
+		unsigned x, y;
+		if (blocked) crg_block_xy(i, w, h, x, y);
+		else { y = i / w; x = i - y * w; }
 		out[i] = (uint32_t)(r.x + (int)x) | ((uint32_t)(r.y + (int)y) << 16);
 	}
 }
-void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, cudaStream_t st) {
+void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, int blocked, cudaStream_t st) {
 	for (int first = 0; first < nrects; first += 32768) {            /* gridDim.y <= 65535 */
 		const int cnt = nrects - first < 32768 ? nrects - first : 32768;
-		k_pixel_list<<<dim3(4, (unsigned)cnt), 256, 0, st>>>(pixels, rects + first, offs + first);
+		k_pixel_list<<<dim3(4, (unsigned)cnt), 256, 0, st>>>(pixels, rects + first, offs + first, blocked);
 	}
+}
+
+/* CRGPU_PATH_ORDER (crg_path_order_of), read once per process; any value outside 0 .. CRG_PATH_ORDERS - 1 selects the default.
+ * 6 (16 passes of a 2x1 pixel pair per warp): on hdr.json (1080p, 1000 spp, one H100 80GB HBM3 at 700 W) bench.py measures
+ * 4696-4698 Mray/s against 4680-4683 in order 2 and 4534-4578 in order 0's build before the knob (DESIGN §4) */
+#define CRG_PATH_ORDER_DEFAULT 6
+const PathOrder &crg_path_order(void) {
+	static const PathOrder o = [] {
+		const char *e = getenv("CRGPU_PATH_ORDER");
+		const int v = e ? atoi(e) : CRG_PATH_ORDER_DEFAULT;
+		return crg_path_order_of(v >= 0 && v < CRG_PATH_ORDERS ? v : CRG_PATH_ORDER_DEFAULT);
+	}();
+	return o;
 }
 
 /* ---- K1 ------------------------------------------------------------------------------------------------------------ */
@@ -30,7 +46,8 @@ __global__ void __launch_bounds__(256) k_generate(DevScene sc, WaveBuffers wb, T
 	const unsigned tile_pixels = td.npix;
 	const unsigned n = tile_pixels * (unsigned)td.pass_count;
 	for (unsigned id = blockIdx.x * blockDim.x + threadIdx.x; id < n; id += gridDim.x * blockDim.x) {
-		const unsigned pl = id / tile_pixels, px = id - pl * tile_pixels;
+		unsigned pl, px;
+		crg_path_pass_pixel(id, tile_pixels, (unsigned)td.pass_count, td.order.p, td.order.q, pl, px);
 		int x, y;
 		crg_pixel_xy(td, px, x, y);
 		const uint32_t pixIdx = (uint32_t)(y * (int)sc.image_width + x);                        /* renderer.c:280 */

@@ -2,7 +2,8 @@
  * crgpu_wave.cuh — wavefront buffers and kernel launchers shared by the translation units of libcrgpu.so.
  *
  * One `crgpu_render_tile` call processes a tile rectangle in batches of B passes; a batch has
- * N = tile_pixels * B paths, path id = p_local * tile_pixels + pixel_local.  Per batch:
+ * N = tile_pixels * B paths, numbered by the path order (crg_path_pass_pixel below; pass-major, id = p_local * tile_pixels +
+ * pixel_local, with CRGPU_PATH_ORDER=0).  Per batch:
  *
  *   K1 k_generate    initSampler + getCameraRay for every path            (sampler.c:41-44, camera.c:58-87)
  *   per bounce:
@@ -62,15 +63,78 @@ __device__ __forceinline__ unsigned crg_ld_sys(const unsigned *p) {
 }
 __device__ __forceinline__ void crg_st_sys(unsigned *p, unsigned v) { asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
+/* ---- path order (CRGPU_PATH_ORDER, crg_path_order) ---------------------------------------------------------------------------
+ * K2 hands rays to its lanes in path-id order at bounce 0, and K3's compaction keeps that order within a material bucket for the
+ * bounces after, so the order in which a batch numbers its (pass, pixel) pairs decides which rays share a warp.  Two choices:
+ *   blocked  the pixels of a rectangle (a tile of a tile list, or the rectangle of crgpu_render_tile) are numbered in 8x4 blocks,
+ *            Morton order inside a block (crg_block_xy), instead of row by row;
+ *   P, Q     the passes are taken in groups of P, and inside a group the paths run over Q consecutive pixels for each of the
+ *            group's passes before the next Q pixels (crg_path_pass_pixel).  P = 1 is pass-major order.
+ * With blocked pixels and P * Q = 32, the 32 lanes a warp refills at bounce 0 trace P passes of one 2D block of Q pixels. */
+struct PathOrder { unsigned p, q; int blocked; };
+/* the values of CRGPU_PATH_ORDER: 0 = pass-major over row-by-row pixels (the order before the knob existed); 1 = pass-major over
+ * 8x4 pixel blocks; 2, 3, 4 = 8, 4, 2 passes of one 2x2, 4x2, 4x4 pixel block per 32 paths; 5 = 8 passes of a 4x1 strip of
+ * row-by-row pixels; 6 = 16 passes of a 2x1 pair of blocked pixels; 7 = 32 passes of one pixel (pixels in blocked order) */
+#define CRG_PATH_ORDERS 8
+inline PathOrder crg_path_order_of(int v) {
+	static const PathOrder t[CRG_PATH_ORDERS] = { { 1u, 32u, 0 }, { 1u, 32u, 1 }, { 8u, 4u, 1 }, { 4u, 8u, 1 }, { 2u, 16u, 1 }, { 8u, 4u, 0 },
+	                                              { 16u, 2u, 1 }, { 32u, 1u, 1 } };
+	return t[v];
+}
+const PathOrder &crg_path_order(void);     /* the frame path's order, CRGPU_PATH_ORDER (crgpu_trace.cu) */
+
+/* pixel i of a w x h rectangle in blocked order: the whole 8x4 blocks row of blocks by row of blocks, Morton order inside a block
+ * (bits x0 y0 x1 y1 x2: 4, 8, 16 and 32 aligned consecutive pixels are 2x2, 4x2, 4x4 and 8x4 squares), then the pixels right of
+ * the whole blocks row by row, then the rows below them.  A bijection of [0, w*h) for every w, h >= 1. */
+__host__ __device__ __forceinline__ void crg_block_xy(unsigned i, unsigned w, unsigned h, unsigned &x, unsigned &y) {
+	const unsigned bw = w >> 3, bh = h >> 2, inner = bw * bh * 32u;
+	if (i < inner) {
+		const unsigned b = i >> 5, m = i & 31u, by = b / bw, bx = b - by * bw;
+		x = (bx << 3) | (m & 1u) | ((m >> 1) & 2u) | ((m >> 2) & 4u);
+		y = (by << 2) | ((m >> 1) & 1u) | ((m >> 2) & 2u);
+		return;
+	}
+	const unsigned r = i - inner, rw = w - (bw << 3), right = rw * (bh << 2);
+	if (r < right) { y = r / rw; x = (bw << 3) + (r - y * rw); return; }
+	const unsigned r2 = r - right;
+	y = (bh << 2) + r2 / w; x = r2 - (y - (bh << 2)) * w;
+}
+
+/* the path order of a batch of npix pixels and pass_count passes (P = o.p, Q = o.q): pass group c holds passes [cP, cP + Pc),
+ * Pc = min(P, pass_count - cP), and paths [cP * npix, (cP + Pc) * npix); inside it the whole blocks of Q pixels come first, each
+ * as Pc runs of Q paths (one run per pass), then the last npix mod Q pixels as Pc runs of that many.  A bijection of
+ * [0, npix * pass_count) onto (pass_local, pixel_local) for every npix, pass_count >= 1 (checked on the host through crgpu_path_order_map). */
+__host__ __device__ __forceinline__ void crg_path_pass_pixel(unsigned id, unsigned npix, unsigned pass_count, unsigned P, unsigned Q,
+                                                            unsigned &pl, unsigned &px) {
+	const unsigned c0 = (id / npix) / P * P;                                  /* = floor(id / (P npix)) * P without the product */
+	const unsigned pc = pass_count - c0 < P ? pass_count - c0 : P;
+	const unsigned r = id - c0 * npix, h = npix / Q, full = pc * Q * h;
+	if (r < full) {
+		const unsigned run = pc * Q, b = r / run, k = r - b * run, j = k / Q;
+		pl = c0 + j; px = b * Q + (k - j * Q);
+	} else {
+		const unsigned s = npix - Q * h, r2 = r - full, j = r2 / s;
+		pl = c0 + j; px = Q * h + (r2 - j * s);
+	}
+}
+/* the inverse: the path id of (pass_local, pixel_local) */
+__host__ __device__ __forceinline__ unsigned crg_path_id(unsigned pl, unsigned px, unsigned npix, unsigned pass_count, unsigned P, unsigned Q) {
+	const unsigned c0 = pl / P * P, pc = pass_count - c0 < P ? pass_count - c0 : P, j = pl - c0, h = npix / Q;
+	if (px < Q * h) { const unsigned b = px / Q; return c0 * npix + b * pc * Q + j * Q + (px - b * Q); }
+	return c0 * npix + pc * Q * h + j * (npix - Q * h) + (px - Q * h);
+}
+
 struct TileDesc {
 	int x0, y0, tw, th;     /* tile origin and size (pixels); y up */
 	int pass_begin, pass_count; /* this batch */
 	const uint32_t *pixels; /* NULL: the pixel set is the rectangle above; else an explicit list x | y << 16 (a union of tiles) */
 	unsigned npix;          /* number of pixels in the set */
+	PathOrder order;        /* how the batch numbers its paths (set by render_batches) */
 };
 
 __device__ __forceinline__ void crg_pixel_xy(const TileDesc &td, unsigned px, int &x, int &y) {
 	if (td.pixels) { const uint32_t p = __ldg(td.pixels + px); x = (int)(p & 0xffffu); y = (int)(p >> 16); }
+	else if (td.order.blocked) { unsigned bx, by; crg_block_xy(px, (unsigned)td.tw, (unsigned)td.th, bx, by); x = td.x0 + (int)bx; y = td.y0 + (int)by; }
 	else { x = td.x0 + (int)(px % (unsigned)td.tw); y = td.y0 + (int)(px / (unsigned)td.tw); }
 }
 
@@ -86,7 +150,7 @@ struct TraceKnobs { int minb, defer, refill, burst, inst_min; };
 const TraceKnobs &crg_trace_knobs_env(void);
 
 /* launchers (defined in crgpu_trace.cu / crgpu_shade.cu); `dsc` is the device copy of `sc` */
-void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, cudaStream_t st);
+void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, int blocked, cudaStream_t st);
 void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st);
 void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, const TraceKnobs &kn, cudaStream_t st);
 /* per-ray records of K2's write-back (crgpu_trace_rays): t, u, v, instance, poly (-1 for spheres and misses), key */

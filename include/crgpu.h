@@ -325,6 +325,13 @@ enum { CRGPU_LIBM_SIN, CRGPU_LIBM_COS, CRGPU_LIBM_TAN, CRGPU_LIBM_LOG, CRGPU_LIB
        CRGPU_LIBM_ASIN, CRGPU_LIBM_POW, CRGPU_LIBM_POW5, CRGPU_LIBM_SINCOS_SIN, CRGPU_LIBM_SINCOS_COS, CRGPU_LIBM_COUNT };
 int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *out, uint32_t n);
 
+/* The path order of the frame path (CRGPU_PATH_ORDER, c-ray_b200/csrc/crgpu_wave.cuh), evaluated on the host for order `order`
+ * (0..7): for a batch of npix pixels and pass_count passes, pass_out[id] and pixel_out[id] are the pass and pixel (local to the
+ * batch) that path id renders, id_out[pass * npix + pixel] is the path id of that pair (any of the three may be NULL); and, when
+ * w and h are not 0, xy_out[i] = x | y << 16 is pixel i of a w x h rectangle in that order's pixel order.  Needs no device. */
+int crgpu_path_order_map(int order, uint32_t npix, uint32_t pass_count, uint32_t *pass_out, uint32_t *pixel_out, uint32_t *id_out,
+                         uint32_t w, uint32_t h, uint32_t *xy_out);
+
 /* SURVEY §8(f1): the reference's binned-SAH BVH build (reference src/accelerators/bvh.c:96-296: partitionPrimitives,
  * buildBvhRecursive, buildBvhGeneric) on device `device`, level-synchronous (c-ray_b200/csrc/crgpu_bvh_build.cu).  Produces the
  * SAME tree as the reference and as the host builder (crloader_build_bvh): node order, leaf ranges, primitive order, bounds.

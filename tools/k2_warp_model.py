@@ -17,6 +17,9 @@ GPU time is scarce (180 min a round); this tool screens scheduling policies befo
      launch of hdr.json).
 
 usage: tools/k2_warp_model.py [scene=hdr] [W H x0 y0 x1 y1 passes]     (defaults: hdr 1920x1080, a 512x64 strip, 2 passes)
+       tools/k2_warp_model.py --orders [scene=hdr] [W H x0 y0 x1 y1 passes]
+                                      the path orders of CRGPU_PATH_ORDER (crgpu_wave.cuh) over the region as ONE batch's pixel set
+                                      (defaults: hdr 1920x1080, the 64x64 tile at (896, 512), 8 passes)
 """
 import ctypes as C
 import os
@@ -33,7 +36,7 @@ import oracle_lib as O                                                    # noqa
 W_NODE, W_TRI, W_INST, W_REFILL, W_WRITEBACK, W_LOOP = 70, 48, 95, 45, 30, 14
 
 
-def load_traces(scene, W, H, x0, y0, x1, y1, passes):
+def load_traces(scene, W, H, x0, y0, x1, y1, passes, with_keys=False):
     L = O.lib()
     L.cro_trace_region.restype = C.c_size_t
     L.cro_trace_region.argtypes = [C.POINTER(O.Scene)] + [C.c_int] * 6 + [C.c_void_p, C.c_size_t]
@@ -52,12 +55,13 @@ def load_traces(scene, W, H, x0, y0, x1, y1, passes):
         ev = raw[pos + 36:pos + 36 + cnt]
         rays[int(d)].append(((int(p), int(y), int(x)), ev, od))
         pos += 36 + cnt
-    out, geo = {}, {}
+    out, geo, keys = {}, {}, {}
     for d, lst in rays.items():
         lst.sort(key=lambda t: t[0])
         out[d] = [e for _, e, _ in lst]
         geo[d] = np.array([g for _, _, g in lst], dtype=np.float32).reshape(-1, 6)
-    return out, geo
+        keys[d] = [k for k, _, _ in lst]                          # (pass, y, x) of each ray's path
+    return (out, geo, keys) if with_keys else (out, geo)
 
 
 class Ray:
@@ -227,8 +231,45 @@ def first_cell_key(ev):
     return (min(first, 255), int(np.log2(len(ev) + 1)))
 
 
+ORDER_NAMES = {0: "pass-major, row strips (32x1 per warp)", 1: "pass-major, 8x4 Morton blocks", 2: "8 passes x 2x2 block",
+               3: "4 passes x 4x2 block", 4: "2 passes x 4x4 block", 5: "8 passes x 4x1 strip"}
+
+
+def path_ids(keys, x0, y0, w, h, passes, order):
+    """path id of every (pass, y, x) of the region rendered as one batch (pixel set = the w x h rectangle) in path order `order`,
+    from the library's own map (crgpu_path_order_map)"""
+    import crgpu
+    npix = w * h
+    xy = np.zeros(npix, dtype=np.uint32)
+    inv = np.zeros(npix * passes, dtype=np.uint32)
+    assert crgpu.lib().crgpu_path_order_map(order, npix, passes, None, None, inv.ctypes.data, w, h, xy.ctypes.data) == 0
+    local = np.empty(npix, dtype=np.int64)                        # (y - y0) * w + (x - x0) -> pixel index in the order
+    local[(xy >> 16).astype(np.int64) * w + (xy & 0xffff).astype(np.int64)] = np.arange(npix)
+    k = np.asarray(keys, dtype=np.int64).reshape(-1, 3)
+    return inv[k[:, 0] * npix + local[(k[:, 1] - y0) * w + (k[:, 2] - x0)]]
+
+
+def screen_orders(a):
+    scene = a[0] if a else "hdr"
+    W, H, x0, y0, x1, y1, passes = (int(v) for v in a[1:8]) if len(a) >= 8 else (1920, 1080, 896, 512, 960, 576, 8)
+    traces, geo, keys = load_traces(scene, W, H, x0, y0, x1, y1, passes, with_keys=True)
+    print(f"scene {scene} {W}x{H}, region x {x0}..{x1} y {y0}..{y1} as one batch of {passes} passes; rays per bounce:",
+          {d: len(v) for d, v in sorted(traces.items()) if d < 4})
+    print("K2 as built (phase-separated, burst 3, refill<16); bounce 1 keeps bounce 0's order for its survivors (K3's compaction),"
+          " without K4's material buckets")
+    for d in (0, 1):
+        for o, name in ORDER_NAMES.items():
+            ids = path_ids(keys[d], x0, y0, x1 - x0, y1 - y0, passes, o)
+            rays = [traces[d][i] for i in np.argsort(ids, kind="stable")]
+            act, ipr = simulate(rays, policy="phase", burst=3, refill=16)
+            print(f"  bounce {d}  order {o}  {name:42s} active lanes {act:5.1f}   instructions/ray {ipr:7.0f}", flush=True)
+
+
 def main():
     a = sys.argv[1:]
+    if a and a[0] == "--orders":
+        screen_orders(a[1:])
+        return
     scene = a[0] if a else "hdr"
     W, H, x0, y0, x1, y1, passes = (int(v) for v in a[1:8]) if len(a) >= 8 else (1920, 1080, 704, 500, 1216, 564, 2)
     traces, geo = load_traces(scene, W, H, x0, y0, x1, y1, passes)
