@@ -150,6 +150,16 @@ def lib():
             L.crgpu_scene_set_shading.argtypes = [P, C.POINTER(FlatScene)]
             L.crgpu_scene_shading.argtypes = [P, P, P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
             L.crgpu_scene_set_shading.restype = L.crgpu_scene_shading.restype = C.c_int
+        if hasattr(L, "crgpu_render_views"):      # absent from libraries built before views
+            L.crgpu_scene_set_views.argtypes = [P, P, C.c_uint32]
+            L.crgpu_scene_view_count.argtypes = [P, C.POINTER(C.c_uint32)]
+            L.crgpu_render_views.argtypes = [P, C.c_uint32, C.c_uint32, P, C.c_int, C.c_int, C.c_int, C.c_uint, C.POINTER(Stats)]
+            L.crgpu_view_clear.argtypes = [P, C.c_uint32]
+            L.crgpu_view_read.argtypes = [P, C.c_uint32, P]
+            L.crgpu_view_to_srgb8.argtypes = [P, C.c_uint32, P]
+            for f in ("crgpu_scene_set_views", "crgpu_scene_view_count", "crgpu_render_views", "crgpu_view_clear", "crgpu_view_read",
+                      "crgpu_view_to_srgb8"):
+                getattr(L, f).restype = C.c_int
         _lib = L
     return _lib
 
@@ -307,6 +317,43 @@ class GpuScene:
         kinds, flags = np.zeros(n.value, np.uint32), np.zeros(n.value, np.uint32)
         _check(lib().crgpu_scene_shading(self.handle, kinds.ctypes.data, flags.ctypes.data, n.value, None, None, None), "crgpu_scene_shading")
         return {"kinds": kinds, "flags": flags, "background_kind": bg.value, "complete_interpreter": bool(x.value)}
+
+    def set_views(self, cameras):
+        """Replace the view list (crgpu_scene_set_views): a sequence of Camera of the scene's image size, taken bit for bit; the first
+        becomes the scene camera.  Surviving views keep their framebuffers, new views start zeroed."""
+        arr = (Camera * len(cameras))(*cameras)
+        _check(lib().crgpu_scene_set_views(self.handle, arr, len(cameras)), "crgpu_scene_set_views")
+
+    def view_count(self):
+        n = C.c_uint32(0)
+        _check(lib().crgpu_scene_view_count(self.handle, C.byref(n)), "crgpu_scene_view_count")
+        return n.value
+
+    def render_views(self, rects, first=0, count=None, pass_begin=0, pass_count=None, flags=0):
+        """Render the tile set [(x0, y0, x1, y1), ...] in views [first, first + count) as ONE wavefront (crgpu_render_views); each
+        view ends as render_tiles would leave it under its own camera.  The result as for render_tile."""
+        st = Stats()
+        if count is None:
+            count = self.view_count() - first
+        if pass_count is None:
+            pass_count = self.samples - pass_begin
+        arr = np.ascontiguousarray(rects, dtype=np.int32).reshape(-1, 4)
+        rc = lib().crgpu_render_views(self.handle, first, count, arr.ctypes.data, len(arr), pass_begin, pass_count, flags, C.byref(st))
+        return self._render_result(rc, flags, st, "crgpu_render_views")
+
+    def view_read(self, view):
+        """float32 [H, W, 3] framebuffer of one view (the framebuffer layout, as read() gives view 0)."""
+        out = np.empty((self.H, self.W, 3), dtype=np.float32)
+        _check(lib().crgpu_view_read(self.handle, view, out.ctypes.data), "crgpu_view_read")
+        return out
+
+    def view_srgb8(self, view):
+        out = np.empty((self.H, self.W, 3), dtype=np.uint8)
+        _check(lib().crgpu_view_to_srgb8(self.handle, view, out.ctypes.data), "crgpu_view_to_srgb8")
+        return out
+
+    def view_clear(self, view):
+        _check(lib().crgpu_view_clear(self.handle, view), "crgpu_view_clear")
 
     def set_stream(self, cuda_stream_ptr):
         """Enqueue on a caller-owned cudaStream_t (int pointer, e.g. torch.cuda.current_stream().cuda_stream)."""

@@ -237,6 +237,11 @@ struct crgpu_scene {
 	DevBlock scratch;                /* a geometry edit's inputs, records and builder scratch; grows only, and nothing in it outlives a call */
 	DevBlock shade;                  /* NULL until the first shading edit: the node graph, texture table and texel data the kernels read in
 	                                    place of the slab's */
+	/* views (crgpu_scene_set_views): view 0 is the scene's camera and framebuffer; views 1 .. view_count - 1 live in the views block */
+	uint32_t view_count = 1;
+	uint32_t view_cap = 1;           /* views the block has room for (1: no block) */
+	DevBlock views;                  /* NULL until the first set_views of more than one view: view_cap - 1 cameras, then view_cap - 1
+	                                    framebuffers (views_layout); grows only */
 };
 
 /* K1 and K2 take the host descriptor s->dev by value; K3, the tail kernel and the KAT read its HBM copy s->dev_copy.  Writes the
@@ -748,7 +753,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->fb8, s->fb_floats);
 	ctx_free(s->device, s->snap8, s->fb_floats);
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
-	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade }) ctx_free(s->device, b->p, b->bytes);
+	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade, &s->views }) ctx_free(s->device, b->p, b->bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -1269,8 +1274,10 @@ static uint64_t enqueue_bounce(const crgpu_scene *s, const WaveBuffers &wb, int 
 	return launches;
 }
 
-/* The batch loop: passes [pass_begin, +pass_count) over one piece of at most max_paths pixels (pass_count > 0). */
-static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, const Gates &gates) {
+/* The batch loop: passes [pass_begin, +pass_count) over one piece of at most max_paths pixels (pass_count > 0).  vd: NULL, or the
+ * piece's views (a views call: K1 and K5 in their views instantiations). */
+static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, const Gates &gates,
+                          const ViewDesc *vd) {
 	const bool armed = s->armed;
 	const bool count = (flags & CRGPU_FLAG_COUNT) != 0;
 	const bool timing = (flags & CRGPU_FLAG_TIME_KERNELS) != 0;
@@ -1317,7 +1324,7 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 		td.pass_begin = pb;
 		td.pass_count = (pass_begin + pass_count - pb) < (int)batch ? (pass_begin + pass_count - pb) : (int)batch;
 		if (timing) times.mark(times.k1, st);
-		crg_launch_generate(s->dev, wb, td, grid, st); ++launches;
+		crg_launch_generate(s->dev, wb, td, vd, grid, st); ++launches;
 		if (timing) times.mark(times.k1, st);
 		/* bounces == 0: pathTrace's loop never runs and every sample is black (pathtrace.c:34-36,59).  L is write-once by
 		 * design (cr_add_radiance / cr_finish_path), so with no bounce nothing would write it: clear it here instead */
@@ -1333,7 +1340,7 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
 		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set,
-		                      armed && gates.publish ? s->stop_host : nullptr); ++launches;
+		                      armed && gates.publish ? s->stop_host : nullptr, vd); ++launches;
 		if (armed && gates.publish) {       /* stages a snapshot when K5 found one requested (crgpu_request_snapshot) */
 			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats,
 			                        s->fb, s->snap8, s->fb_floats, s->sm_count * 4, st);
@@ -1357,15 +1364,18 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 	return CRGPU_OK;
 }
 
-/* A pixel set cut into pieces of at most max_paths pixels: rows of the rectangle, or ranges of the list.  A set that fits is one piece. */
-struct Piece { TileDesc td; uint64_t pixels; };
-static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, std::vector<Piece> &pieces) {
+/* A pixel set cut into pieces of at most max_paths pixels: rows of the rectangle, or ranges of the list, or of a views call's view-major
+ * numbering (so a piece may hold several views, or part of one).  A set that fits is one piece. */
+struct Piece { TileDesc td; uint64_t pixels; ViewDesc vd; };
+static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, const ViewDesc *vd, std::vector<Piece> &pieces) {
 	const uint64_t most = s->max_paths;
-	if (tile_pixels <= most) { pieces.push_back({ base, tile_pixels }); return CRGPU_OK; }
+	const ViewDesc none = {};
+	if (tile_pixels <= most) { pieces.push_back({ base, tile_pixels, vd ? *vd : none }); return CRGPU_OK; }
 	if (base.pixels) {
 		for (uint64_t p0 = 0; p0 < tile_pixels; p0 += most) {
-			Piece p = { base, tile_pixels - p0 < most ? tile_pixels - p0 : most };
-			p.td.pixels = base.pixels + p0;
+			Piece p = { base, tile_pixels - p0 < most ? tile_pixels - p0 : most, vd ? *vd : none };
+			if (vd) p.vd.p0 = (unsigned)p0;
+			else p.td.pixels = base.pixels + p0;
 			pieces.push_back(p);
 		}
 		return CRGPU_OK;
@@ -1373,7 +1383,7 @@ static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t til
 	const uint64_t rows = most / (uint64_t)base.tw;
 	if (rows < 1) return fail(CRGPU_ERR_BAD_ARGUMENT, "tile is %d pixels wide > max paths in flight %llu", base.tw, (unsigned long long)most);
 	for (int y = 0; y < base.th; y += (int)rows) {
-		Piece p = { base, 0 };
+		Piece p = { base, 0, none };
 		p.td.y0 = base.y0 + y;
 		p.td.th = base.th - y < (int)rows ? base.th - y : (int)rows;
 		p.pixels = (uint64_t)p.td.tw * (uint64_t)p.td.th;
@@ -1387,8 +1397,10 @@ static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t til
  * commits in pass order or not at all (Gates, k_accumulate<true>, k_stop_publish), so the framebuffer then holds exactly passes
  * [0, committed) and a later call for [committed, end) finishes it bit for bit; several pieces are walked pass-major, each batch of
  * passes over every piece, so that one pass count describes the set.  Only the first piece of a pass batch takes a stop (the later
- * ones complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set. */
-static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats) {
+ * ones complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set.
+ * vd: NULL, or the views of a views call over its whole (view, pixel) set of tile_pixels pairs (crgpu_render_views). */
+static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats,
+                       const ViewDesc *vd = nullptr) {
 	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
 	const bool armed = s->armed;
@@ -1406,10 +1418,10 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 	}
 	std::vector<Piece> pieces;
 	int rc = CRGPU_OK;
-	if (pass_count > 0 && tile_pixels > 0) rc = split_pieces(s, base, tile_pixels, pieces);   /* an empty call renders nothing */
+	if (pass_count > 0 && tile_pixels > 0) rc = split_pieces(s, base, tile_pixels, vd, pieces);   /* an empty call renders nothing */
 	if (!armed || pieces.size() < 2) {
 		for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
-			rc = render_batches(s, pieces[k].td, pieces[k].pixels, pass_begin, pass_count, flags, { true, true, true, tile_pixels });
+			rc = render_batches(s, pieces[k].td, pieces[k].pixels, pass_begin, pass_count, flags, { true, true, true, tile_pixels }, vd ? &pieces[k].vd : nullptr);
 	} else {
 		uint64_t widest = 1;
 		for (const Piece &p : pieces) widest = p.pixels > widest ? p.pixels : widest;
@@ -1418,7 +1430,8 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 			if (stop_requested(s)) break;
 			const int n = pass_begin + pass_count - pb < passes ? pass_begin + pass_count - pb : passes;
 			for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
-				rc = render_batches(s, pieces[k].td, pieces[k].pixels, pb, n, flags, { k == 0, k + 1 == pieces.size(), false, tile_pixels });
+				rc = render_batches(s, pieces[k].td, pieces[k].pixels, pb, n, flags, { k == 0, k + 1 == pieces.size(), false, tile_pixels },
+				                    vd ? &pieces[k].vd : nullptr);
 		}
 	}
 	if (armed) {
@@ -2017,9 +2030,10 @@ extern "C" int crgpu_render_tile(crgpu_scene *s, int x0, int y0, int x1, int y1,
 	return render_call(s, td, (uint64_t)td.tw * (uint64_t)td.th, pass_begin, pass_count, flags, stats);
 }
 
-extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, int pass_begin, int pass_count,
-								  unsigned flags, struct crgpu_stats *stats) {
-	if (!s || !rects || nrects < 1) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad tile list");
+/* The device pixel list of a tile set (rects = 4 ints per tile), built on the device and kept for the next call with the same set.
+ * views: the view count of a views call, whose (view, pixel) pairs must number at most 2^32 - 1; 0 for crgpu_render_tiles. */
+static int tile_set(crgpu_scene *s, const int *rects, int nrects, uint64_t views, uint64_t *total_out) {
+	if (!rects || nrects < 1) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad tile list");
 	if (s->dev.image_width > 65535u || s->dev.image_height > 65535u) return fail(CRGPU_ERR_UNSUPPORTED, "tile lists need image dimensions <= 65535");
 	CU(cudaSetDevice(s->device));
 	uint64_t total = 0;
@@ -2028,6 +2042,10 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 		if (rc) return rc;
 		total += (uint64_t)(rects[4 * i + 2] - rects[4 * i]) * (uint64_t)(rects[4 * i + 3] - rects[4 * i + 1]);
 	}
+	if (views && total * views > 0xffffffffull)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "%llu views of %llu pixels are more than 2^32 - 1 (view, pixel) pairs", (unsigned long long)views,
+		            (unsigned long long)total);
+	*total_out = total;
 	std::vector<int> key(rects, rects + 4 * (size_t)nrects);
 	if (key != s->pixel_key) {                         /* rebuild the pixel list only when the tile set changes */
 		if (total > 0xffffffffull) return fail(CRGPU_ERR_UNSUPPORTED, "tile set of more than 2^32 pixels");
@@ -2058,10 +2076,136 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 		CU(cudaGetLastError());
 		s->pixel_key.swap(key);
 	}
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, int pass_begin, int pass_count,
+								  unsigned flags, struct crgpu_stats *stats) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "bad tile list");
+	uint64_t total = 0;
+	int rc = tile_set(s, rects, nrects, 0, &total);
+	if (rc) return rc;
 	TileDesc td;
 	memset(&td, 0, sizeof td);
 	td.pixels = s->pixels;
 	return render_call(s, td, total, pass_begin, pass_count, flags, stats);
+}
+
+/* ---- several views in one call ---------------------------------------------------------------------------------------------------
+ * The views block holds view_cap - 1 cameras, then view_cap - 1 framebuffers of fb_floats each (views 1 .. view_cap - 1). */
+static size_t views_cam_bytes(uint32_t cap) { return align256((size_t)(cap - 1u) * sizeof(DevCamera)); }
+static size_t views_bytes(uint32_t cap, size_t fb_floats) { return views_cam_bytes(cap) + (size_t)(cap - 1u) * fb_floats * sizeof(float); }
+static float *views_fb(const DevBlock &b, uint32_t cap) { return b.p ? reinterpret_cast<float *>(static_cast<uint8_t *>(b.p) + views_cam_bytes(cap)) : nullptr; }
+static float *view_fb(const crgpu_scene *s, uint32_t v) { return v ? views_fb(s->views, s->view_cap) + (size_t)(v - 1u) * s->fb_floats : s->fb; }
+
+extern "C" int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *cams, uint32_t count) {
+	if (!s || !cams) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (count < 1 || count > CRGPU_MAX_VIEWS) return fail(CRGPU_ERR_BAD_ARGUMENT, "%u views: the list holds 1 to %u", count, (unsigned)CRGPU_MAX_VIEWS);
+	for (uint32_t i = 0; i < count; ++i)
+		if (cams[i].width != (int32_t)s->dev.image_width || cams[i].height != (int32_t)s->dev.image_height)
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "camera %u is %dx%d, the scene renders %ux%u", i, cams[i].width, cams[i].height, s->dev.image_width,
+			            s->dev.image_height);
+	int rc = drain(s);
+	if (rc) return rc;
+	std::vector<DevCamera> dc(count - 1u);
+	for (uint32_t i = 1; i < count; ++i) dc[i - 1u] = dev_camera(cams[i]);
+	DevBlock blk = s->views;
+	uint32_t cap = s->view_cap;
+	if (count > cap) {                                   /* a larger block; the surviving views' framebuffers move into it */
+		cap = count;
+		blk.bytes = views_bytes(cap, s->fb_floats);
+		rc = ctx_alloc(s->device, blk.bytes, &blk.p);
+		if (rc) return rc;
+	}
+	const bool moved = blk.p != s->views.p;
+	const uint32_t keep = s->view_count < count ? s->view_count : count;     /* views 0 .. keep - 1 keep their pixels */
+	float *fbs = views_fb(blk, cap);
+	const size_t fb_bytes = s->fb_floats * sizeof(float);
+	cudaStream_t st = s->stream;
+	cudaError_t ce = cudaSuccess;
+	if (moved && keep > 1u) ce = cudaMemcpyAsync(fbs, views_fb(s->views, s->view_cap), (size_t)(keep - 1u) * fb_bytes, cudaMemcpyDeviceToDevice, st);
+	if (ce == cudaSuccess && count > keep) ce = cudaMemsetAsync(fbs + (size_t)(keep - 1u) * s->fb_floats, 0, (size_t)(count - keep) * fb_bytes, st);
+	if (ce == cudaSuccess && count > 1u) ce = cudaMemcpyAsync(blk.p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (ce != cudaSuccess) {
+		if (moved) ctx_free(s->device, blk.p, blk.bytes);
+		return fail(CRGPU_ERR_CUDA, "set_views: %s", cudaGetErrorString(ce));
+	}
+	/* commit */
+	if (moved) {
+		ctx_free(s->device, s->views.p, s->views.bytes);
+		s->views = blk;
+		s->view_cap = cap;
+	}
+	s->view_count = count;
+	s->dev.cam = dev_camera(cams[0]);
+	return publish(s);
+}
+
+extern "C" int crgpu_scene_view_count(crgpu_scene *s, uint32_t *count) {
+	if (!s || !count) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	*count = s->view_count;
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_render_views(crgpu_scene *s, uint32_t first_view, uint32_t view_count, const int *rects, int nrects, int pass_begin,
+                                  int pass_count, unsigned flags, struct crgpu_stats *stats) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	if (view_count < 1 || first_view >= s->view_count || view_count > s->view_count - first_view)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "views [%u,%llu) outside the list of %u", first_view, (unsigned long long)first_view + view_count, s->view_count);
+	uint64_t npix = 0;
+	int rc = tile_set(s, rects, nrects, view_count, &npix);
+	if (rc) return rc;
+	ViewDesc vd;
+	vd.cam0 = &s->dev_copy->cam;
+	vd.cams = static_cast<const DevCamera *>(s->views.p);
+	vd.fb = views_fb(s->views, s->view_cap);
+	vd.fb_floats = s->fb_floats;
+	vd.npix = (unsigned)npix;
+	vd.view0 = first_view;
+	vd.p0 = 0u;
+	TileDesc td;
+	memset(&td, 0, sizeof td);
+	td.pixels = s->pixels;
+	return render_call(s, td, npix * view_count, pass_begin, pass_count, flags, stats, &vd);
+}
+
+static int check_view(const crgpu_scene *s, uint32_t view) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	if (view >= s->view_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "view %u outside the list of %u", view, s->view_count);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_view_clear(crgpu_scene *s, uint32_t view) {
+	int rc = check_view(s, view);
+	if (rc) return rc;
+	CU(cudaSetDevice(s->device));
+	CU(cudaMemsetAsync(view_fb(s, view), 0, s->fb_floats * sizeof(float), s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_view_read(crgpu_scene *s, uint32_t view, float *host_rgb) {
+	int rc = check_view(s, view);
+	if (rc) return rc;
+	if (!host_rgb) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	CU(cudaSetDevice(s->device));
+	CU(cudaMemcpyAsync(host_rgb, view_fb(s, view), s->fb_floats * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_view_to_srgb8(crgpu_scene *s, uint32_t view, uint8_t *host_rgb8) {
+	int rc = check_view(s, view);
+	if (rc) return rc;
+	if (!host_rgb8) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	CU(cudaSetDevice(s->device));
+	if (!s->fb8) { void *q = nullptr; int arc = ctx_alloc(s->device, s->fb_floats, &q); if (arc) return arc; s->fb8 = static_cast<uint8_t *>(q); }
+	crg_launch_to_srgb8(view_fb(s, view), s->fb8, s->fb_floats, s->sm_count * 8, s->stream);
+	CU(cudaGetLastError());
+	CU(cudaMemcpyAsync(host_rgb8, s->fb8, s->fb_floats, cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
 }
 
 extern "C" int crgpu_get_stats(crgpu_scene *s, struct crgpu_stats *stats) {

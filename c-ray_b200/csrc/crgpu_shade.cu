@@ -325,18 +325,28 @@ __global__ void __launch_bounds__(128) k_tail(const DevScene *__restrict__ scp, 
  * its first pass — both written by earlier kernels in stream order, so every block takes the same decision.
  * snap_host (a batch that publishes): one thread reads the snapshot state once and tells the publish step that follows whether to
  * stage the image (gate[3]).  K5s run in pass order with a publish step between, so the state read here is what the previous
- * publish step left. */
-template <bool ARMED>
+ * publish step left.
+ * VIEWS (crgpu_render_views): px is a piece pixel of the view-major numbering (ViewDesc) and goes to its view's framebuffer with the
+ * same walk and arithmetic.  Armed, a views call stages no snapshot: block 0 clears gate[3] so that its publish steps stay one
+ * thread's work, and a request stays pending. */
+template <bool ARMED, bool VIEWS>
 __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, const float4 *__restrict__ L, TileDesc td,
 													 int image_width, int image_height, unsigned *__restrict__ gate, int set,
-													 const unsigned *__restrict__ snap_host) {
-	if (ARMED && snap_host && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = crg_ld_sys(snap_host + 3) == 1u ? 1u : 0u;
+													 const unsigned *__restrict__ snap_host, ViewDesc vd) {
+	if (ARMED && VIEWS && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = 0u;
+	else if (ARMED && snap_host && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = crg_ld_sys(snap_host + 3) == 1u ? 1u : 0u;
 	if (ARMED && (gate[1 + set] != 0u || gate[0] != (unsigned)td.pass_begin)) return;
 	const unsigned tile_pixels = td.npix, npass = (unsigned)td.pass_count, P = td.order.p, Q = td.order.q, h = tile_pixels / Q;
 	for (unsigned px = blockIdx.x * blockDim.x + threadIdx.x; px < tile_pixels; px += gridDim.x * blockDim.x) {
 		int x, y;
-		crg_pixel_xy(td, px, x, y);
-		float *dst = fb + ((size_t)x + (size_t)(image_height - (y + 1)) * (size_t)image_width) * 3u;  /* texture.c:24-28 */
+		float *img = fb;
+		if (VIEWS) {
+			unsigned v, tp;
+			crg_view_pixel(vd, px, v, tp);
+			crg_pixel_xy(td, tp, x, y);
+			if (v) img = vd.fb + (size_t)(v - 1u) * vd.fb_floats;
+		} else crg_pixel_xy(td, px, x, y);
+		float *dst = img + ((size_t)x + (size_t)(image_height - (y + 1)) * (size_t)image_width) * 3u;  /* texture.c:24-28 */
 		float r = dst[0], g = dst[1], b = dst[2];
 		/* the pixel's passes in pass order (crg_path_pass_pixel): within a pass group its paths are `step` apart, and the whole groups
 		 * start P * tile_pixels apart, so only the first group and a last, shorter one need the map.  With P = 1 this is the
@@ -515,9 +525,12 @@ void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigne
 	k_libm<<<256, 256, 0, st>>>(fn, x, y, out, n);
 }
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st, unsigned *gate, int set,
-                           const unsigned *snap_host) {
-	if (gate) k_accumulate<true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, snap_host);
-	else k_accumulate<false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr);
+                           const unsigned *snap_host, const ViewDesc *vd) {
+	if (vd) {
+		if (gate) k_accumulate<true, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, nullptr, *vd);
+		else k_accumulate<false, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr, *vd);
+	} else if (gate) k_accumulate<true, false><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, snap_host, ViewDesc{});
+	else k_accumulate<false, false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr, ViewDesc{});
 }
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st) {
 	k_to_srgb8<<<grid, 256, 0, st>>>(fb, out, n);

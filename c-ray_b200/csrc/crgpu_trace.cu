@@ -41,19 +41,25 @@ const PathOrder &crg_path_order(void) {
 	return o;
 }
 
-/* ---- K1 ------------------------------------------------------------------------------------------------------------ */
-__global__ void __launch_bounds__(256) k_generate(DevScene sc, WaveBuffers wb, TileDesc td) {
+/* ---- K1 ------------------------------------------------------------------------------------------------------------
+ * VIEWS (crgpu_render_views): px is a piece pixel of the view-major numbering (ViewDesc), and the ray is taken from its view's camera
+ * with the same arithmetic; vd is unused otherwise. */
+template <bool VIEWS>
+__global__ void __launch_bounds__(256) k_generate(DevScene sc, WaveBuffers wb, TileDesc td, ViewDesc vd) {
 	const unsigned tile_pixels = td.npix;
 	const unsigned n = tile_pixels * (unsigned)td.pass_count;
 	for (unsigned id = blockIdx.x * blockDim.x + threadIdx.x; id < n; id += gridDim.x * blockDim.x) {
 		unsigned pl, px;
 		crg_path_pass_pixel(id, tile_pixels, (unsigned)td.pass_count, td.order.p, td.order.q, pl, px);
 		int x, y;
-		crg_pixel_xy(td, px, x, y);
+		unsigned v = 0u;
+		if (VIEWS) { unsigned tp; crg_view_pixel(vd, px, v, tp); crg_pixel_xy(td, tp, x, y); }
+		else crg_pixel_xy(td, px, x, y);
 		const uint32_t pixIdx = (uint32_t)(y * (int)sc.image_width + x);                        /* renderer.c:280 */
 		uint64_t rng = cr_rng_init(pixIdx, (uint32_t)(td.pass_begin + (int)pl), sc.sample_count);
 		v3 o, d;
-		cr_camera_ray(sc.cam, x, y, rng, o, d);
+		if (VIEWS) cr_camera_ray(*(v ? vd.cams + (v - 1u) : vd.cam0), x, y, rng, o, d);
+		else cr_camera_ray(sc.cam, x, y, rng, o, d);
 		wb.stA[0][id] = make_float4(o.x, o.y, o.z, d.x);
 		wb.stB[0][id] = make_float4(d.y, d.z, 1.0f, 1.0f);
 		wb.stC[0][id] = make_uint4(__float_as_uint(1.0f), id, (unsigned)(rng & 0xffffffffull), (unsigned)(rng >> 32));
@@ -203,8 +209,9 @@ __global__ void __launch_bounds__(256, MINB) k_trace(DevScene sc, WaveBuffers wb
 	}
 }
 
-void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st) {
-	k_generate<<<grid, 256, 0, st>>>(sc, wb, td);
+void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, const ViewDesc *vd, int grid, cudaStream_t st) {
+	if (vd) k_generate<true><<<grid, 256, 0, st>>>(sc, wb, td, *vd);
+	else k_generate<false><<<grid, 256, 0, st>>>(sc, wb, td, ViewDesc{});
 }
 
 /* ---- stop gates of an armed scene (crgpu_wave.cuh): one thread each, but for a publish step that stages a snapshot ------------------

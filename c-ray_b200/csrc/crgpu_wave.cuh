@@ -138,6 +138,27 @@ __device__ __forceinline__ void crg_pixel_xy(const TileDesc &td, unsigned px, in
 	else { x = td.x0 + (int)(px % (unsigned)td.tw); y = td.y0 + (int)(px / (unsigned)td.tw); }
 }
 
+/* ---- several views in one call (crgpu_render_views) ---------------------------------------------------------------------------
+ * A views call numbers its (view, pixel) pairs view-major: call pixel g is view view0 + g / npix at pixel g mod npix of the tile
+ * set's pixel list (TileDesc::pixels, never a rectangle).  A piece is the range [p0, p0 + TileDesc::npix) of that numbering, and
+ * the path order maps a batch's ids onto (pass, piece pixel) exactly as for one view.  Only K1 (the camera) and K5 (the framebuffer)
+ * look at the view; they are launched in their <VIEWS = true> instantiations.  The camera of view 0 is the scene's (cam0: the HBM
+ * copy of DevScene::cam, which every edit publishes), its framebuffer the scene's. */
+struct ViewDesc {
+	const DevCamera *cam0;  /* view 0's camera */
+	const DevCamera *cams;  /* views 1..: view v's camera is cams[v - 1] */
+	float *fb;              /* views 1..: view v's framebuffer is fb + (v - 1) * fb_floats */
+	size_t fb_floats;
+	unsigned npix;          /* pixels of the tile set (per view) */
+	unsigned view0;         /* the call's first view */
+	unsigned p0;            /* the piece's first call pixel */
+};
+/* view and tile-set pixel of piece pixel px */
+__device__ __forceinline__ void crg_view_pixel(const ViewDesc &vd, unsigned px, unsigned &v, unsigned &tp) {
+	const unsigned g = vd.p0 + px, q = g / vd.npix;
+	v = vd.view0 + q; tp = g - q * vd.npix;
+}
+
 /* Launch variant of K2.  Every variant computes the same hit records; they differ in how a warp schedules its work.
  *   minb      blocks per SM the compiler makes room for: 2, 3 or 4 (the instrumented kernel, count = true, always uses 3)
  *   defer     0 = leaf triangles tested inside the node step, 1 = after the node burst by each lane, 2 = dealt over the warp
@@ -151,7 +172,8 @@ const TraceKnobs &crg_trace_knobs_env(void);
 
 /* launchers (defined in crgpu_trace.cu / crgpu_shade.cu); `dsc` is the device copy of `sc` */
 void crg_launch_pixel_list(uint32_t *pixels, const int4 *rects, const unsigned *offs, int nrects, int blocked, cudaStream_t st);
-void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, int grid, cudaStream_t st);
+/* vd: NULL, or the views of a views call (K1 <VIEWS = true>) */
+void crg_launch_generate(const DevScene &sc, const WaveBuffers &wb, const TileDesc &td, const ViewDesc *vd, int grid, cudaStream_t st);
 void crg_launch_trace(const DevScene &sc, const WaveBuffers &wb, int cur, bool count, bool sorted, const TraceKnobs &kn, cudaStream_t st);
 /* per-ray records of K2's write-back (crgpu_trace_rays): t, u, v, instance, poly (-1 for spheres and misses), key */
 void crg_launch_trace_records(const DevScene &sc, const WaveBuffers &wb, unsigned n, void *out, int grid, cudaStream_t st);
@@ -186,9 +208,10 @@ bool crg_shade_flat_order(const ShadeKnobs &kn);
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
 /* gate: NULL, or the stop words of an armed scene (below): K5 then adds the batch only if wave set `set`'s batch was not abandoned
  * and the committed pass index equals td.pass_begin.  snap_host: NULL, or (a batch that publishes) the host words, whose snapshot
- * state K5 reads once into gate[3] for the publish step */
+ * state K5 reads once into gate[3] for the publish step.  vd: NULL, or the views of a views call (K5 <ARMED, VIEWS = true>: each
+ * (view, pixel) into its view's framebuffer; armed, it clears gate[3], so a views call never stages a snapshot) */
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st,
-                           unsigned *gate = nullptr, int set = 0, const unsigned *snap_host = nullptr);
+                           unsigned *gate = nullptr, int set = 0, const unsigned *snap_host = nullptr, const ViewDesc *vd = nullptr);
 
 /* ---- stopping an armed scene at a pass boundary (crgpu_stop_enable) ----------------------------------------------------------------
  * ctl (device memory): [0] the pass index the running average has reached in this call, [1 + set] wave set `set`'s batch was

@@ -230,6 +230,48 @@ int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat);
 int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,
                         uint32_t *background_kind, int *complete_interpreter);
 
+/* Rendering several views of a resident scene in one call (c-ray's scene.h cameraCount, "Currently only one camera supported"): stereo
+ * pairs, turntables, camera rigs, thumbnails.  A scene has a list of views, each a camera and a framebuffer of the scene's image size;
+ * after upload it has one.  View 0 IS the scene's camera and framebuffer: crgpu_render_tile(s), crgpu_framebuffer_*, snapshots and
+ * crgpu_trace_kat work on it as before, and crgpu_scene_set_camera sets its camera.
+ *   crgpu_scene_set_views   takes `count` cameras (1 .. CRGPU_MAX_VIEWS) bit for bit, each of the scene's image size; cams[0] becomes the
+ *                           scene camera.  Like the edits above it first waits for the queued work and leaves the scene unchanged when it
+ *                           fails: a NULL scene or cams, a count of 0 or above the limit, or a camera of another size is refused with
+ *                           CRGPU_ERR_BAD_ARGUMENT, a failed allocation with CRGPU_ERR_NOMEM.  It never changes a surviving view's pixels:
+ *                           views 0 .. min(old, new count) - 1 keep their framebuffers, views beyond the old count start zeroed.  The
+ *                           cameras and framebuffers of views 1 .. count - 1 live in one views block from the per-device cache, which
+ *                           only grows and goes back to the cache at crgpu_scene_destroy; the paths-in-flight budget is not changed.
+ *   crgpu_render_views      renders passes [pass_begin, pass_begin + pass_count) of the tile set `rects` (as crgpu_render_tiles takes
+ *                           it, and sharing its cached device pixel list) in each view [first_view, first_view + view_count) as ONE
+ *                           wavefront: one set of batches, and one tail per batch, for all of them.  Afterwards each of those views'
+ *                           framebuffers holds, bit for bit, what crgpu_render_tiles(rects, pass_begin, pass_count) gives after
+ *                           crgpu_scene_set_camera(its camera) on the same framebuffer contents; other views are untouched.  The views
+ *                           share their sampler seeds by design (a seed depends on pixel, pass and sample count only: sampler.c:41-44),
+ *                           which is what makes each view equal to its single render; their noise is therefore correlated.  The call
+ *                           numbers its (view, pixel) pairs view-major and cuts them into pieces of at most max_paths as one pixel set;
+ *                           flags work as in crgpu_render_tiles.  stats.paths is view_count x pixels x passes; rays and, with
+ *                           CRGPU_FLAG_COUNT, P/T/S/I are the sums of the views' single renders.  A view range outside the list, more
+ *                           than 2^32 - 1 (view, pixel) pairs, or a tile set crgpu_render_tiles refuses is refused (nothing rendered).
+ *                           On an armed scene the call is pass-major over all its pairs, so one committed pass index holds for every
+ *                           view: crgpu_request_stop ends it at a pass boundary, crgpu_progress reports it, and a later call for
+ *                           [committed, end) finishes every view bit for bit.  A views call stages no snapshot: a request made during it
+ *                           stays pending (crgpu_take_snapshot returns CRGPU_PENDING while it runs) and is served afterwards as always,
+ *                           by the next publishing call or by crgpu_take_snapshot with no call in flight (view 0's framebuffer).
+ *   crgpu_scene_view_count  the number of views in the list.
+ *   crgpu_view_clear / crgpu_view_read / crgpu_view_to_srgb8
+ *                           zero, copy out (W*H*3 floats in the framebuffer layout) or convert to sRGB8 (crgpu_framebuffer_to_srgb8's
+ *                           arithmetic and layout, W*H*3 bytes) the whole framebuffer of one view of the list.
+ * crgpu_scene_set_instances, _set_instance_list, _set_meshes and _set_shading do not touch the views; every view renders the edited
+ * scene. */
+#define CRGPU_MAX_VIEWS 65536u
+int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *cams, uint32_t count);
+int crgpu_scene_view_count(crgpu_scene *s, uint32_t *count);
+int crgpu_render_views(crgpu_scene *s, uint32_t first_view, uint32_t view_count, const int *rects, int nrects,
+                       int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats);
+int crgpu_view_clear(crgpu_scene *s, uint32_t view);
+int crgpu_view_read(crgpu_scene *s, uint32_t view, float *host_rgb);
+int crgpu_view_to_srgb8(crgpu_scene *s, uint32_t view, uint8_t *host_rgb8);
+
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
  * use) order the kernels with its own work and time them with its own events.  crgpu_use_own_stream goes
