@@ -150,6 +150,9 @@ def lib():
             L.crgpu_scene_set_shading.argtypes = [P, C.POINTER(FlatScene)]
             L.crgpu_scene_shading.argtypes = [P, P, P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
             L.crgpu_scene_set_shading.restype = L.crgpu_scene_shading.restype = C.c_int
+        if hasattr(L, "crgpu_scene_add_objects"):  # absent from libraries built before object adds
+            L.crgpu_scene_add_objects.argtypes = [P, C.POINTER(FlatScene)]
+            L.crgpu_scene_add_objects.restype = C.c_int
         if hasattr(L, "crgpu_render_views"):      # absent from libraries built before views
             L.crgpu_scene_set_views.argtypes = [P, P, C.c_uint32]
             L.crgpu_scene_view_count.argtypes = [P, C.POINTER(C.c_uint32)]
@@ -308,6 +311,12 @@ class GpuScene:
         """Replace the materials, node graph, textures, texel data and background of the resident scene with those of the FlatScene
         `flat` (crgpu_scene_set_shading): same material count, everything else of `flat` is ignored."""
         _check(lib().crgpu_scene_set_shading(self.handle, C.byref(flat)), "crgpu_scene_set_shading")
+
+    def add_objects(self, flat):
+        """Put new meshes and spheres into the resident scene (crgpu_scene_add_objects): the FlatScene `flat` is the grown scene as a
+        whole, its first meshes and spheres the scene's own; the new meshes' BVHs are built on the device, and flat's shading and
+        instance list replace the scene's."""
+        _check(lib().crgpu_scene_add_objects(self.handle, C.byref(flat)), "crgpu_scene_add_objects")
 
     def shading(self):
         """How the shading kernels sample the live scene (crgpu_scene_shading): dict of kinds and flags (uint32 per material, as

@@ -16,6 +16,7 @@
 #include <cstring>
 #include <cstdarg>
 #include <vector>
+#include <algorithm>
 #include <queue>
 #include <thread>
 #include <mutex>
@@ -229,7 +230,12 @@ struct crgpu_scene {
 	uint32_t top_off = 0, top_cap = 0;   /* the top region in the pairs block: first pair and room, at least max(1, n - 1) for the current
 	                                        n instances (reserved behind the uploaded pairs until a list outgrows it) */
 	uint32_t top_stage_cap = 0;      /* staged top-level pairs reserved at upload */
-	uint32_t material_count = 0;     /* as uploaded: a shading edit must keep it */
+	uint32_t material_count = 0;     /* as uploaded or as the last crgpu_scene_add_objects left it: a shading edit must keep it */
+	uint32_t mat_cap = 0;            /* materials dev.materials and dev.flat have room for */
+	uint32_t slot_count = 0, poly_count = 0;             /* triangle slots and polys of the scene */
+	uint32_t slot_cap = 0, poly_cap = 0, bvh_cap = 0;    /* room of the geometry sections dev points at (GeomParts) */
+	DevBlock geom;                   /* NULL until the first add: the geometry block (GeomParts), in place of the slab's sections */
+	DevBlock mats;                   /* NULL until an add outgrows the uploaded materials: the materials block (MatParts) */
 	DevBlock pairs;                  /* NULL until the first geometry edit: the uploaded pairs, the top region, the edited meshes' regions */
 	DevBlock insts;                  /* NULL until the first geometry edit: the instance block (InstParts) */
 	InstParts ip = {};               /* its parts */
@@ -753,7 +759,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	ctx_free(s->device, s->fb8, s->fb_floats);
 	ctx_free(s->device, s->snap8, s->fb_floats);
 	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
-	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade, &s->views }) ctx_free(s->device, b->p, b->bytes);
+	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade, &s->views, &s->geom, &s->mats }) ctx_free(s->device, b->p, b->bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -1080,7 +1086,10 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->top_off = s->pair_count;
 	s->top_cap = p->instance_count > 1u ? p->instance_count - 1u : 1u;
 	s->top_stage_cap = p->top.stage_count;
-	s->material_count = p->material_count;
+	s->material_count = s->mat_cap = p->material_count;
+	s->slot_count = s->slot_cap = (uint32_t)p->key_inst_off;
+	s->poly_count = s->poly_cap = (uint32_t)(p->len[SEC_SPOLYS] / sizeof(ShadePoly));
+	s->bvh_cap = (uint32_t)s->bvhs.size();
 #define FAIL_IF(x) do { int rc_ = (x); if (rc_) { crgpu_scene_destroy(s); return rc_; } } while (0)
 #define CUS(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { int rc_ = fail(CRGPU_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); crgpu_scene_destroy(s); return rc_; } } while (0)
 	CUS(cudaDeviceGetAttribute(&s->sm_count, cudaDevAttrMultiProcessorCount, device));
@@ -1569,9 +1578,9 @@ struct TopParts {
 	uint32_t *last;
 	uint8_t *keys;
 };
-static TopParts take_top(Carve &c, const crgpu_scene *s, uint32_t n, bool list = false) {
+static TopParts take_top(Carve &c, size_t roots, uint32_t n, bool list = false) {
 	TopParts t;
-	t.roots = c.take<float>(s->rec.bvh_root.size());
+	t.roots = c.take<float>(roots);
 	t.bb = c.take<float>(6 * (size_t)n); t.ctr = c.take<float>(3 * (size_t)n); t.offs = c.take<float>(n);
 	t.insts = c.take<DevInstance>(n);
 	t.pairs = c.take<PairNode>(region_pairs(n));
@@ -1692,7 +1701,7 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	crs_instance *dinst = nullptr;
 	TopParts t;
 	void *build = nullptr;
-	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s, n); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
+	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s->rec.bvh_root.size(), n); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
 	if (!rc) rc = alloc_insts(s);
 	if (rc) return rc;
 	/* the roots in a copy of their own: packing them behind the caller's instances would cost a host copy of every instance */
@@ -1707,35 +1716,31 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 
 /* ---- instance-list edits ------------------------------------------------------------------------------------------------------------
  * The new list is validated and packed on the host (pack_instances, as crgpu_prepare packs it), and its boxes, ray offsets and top level
- * are built on the device into scratch.  Only once the build has passed the upload's checks do the blocks change: the pairs block
- * grows when the top region cannot hold a top level of the new count, and the instance block is replaced when it has no records of
- * its own or no room for the new count.  Then the records, keys, last table, top region, item records and staged prefix are
- * committed and published, and the replaced instance block goes back to the per-device cache. */
-extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
-	if (!s || (count && !inst)) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	if (count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "%u instances (the device builder's limit is 4194304)", count);
-	InstancePack pk;
-	int rc = pack_instances(inst, count, s->rec.spheres.data(), (uint32_t)s->rec.spheres.size(), s->rec.meshes.data(), (uint32_t)s->rec.meshes.size(),
-	                        s->material_count, CRGPU_ERR_BAD_ARGUMENT, pk);
-	if (rc) return rc;
-	rc = drain(s);
-	if (rc) return rc;
-	const uint32_t n = count;
-	TopParts t;
-	void *build = nullptr;
-	rc = carve(s->device, s->scratch, [&](Carve &c) { t = take_top(c, s, n, true); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
-	if (rc) return rc;
+ * are built on the device into scratch (stage_list).  Only once the build has passed the upload's checks do the blocks change
+ * (commit_list): the pairs block grows when the top region cannot hold a top level of the new count, and the instance block is replaced
+ * when it has no records of its own or no room for the new count.  Then the records, keys, last table, top region, item records and
+ * staged prefix are committed and published, and the replaced instance block goes back to the per-device cache. */
+
+/* Uploads the packed list of n instances and the BVH roots (6 floats per BVH) into the scratch parts t (take_top with `list`) and builds
+ * their boxes, ray offsets and top level there.  Changes nothing the kernels read. */
+static int stage_list(crgpu_scene *s, const InstancePack &pk, uint32_t n, const std::vector<float> &roots, const TopParts &t, void *build,
+                      CrgBuildResult *res) {
 	cudaStream_t st = s->stream;
 	if (n) {
 		CU(cudaMemcpyAsync(t.insts, pk.recs.data(), (size_t)n * sizeof(DevInstance), cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(t.last, pk.last.data(), (size_t)n * 4u, cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(t.keys, pk.keys.data(), n, cudaMemcpyHostToDevice, st));
 	}
-	CU(cudaMemcpyAsync(t.roots, s->rec.bvh_root.data(), s->rec.bvh_root.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-	CrgBuildResult res;
-	rc = build_top(s, n, nullptr, nullptr, t, build, &res);
-	if (rc) return rc;
+	CU(cudaMemcpyAsync(t.roots, roots.data(), roots.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+	return build_top(s, n, nullptr, nullptr, t, build, res);
+}
 
+/* Makes a staged list of n instances (kinds and objects from inst) the scene's: grows the top region and the instance block as needed,
+ * runs before_commit (the caller's own commits, which the item records may read), then commits the list and the top level and
+ * publishes the descriptor. */
+template <class F>
+static int commit_list(crgpu_scene *s, const crs_instance *inst, uint32_t n, const InstancePack &pk, const TopParts &t, const CrgBuildResult &res,
+                       F before_commit) {
 	/* the top region: the current one while it holds any top level of n instances (region_pairs(n)), else a new one behind every pair
 	 * of the block; mesh regions never move.  A region that has to move grows by half at least, so that adding instances a few at a
 	 * time does not leave a trail of abandoned regions. */
@@ -1746,7 +1751,8 @@ extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_in
 		if (s->pairs.p) top_off = s->pair_cap;            /* before the first geometry edit the reserved region is simply larger */
 	}
 	const uint64_t need = (uint64_t)top_off + top_cap;
-	if (need > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "set_instance_list: more pair nodes than the scene can address");
+	if (need > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "instance list: more pair nodes than the scene can address");
+	int rc;
 	if (!s->pairs.p || need > s->pair_cap) {
 		rc = reserve_pairs(s, (uint32_t)(need > s->pair_cap ? need : s->pair_cap));
 		if (rc) return rc;
@@ -1767,6 +1773,9 @@ extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_in
 	}
 
 	/* commit */
+	rc = before_commit();
+	if (rc) return rc;
+	cudaStream_t st = s->stream;
 	if (n) {
 		CU(cudaMemcpyAsync(s->ip.last, t.last, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
 		CU(cudaMemcpyAsync(s->ip.keys, t.keys, n, cudaMemcpyDeviceToDevice, st));
@@ -1785,6 +1794,26 @@ extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_in
 	for (uint32_t i = 0; i < n; ++i) { r.inst_kind[i] = inst[i].kind; r.inst_object[i] = inst[i].object; }
 	r.last = pk.last;
 	return CRGPU_OK;
+}
+
+extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
+	if (!s || (count && !inst)) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "%u instances (the device builder's limit is 4194304)", count);
+	InstancePack pk;
+	int rc = pack_instances(inst, count, s->rec.spheres.data(), (uint32_t)s->rec.spheres.size(), s->rec.meshes.data(), (uint32_t)s->rec.meshes.size(),
+	                        s->material_count, CRGPU_ERR_BAD_ARGUMENT, pk);
+	if (rc) return rc;
+	rc = drain(s);
+	if (rc) return rc;
+	const uint32_t n = count;
+	TopParts t;
+	void *build = nullptr;
+	rc = carve(s->device, s->scratch, [&](Carve &c) { t = take_top(c, s->rec.bvh_root.size(), n, true); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
+	if (rc) return rc;
+	CrgBuildResult res;
+	rc = stage_list(s, pk, n, s->rec.bvh_root, t, build, &res);
+	if (rc) return rc;
+	return commit_list(s, inst, n, pk, t, res, [] { return CRGPU_OK; });
 }
 
 /* ---- mesh edits ---------------------------------------------------------------------------------------------------------------------
@@ -1840,6 +1869,84 @@ static int check_mesh_polys(const crs_scene *f, const crs_mesh &mesh, MeshEdit &
 	return CRGPU_OK;
 }
 
+/* the fields of a mesh record that fix its topology: an edit keeps them */
+static bool same_mesh(const crs_mesh &a, const crs_mesh &b) {
+	return a.poly_offset == b.poly_offset && a.poly_count == b.poly_count && a.material_offset == b.material_offset &&
+	       a.material_count == b.material_count && a.texcoord_count == b.texcoord_count && a.bvh == b.bvh;
+}
+
+/* a mesh build's inputs and records in an edit call's scratch */
+static void take_mesh(Carve &c, MeshEdit &e) {
+	e.polys = c.take<crs_poly>(e.n);
+	e.verts = c.take<float>(3 * (size_t)(e.vhi - e.vlo)); e.norms = c.take<float>(3 * (size_t)(e.nhi - e.nlo)); e.uvs = c.take<float>(2 * (size_t)(e.thi - e.tlo));
+	e.bb = c.take<float>(6 * (size_t)e.n); e.ctr = c.take<float>(3 * (size_t)e.n);
+	e.pairs = c.take<PairNode>(region_pairs(e.n)); e.prims = c.take<int32_t>(e.n);
+	e.tris = c.take<PackedTri>(e.n); e.slot = c.take<uint32_t>(e.n); e.keys = c.take<uint8_t>(e.n); e.spolys = c.take<ShadePoly>(e.n);
+}
+
+/* Each mesh's triangle boxes, BVH, triangles, slot records and shading records, built on the device into its scratch parts from the
+ * polys and the record f gives it.  Changes nothing the kernels read. */
+static int build_meshes(crgpu_scene *s, const crs_scene *f, std::vector<MeshEdit> &edits, void *build) {
+	cudaStream_t st = s->stream;
+	for (MeshEdit &e : edits) {
+		const crs_mesh &mesh = f->meshes[e.mesh];
+		CU(cudaMemcpyAsync(e.polys, f->polys + mesh.poly_offset, (size_t)e.n * sizeof(crs_poly), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(e.verts, f->vertices + 3 * (size_t)e.vlo, (size_t)(e.vhi - e.vlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.nhi > e.nlo) CU(cudaMemcpyAsync(e.norms, f->normals + 3 * (size_t)e.nlo, (size_t)(e.nhi - e.nlo) * 12u, cudaMemcpyHostToDevice, st));
+		if (e.thi > e.tlo) CU(cudaMemcpyAsync(e.uvs, f->texcoords + 2 * (size_t)e.tlo, (size_t)(e.thi - e.tlo) * 8u, cudaMemcpyHostToDevice, st));
+		crg_launch_poly_boxes(e.polys, e.verts, e.vlo, e.n, e.bb, e.ctr, st);
+		CU(cudaGetLastError());
+		int rc = crg_bvh_build_pairs(e.bb, e.ctr, e.n, build, st, e.pairs, e.prims, &e.res);
+		if (rc) return rc;
+		if (e.res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: BVH deeper than 64 levels", e.mesh);
+		const CrgMeshRepack r = { e.polys, e.verts, e.norms, e.uvs, e.vlo, e.nlo, e.tlo, e.n, mesh.poly_offset, mesh.material_offset, mesh.texcoord_count };
+		crg_launch_mesh_repack(r, e.prims, e.tris, e.slot, e.keys, e.spolys, st);
+		CU(cudaGetLastError());
+	}
+	return CRGPU_OK;
+}
+
+/* Gives each mesh of `edits` that has no region yet (region[mesh] == UINT32_MAX) its own region of pair nodes behind every pair of the
+ * block, in one reserve_pairs; the first geometry edit also reserves the top region behind the uploaded pairs. */
+static int reserve_regions(crgpu_scene *s, std::vector<uint32_t> &region, const std::vector<MeshEdit> &edits) {
+	const uint32_t first = s->pairs.p ? s->pair_cap : s->top_off + s->top_cap;
+	uint64_t add = 0;
+	for (const MeshEdit &e : edits) if (region[e.mesh] == 0xffffffffu) add += region_pairs(e.n);
+	if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "mesh edit: more pair nodes than the scene can address");
+	if (first + add <= s->pair_cap) return CRGPU_OK;
+	int rc = reserve_pairs(s, first + (uint32_t)add);
+	if (rc) return rc;
+	uint32_t next = first;
+	for (const MeshEdit &e : edits)
+		if (region[e.mesh] == 0xffffffffu) { region[e.mesh] = next; next += region_pairs(e.n); }
+	return CRGPU_OK;
+}
+
+/* The sections the kernels read by triangle slot (tris, slot_poly, slot_key), by global poly (spolys) and by BVH (bvhs).  The slab holds
+ * them until crgpu_scene_add_objects first grows them; the geometry block then holds them in this order. */
+struct GeomParts {
+	PackedTri *tris;
+	uint32_t *slot_poly;
+	uint8_t *slot_key;
+	ShadePoly *spolys;
+	DevBvh *bvhs;
+};
+static GeomParts geom_live(const crgpu_scene *s) {
+	return { const_cast<PackedTri *>(s->dev.tris), const_cast<uint32_t *>(s->dev.slot_poly), const_cast<uint8_t *>(s->dev.slot_key),
+	         const_cast<ShadePoly *>(s->dev.spolys), const_cast<DevBvh *>(s->dev.bvhs) };
+}
+
+/* Copies a built mesh over its pair region, its slots from slot_offset and its polys from poly_offset in the sections g. */
+static int commit_mesh(crgpu_scene *s, const MeshEdit &e, const GeomParts &g, uint32_t region, uint32_t slot_offset, uint32_t poly_offset) {
+	cudaStream_t st = s->stream;
+	if (e.res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + region, e.pairs, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	CU(cudaMemcpyAsync(g.tris + slot_offset, e.tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
+	CU(cudaMemcpyAsync(g.slot_poly + slot_offset, e.slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
+	CU(cudaMemcpyAsync(g.slot_key + slot_offset, e.keys, e.n, cudaMemcpyDeviceToDevice, st));
+	CU(cudaMemcpyAsync(g.spolys + poly_offset, e.spolys, (size_t)e.n * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
+	return CRGPU_OK;
+}
+
 /* Each listed mesh's triangle boxes, BVH, triangles, slot records and shading records, then the instances and the top level, are
  * rebuilt on the device into scratch; only once every build has passed the upload's checks are they copied over the scene. */
 extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count) {
@@ -1853,8 +1960,7 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 		if (listed[m]) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u listed twice", m);
 		listed[m] = 1u;
 		const crs_mesh &a = s->rec.meshes[m], &b = flat->meshes[m];
-		if (a.poly_offset != b.poly_offset || a.poly_count != b.poly_count || a.material_offset != b.material_offset || a.material_count != b.material_count ||
-		    a.texcoord_count != b.texcoord_count || a.bvh != b.bvh)
+		if (!same_mesh(a, b))
 			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its record differs from the uploaded one (the topology cannot change)", m);
 		if (a.bvh >= s->rec.bvh_prims.size() || s->rec.bvh_prims[a.bvh] != a.poly_count)
 			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its uploaded BVH does not cover exactly its polys", m);
@@ -1878,33 +1984,14 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	TopParts t;
 	void *build = nullptr;
 	rc = carve(s->device, s->scratch, [&](Carve &c) {
-		for (MeshEdit &e : edits) {
-			e.polys = c.take<crs_poly>(e.n);
-			e.verts = c.take<float>(3 * (size_t)(e.vhi - e.vlo)); e.norms = c.take<float>(3 * (size_t)(e.nhi - e.nlo)); e.uvs = c.take<float>(2 * (size_t)(e.thi - e.tlo));
-			e.bb = c.take<float>(6 * (size_t)e.n); e.ctr = c.take<float>(3 * (size_t)e.n);
-			e.pairs = c.take<PairNode>(region_pairs(e.n)); e.prims = c.take<int32_t>(e.n);
-			e.tris = c.take<PackedTri>(e.n); e.slot = c.take<uint32_t>(e.n); e.keys = c.take<uint8_t>(e.n); e.spolys = c.take<ShadePoly>(e.n);
-		}
-		t = take_top(c, s, ninst);
+		for (MeshEdit &e : edits) take_mesh(c, e);
+		t = take_top(c, s->rec.bvh_root.size(), ninst);
 		build = c.take<uint8_t>(crg_bvh_scratch_bytes(nmax));
 	});
 	if (rc) return rc;
+	rc = build_meshes(s, flat, edits, build);
+	if (rc) return rc;
 	cudaStream_t st = s->stream;
-	for (MeshEdit &e : edits) {
-		const crs_mesh &mesh = flat->meshes[e.mesh];
-		CU(cudaMemcpyAsync(e.polys, flat->polys + mesh.poly_offset, (size_t)e.n * sizeof(crs_poly), cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(e.verts, flat->vertices + 3 * (size_t)e.vlo, (size_t)(e.vhi - e.vlo) * 12u, cudaMemcpyHostToDevice, st));
-		if (e.nhi > e.nlo) CU(cudaMemcpyAsync(e.norms, flat->normals + 3 * (size_t)e.nlo, (size_t)(e.nhi - e.nlo) * 12u, cudaMemcpyHostToDevice, st));
-		if (e.thi > e.tlo) CU(cudaMemcpyAsync(e.uvs, flat->texcoords + 2 * (size_t)e.tlo, (size_t)(e.thi - e.tlo) * 8u, cudaMemcpyHostToDevice, st));
-		crg_launch_poly_boxes(e.polys, e.verts, e.vlo, e.n, e.bb, e.ctr, st);
-		CU(cudaGetLastError());
-		rc = crg_bvh_build_pairs(e.bb, e.ctr, e.n, build, st, e.pairs, e.prims, &e.res);
-		if (rc) return rc;
-		if (e.res.levels > CRG_MAX_STACK) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: BVH deeper than 64 levels", e.mesh);
-		const CrgMeshRepack r = { e.polys, e.verts, e.norms, e.uvs, e.vlo, e.nlo, e.tlo, e.n, mesh.poly_offset, mesh.material_offset, mesh.texcoord_count };
-		crg_launch_mesh_repack(r, e.prims, e.tris, e.slot, e.keys, e.spolys, st);
-		CU(cudaGetLastError());
-	}
 
 	/* the top level over the new mesh roots */
 	std::vector<float> roots = s->rec.bvh_root;
@@ -1917,32 +2004,18 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 		if (!rc) rc = build_top(s, ninst, s->dev.instances, nullptr, t, build, &top);
 		if (rc) return rc;
 	}
-	/* the first geometry edit reserves the top region behind the uploaded pairs, and the first edit of a mesh its own region behind
-	 * every pair of the block */
-	const uint32_t first = s->pairs.p ? s->pair_cap : s->top_off + s->top_cap;
-	uint32_t add = 0;
-	for (const MeshEdit &e : edits) if (s->mesh_region[e.mesh] == 0xffffffffu) add += region_pairs(e.n);
-	if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "set_meshes: more pair nodes than the scene can address");
-	if (first + add > s->pair_cap) {
-		rc = reserve_pairs(s, first + add);
-		if (rc) return rc;
-		uint32_t next = first;
-		for (const MeshEdit &e : edits)
-			if (s->mesh_region[e.mesh] == 0xffffffffu) { s->mesh_region[e.mesh] = next; next += region_pairs(e.n); }
-	}
+	rc = reserve_regions(s, s->mesh_region, edits);
+	if (rc) return rc;
 
 	/* commit: each mesh's region, slot and poly ranges, BVH record and staged prefix, then the instances and the top level */
+	const GeomParts g = geom_live(s);
 	for (const MeshEdit &e : edits) {
-		const crs_mesh &mesh = s->rec.meshes[e.mesh];
 		DevBvh &b = s->bvhs[e.bvh];
 		const uint32_t region = s->mesh_region[e.mesh];
-		if (e.res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + region, e.pairs, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<PackedTri *>(s->dev.tris) + b.slot_offset, e.tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<uint32_t *>(s->dev.slot_poly) + b.slot_offset, e.slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.slot_key) + b.slot_offset, e.keys, e.n, cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<ShadePoly *>(s->dev.spolys) + mesh.poly_offset, e.spolys, (size_t)e.n * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
+		rc = commit_mesh(s, e, g, region, b.slot_offset, s->rec.meshes[e.mesh].poly_offset);
+		if (rc) return rc;
 		b = bvh_record(e.res, region, b.slot_offset, b.stage_base, s->stage_cap[e.bvh]);
-		CU(cudaMemcpyAsync(const_cast<DevBvh *>(s->dev.bvhs) + e.bvh, &b, sizeof b, cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(g.bvhs + e.bvh, &b, sizeof b, cudaMemcpyHostToDevice, st));
 		if (b.stage_count)
 			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, e.pairs, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	}
@@ -1952,9 +2025,51 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 }
 
 /* ---- shading edits ------------------------------------------------------------------------------------------------------------------
- * The records whose size the material count fixes (materials, flat records, K4's key order) are rewritten in the slab; the node graph,
+ * The records whose size the material count fixes (materials, flat records, K4's key order) are rewritten in place; the node graph,
  * texture table and texel data, whose sizes may change, go into a new shading block that replaces the previous one.  Every check and
  * the fold run first and the block is filled before anything the kernels read changes. */
+struct ShadeBlock {
+	DevBlock blk;
+	crs_node *nodes;
+	DevTexture *texs;
+};
+/* The node graph, texture table (with the block's addresses) and texel data of `flat` in a new shading block, uploaded and waited for. */
+static int upload_shading(crgpu_scene *s, const crs_scene *flat, ShadingFold &sh, ShadeBlock &out) {
+	uint8_t *data = nullptr;
+	out = ShadeBlock();
+	int rc = carve(s->device, out.blk, [&](Carve &c) { out.nodes = c.take<crs_node>(flat->node_count); out.texs = c.take<DevTexture>(sh.texs.size()); data = c.take<uint8_t>(flat->texdata_bytes); });
+	if (rc) return rc;
+	for (DevTexture &t : sh.texs) t.data = data + (uintptr_t)t.data;
+	cudaStream_t st = s->stream;
+	cudaError_t ce = cudaSuccess;
+	if (flat->node_count) ce = cudaMemcpyAsync(out.nodes, flat->nodes, (size_t)flat->node_count * sizeof(crs_node), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && !sh.texs.empty()) ce = cudaMemcpyAsync(out.texs, sh.texs.data(), sh.texs.size() * sizeof(DevTexture), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (ce != cudaSuccess) { ctx_free(s->device, out.blk.p, out.blk.bytes); out.blk = DevBlock(); return fail(CRGPU_ERR_CUDA, "shading edit: %s", cudaGetErrorString(ce)); }
+	return CRGPU_OK;
+}
+/* Writes the fold's materials (flat->material_count of them), flat records and key order over dev.materials, dev.flat and dev.key_order,
+ * points the descriptor at the uploaded block and returns the block it replaces in `old` (free it after the publish). */
+static int commit_shading(crgpu_scene *s, const crs_scene *flat, const ShadingFold &sh, const ShadeBlock &b, DevBlock &old) {
+	cudaStream_t st = s->stream;
+	const size_t nm = flat->material_count;
+	if (nm) {
+		CU(cudaMemcpyAsync(const_cast<DevMaterial *>(s->dev.materials), sh.mats.data(), nm * sizeof(DevMaterial), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<DevFlat *>(s->dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
+	}
+	CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
+	s->dev.nodes = b.nodes;
+	s->dev.textures = b.texs;
+	s->dev.bg = sh.bg;
+	s->dev.flat_keys = sh.flat_keys;
+	s->dev.background = flat->background;
+	s->xnodes = sh.xnodes;
+	old = s->shade;
+	s->shade = b.blk;
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat) {
 	if (!s || !flat) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (flat->material_count != s->material_count)
@@ -1964,39 +2079,195 @@ extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *f
 	if (rc) return rc;
 	rc = drain(s);
 	if (rc) return rc;
-	DevBlock blk;
-	crs_node *nodes = nullptr;
-	DevTexture *texs = nullptr;
-	uint8_t *data = nullptr;
-	rc = carve(s->device, blk, [&](Carve &c) { nodes = c.take<crs_node>(flat->node_count); texs = c.take<DevTexture>(sh.texs.size()); data = c.take<uint8_t>(flat->texdata_bytes); });
+	ShadeBlock b;
+	rc = upload_shading(s, flat, sh, b);
 	if (rc) return rc;
-	for (DevTexture &t : sh.texs) t.data = data + (uintptr_t)t.data;
-	cudaStream_t st = s->stream;
-	cudaError_t ce = cudaSuccess;
-	if (flat->node_count) ce = cudaMemcpyAsync(nodes, flat->nodes, (size_t)flat->node_count * sizeof(crs_node), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && !sh.texs.empty()) ce = cudaMemcpyAsync(texs, sh.texs.data(), sh.texs.size() * sizeof(DevTexture), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) { ctx_free(s->device, blk.p, blk.bytes); return fail(CRGPU_ERR_CUDA, "set_shading: %s", cudaGetErrorString(ce)); }
-
-	/* commit */
-	const size_t nm = s->material_count;
-	if (nm) {
-		CU(cudaMemcpyAsync(const_cast<DevMaterial *>(s->dev.materials), sh.mats.data(), nm * sizeof(DevMaterial), cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<DevFlat *>(s->dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
-	}
-	CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
-	s->dev.nodes = nodes;
-	s->dev.textures = texs;
-	s->dev.bg = sh.bg;
-	s->dev.flat_keys = sh.flat_keys;
-	s->dev.background = flat->background;
-	s->xnodes = sh.xnodes;
-	const DevBlock old = s->shade;
-	s->shade = blk;
-	rc = publish(s);
+	DevBlock old;
+	rc = commit_shading(s, flat, sh, b, old);
+	if (!rc) rc = publish(s);
 	if (!rc) ctx_free(s->device, old.p, old.bytes);   /* the descriptor no longer points at it */
 	return rc;
+}
+
+/* ---- adding objects -----------------------------------------------------------------------------------------------------------------
+ * The scene takes the objects, shading and instance list of a grown flat scene B whose first meshes and spheres are the scene's.  Every
+ * check, the shading fold and the instance packing run on the host first; then each new mesh is built on the device and the top level
+ * over B's list, all into scratch (build_meshes, stage_list).  Only then are the blocks grown: a new shading block, the geometry block
+ * when B's slots, polys or BVHs outgrow it, the materials block when B's materials do, one reserve_pairs for the new meshes' regions,
+ * and the top region and instance block as an instance-list edit grows them.  The new meshes' records and the grown BVH table are
+ * written behind the existing ones, the descriptor is published once, and only then do the replaced blocks go back to the cache. */
+
+/* The geometry block's parts for the given room (GeomParts). */
+static GeomParts take_geom(Carve &c, uint32_t slots, uint32_t polys, uint32_t bvhs) {
+	GeomParts g;
+	g.tris = c.take<PackedTri>(slots);
+	g.slot_poly = c.take<uint32_t>(slots);
+	g.slot_key = c.take<uint8_t>(slots);
+	g.spolys = c.take<ShadePoly>(polys);
+	g.bvhs = c.take<DevBvh>(bvhs);
+	return g;
+}
+/* room for `need` in a section that holds `cap`: at least half as much again, so that objects added one at a time do not copy the
+ * section every time */
+static uint32_t grown_cap(uint32_t cap, uint32_t need) {
+	const uint64_t g = (uint64_t)cap + cap / 2u;
+	return need <= cap ? cap : (g > need ? (uint32_t)(g < 0xffffffffull ? g : 0xffffffffull) : need);
+}
+/* The materials block's parts (dev.materials, dev.flat). */
+struct MatParts {
+	DevMaterial *mats;
+	DevFlat *flat;
+};
+
+extern "C" int crgpu_scene_add_objects(crgpu_scene *s, const struct crs_scene *flat) {
+	if (!s || !flat) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	const crs_scene &B = *flat;
+	const uint32_t M = (uint32_t)s->rec.meshes.size(), S = (uint32_t)s->rec.spheres.size(), P = s->poly_count;
+	if (B.mesh_count < M || B.sphere_count < S)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "%u meshes and %u spheres given, the scene has %u and %u", B.mesh_count, B.sphere_count, M, S);
+	if (B.top_bvh >= B.bvh_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "top_bvh out of range");
+	if (B.poly_count < P) return fail(CRGPU_ERR_BAD_ARGUMENT, "%u polys given, the scene has %u", B.poly_count, P);
+	std::vector<uint8_t> bvh_taken(B.bvh_count, 0u);
+	auto take_bvh = [&](uint32_t m, uint32_t b) {
+		if (b >= B.bvh_count || b == B.top_bvh || bvh_taken[b]) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: bvh index %u out of range, the top level's or another mesh's", m, b);
+		bvh_taken[b] = 1u;
+		return CRGPU_OK;
+	};
+	int rc;
+	for (uint32_t m = 0; m < M; ++m) {
+		const crs_mesh &b = B.meshes[m];
+		if (!same_mesh(s->rec.meshes[m], b)) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u: its record differs from the scene's", m);
+		if ((uint64_t)b.material_offset + b.material_count > B.material_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u ranges out of bounds", m);
+		if ((rc = take_bvh(m, b.bvh))) return rc;
+	}
+	for (uint32_t k = 0; k < S; ++k)
+		if (memcmp(&s->rec.spheres[k].radius, &B.spheres[k].radius, sizeof(float)))
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "sphere %u: its radius differs from the scene's", k);
+	/* the new meshes: checked as crgpu_prepare checks them; their polys lie behind the scene's, one range each */
+	std::vector<MeshEdit> edits;
+	std::vector<uint32_t> empty;                     /* BVHs of new meshes without polys (no build: an empty BVH) */
+	std::vector<std::pair<uint32_t, uint32_t>> ranges;
+	uint64_t slots = s->slot_count;
+	for (uint32_t m = M; m < B.mesh_count; ++m) {
+		const crs_mesh &b = B.meshes[m];
+		if (b.poly_offset < P || (uint64_t)b.poly_offset + b.poly_count > B.poly_count || (uint64_t)b.material_offset + b.material_count > B.material_count)
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "mesh %u ranges out of bounds", m);
+		if ((rc = take_bvh(m, b.bvh))) return rc;
+		if (b.poly_count > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "mesh %u: %u polys (the device builder's limit is 4194304)", m, b.poly_count);
+		MeshEdit e;
+		memset(&e, 0, sizeof e);
+		e.mesh = m; e.bvh = b.bvh; e.n = b.poly_count;
+		if ((rc = check_mesh_polys(flat, b, e))) return rc;
+		if (e.n) { edits.push_back(e); ranges.push_back({ b.poly_offset, b.poly_count }); }
+		else empty.push_back(b.bvh);
+		slots += b.poly_count;
+	}
+	std::sort(ranges.begin(), ranges.end());
+	for (size_t k = 1; k < ranges.size(); ++k)
+		if ((uint64_t)ranges[k - 1].first + ranges[k - 1].second > ranges[k].first) return fail(CRGPU_ERR_BAD_ARGUMENT, "new meshes share polys");
+	if (slots > 0xffffffffull) return fail(CRGPU_ERR_UNSUPPORTED, "more than 2^32 triangle slots");
+	ShadingFold sh;
+	if ((rc = fold_shading(flat, sh))) return rc;
+	const uint32_t n = B.instance_count;
+	if (n && !B.instances) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL instances");
+	if (n > 4194304u) return fail(CRGPU_ERR_UNSUPPORTED, "%u instances (the device builder's limit is 4194304)", n);
+	InstancePack pk;
+	if ((rc = pack_instances(B.instances, n, B.spheres, B.sphere_count, B.meshes, B.mesh_count, B.material_count, CRGPU_ERR_BAD_ARGUMENT, pk))) return rc;
+	if ((rc = drain(s))) return rc;
+
+	/* build into scratch: the new meshes, in BVH order (a fresh load gives them slots in that order), then the top level */
+	std::sort(edits.begin(), edits.end(), [](const MeshEdit &a, const MeshEdit &b) { return a.bvh < b.bvh; });
+	uint32_t nmax = n;
+	for (const MeshEdit &e : edits) nmax = e.n > nmax ? e.n : nmax;
+	const size_t nroots = 6 * (size_t)B.bvh_count;
+	TopParts t;
+	void *build = nullptr;
+	rc = carve(s->device, s->scratch, [&](Carve &c) {
+		for (MeshEdit &e : edits) take_mesh(c, e);
+		t = take_top(c, nroots, n, true);
+		build = c.take<uint8_t>(crg_bvh_scratch_bytes(nmax));
+	});
+	if (!rc) rc = build_meshes(s, flat, edits, build);
+	if (rc) return rc;
+	/* the grown host records: the new meshes' roots and primitive counts; B's BVH indices name the device records from here on */
+	std::vector<float> roots = s->rec.bvh_root;
+	std::vector<uint32_t> prims = s->rec.bvh_prims, stage_cap = s->stage_cap;
+	std::vector<DevBvh> bvhs = s->bvhs;
+	roots.resize(nroots, 0.f);
+	prims.resize(B.bvh_count, 0u);
+	stage_cap.resize(B.bvh_count, 0u);
+	bvhs.resize(B.bvh_count);
+	for (uint32_t b : empty) {
+		memset(&bvhs[b], 0, sizeof(DevBvh));
+		memset(&roots[6 * (size_t)b], 0, 6 * sizeof(float));
+		prims[b] = 0u; stage_cap[b] = 0u;
+	}
+	for (const MeshEdit &e : edits) { memcpy(&roots[6 * (size_t)e.bvh], e.res.bounds, 6 * sizeof(float)); prims[e.bvh] = e.n; stage_cap[e.bvh] = 0u; }
+	CrgBuildResult top;
+	if ((rc = stage_list(s, pk, n, roots, t, build, &top))) return rc;
+
+	/* grow: shading block, geometry block, materials block, the new meshes' pair regions */
+	cudaStream_t st = s->stream;
+	ShadeBlock shb;
+	if ((rc = upload_shading(s, flat, sh, shb))) return rc;
+	DevBlock geom, mats;
+	auto drop = [&](int code) { for (DevBlock *b : { &shb.blk, &geom, &mats }) ctx_free(s->device, b->p, b->bytes); return code; };
+	GeomParts g = geom_live(s);
+	const uint32_t slot_need = (uint32_t)slots;
+	uint32_t slot_cap = s->slot_cap, poly_cap = s->poly_cap, bvh_cap = s->bvh_cap;
+	if (slot_need > slot_cap || B.poly_count > poly_cap || B.bvh_count > bvh_cap) {
+		slot_cap = grown_cap(slot_cap, slot_need); poly_cap = grown_cap(poly_cap, B.poly_count); bvh_cap = grown_cap(bvh_cap, B.bvh_count);
+		if ((rc = carve(s->device, geom, [&](Carve &c) { g = take_geom(c, slot_cap, poly_cap, bvh_cap); }))) return drop(rc);
+		const GeomParts live = geom_live(s);
+		const size_t ns = s->slot_count;
+		cudaError_t ce = cudaMemcpyAsync(g.tris, live.tris, ns * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st);
+		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.slot_poly, live.slot_poly, ns * 4u, cudaMemcpyDeviceToDevice, st);
+		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.slot_key, live.slot_key, ns, cudaMemcpyDeviceToDevice, st);
+		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.spolys, live.spolys, (size_t)s->poly_count * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st);
+		if (ce != cudaSuccess) return drop(fail(CRGPU_ERR_CUDA, "add_objects: %s", cudaGetErrorString(ce)));
+	}
+	MatParts mp = { const_cast<DevMaterial *>(s->dev.materials), const_cast<DevFlat *>(s->dev.flat) };
+	if (B.material_count > s->mat_cap &&
+	    (rc = carve(s->device, mats, [&](Carve &c) { mp.mats = c.take<DevMaterial>(B.material_count); mp.flat = c.take<DevFlat>(B.material_count); })))
+		return drop(rc);
+	std::vector<uint32_t> region = s->mesh_region;
+	region.resize(B.mesh_count, 0xffffffffu);
+	if ((rc = reserve_regions(s, region, edits))) return drop(rc);
+
+	/* commit, inside the list's commit: the BVH records the item records read must be in place first */
+	DevBlock old_shade, old_geom, old_mats;
+	rc = commit_list(s, B.instances, n, pk, t, top, [&]() -> int {
+		uint32_t slot = s->slot_count;
+		for (const MeshEdit &e : edits) {
+			int r = commit_mesh(s, e, g, region[e.mesh], slot, B.meshes[e.mesh].poly_offset);
+			if (r) return r;
+			bvhs[e.bvh] = bvh_record(e.res, region[e.mesh], slot, 0u, 0u);
+			slot += e.n;
+		}
+		CU(cudaMemcpyAsync(g.bvhs, bvhs.data(), bvhs.size() * sizeof(DevBvh), cudaMemcpyHostToDevice, st));
+		s->dev.tris = g.tris; s->dev.slot_poly = g.slot_poly; s->dev.slot_key = g.slot_key; s->dev.spolys = g.spolys; s->dev.bvhs = g.bvhs;
+		s->dev.materials = mp.mats; s->dev.flat = mp.flat;
+		int r = commit_shading(s, flat, sh, shb, old_shade);
+		if (r) return r;
+		if (geom.p) { old_geom = s->geom; s->geom = geom; s->slot_cap = slot_cap; s->poly_cap = poly_cap; s->bvh_cap = bvh_cap; }
+		if (mats.p) { old_mats = s->mats; s->mats = mats; s->mat_cap = B.material_count; }
+		geom = mats = shb.blk = DevBlock();                   /* the scene owns them now */
+		return CRGPU_OK;
+	});
+	if (rc) return drop(rc);
+	for (DevBlock *b : { &old_shade, &old_geom, &old_mats }) ctx_free(s->device, b->p, b->bytes);   /* the descriptor no longer points at them */
+	s->material_count = B.material_count;
+	s->slot_count = slot_need;
+	s->poly_count = B.poly_count;
+	s->mesh_region = region;
+	s->bvhs = bvhs;
+	s->stage_cap = stage_cap;
+	EditRecord &r = s->rec;
+	r.meshes.assign(B.meshes, B.meshes + B.mesh_count);
+	r.spheres.assign(B.spheres, B.spheres + B.sphere_count);
+	r.bvh_root = roots;
+	r.bvh_prims = prims;
+	return CRGPU_OK;
 }
 
 extern "C" int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,

@@ -180,9 +180,9 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *                              crloader_build_bvh in crloader.h) or is deeper than 64 levels is refused with CRGPU_ERR_UNSUPPORTED.
  *   crgpu_scene_set_instance_list  replaces the whole instance list: instance i of `inst` becomes instance i of the scene, `count`
  *                              from 0 to 4,194,304 (the device builder's limit; above it CRGPU_ERR_UNSUPPORTED before any instance is
- *                              read).  Each instance is a CRS_INST_SPHERE or CRS_INST_MESH of an uploaded sphere or mesh, also one
- *                              that had no instance; no object is created.  A sphere instance takes its sphere's uploaded radius and
- *                              material, a mesh instance its mesh's current BVH (crgpu_scene_set_meshes included), and every object
+ *                              read).  Each instance is a CRS_INST_SPHERE or CRS_INST_MESH of a sphere or mesh of the scene (uploaded
+ *                              or added by crgpu_scene_add_objects), also one that had no instance; this call creates no object.  A
+ *                              sphere instance takes its sphere's radius and material, a mesh instance its mesh's current BVH (crgpu_scene_set_meshes included), and every object
  *                              the ray offset of its last instance, as the scene loader gives them.  A and Ainv are taken bit for bit.
  *                              A NULL `inst` with count > 0, another kind or an object out of range is refused with
  *                              CRGPU_ERR_BAD_ARGUMENT; a top level of more than 2 count - 1 nodes or deeper than 64 levels with
@@ -209,13 +209,38 @@ int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *passes_done);
  *   crgpu_scene_set_shading    replaces the materials, the node graph, the textures, the texel data and the background root
  *                              (crSetHDR, and recolouring, re-bsdf'ing or lighting surfaces) with those of `flat`, reading only its
  *                              material_count, materials, node_count, nodes, texture_count, textures, texdata_bytes, texdata and
- *                              background.  material_count must be the uploaded count (else CRGPU_ERR_BAD_ARGUMENT): material i of
+ *                              background.  material_count must be the scene's count, as uploaded or as crgpu_scene_add_objects left it (else CRGPU_ERR_BAD_ARGUMENT): material i of
  *                              `flat` becomes material i of the scene, and which material each poly and sphere uses does not change
  *                              (crgpu_scene_set_meshes changes a poly's).  Node count, texture count and texel bytes may grow or
  *                              shrink.  The arrays are validated and folded as crgpu_prepare does it, and a refusal returns the code
  *                              crgpu_prepare returns for them.  Materials, flat records and K4's key order are rewritten in place; the
  *                              nodes, texture table and all texel data are uploaded on every call into a new block that replaces the
  *                              previous edit's (the upload's node and texel sections stay allocated, unread).
+ *   crgpu_scene_add_objects    puts new meshes and spheres into the scene (crLoadMeshFromFile): `flat` is the grown scene B as a whole
+ *                              (the loader places every mesh's materials before the spheres', so adding a mesh moves every sphere's
+ *                              material).  With M meshes, S spheres and P polys in the scene, B's first M meshes and S spheres are the
+ *                              scene's: mesh m < M equals the scene's record in poly_offset, poly_count, material_offset,
+ *                              material_count, texcoord_count and bvh and keeps its current geometry (B's polys, vertices, normals
+ *                              and texcoords for it are not read); sphere s < S keeps its radius bit for bit and takes B's material.
+ *                              Each new mesh's polys lie at or above P inside B's poly_count, apart from every other new mesh's; its
+ *                              indices and poly materials are checked as crgpu_prepare checks them, its material range lies inside
+ *                              B's materials, and its bvh index is below B's bvh_count, is not B's top_bvh and no other mesh's.  From
+ *                              the call on B's BVH indices name the scene's BVH records; B's bvhs, bvh_nodes and prim_indices are not
+ *                              read: each new mesh's tree (the one the scene loader builds), triangles and shading records are built
+ *                              on the device.  New spheres take B's radius and material.  B's materials, nodes, textures, texel data
+ *                              and background replace the scene's as crgpu_scene_set_shading takes them, at B's material count, and
+ *                              B's instance list replaces the scene's as crgpu_scene_set_instance_list takes it; prefs and camera are
+ *                              not read.  When B's first M meshes hold the scene's current geometry the scene then renders, traces and
+ *                              shades the bits of B loaded fresh.  A NULL argument, fewer meshes or spheres than the scene holds, a
+ *                              changed record, a poly range out of bounds or shared, a bad bvh index, an index or material out of range
+ *                              is refused with CRGPU_ERR_BAD_ARGUMENT; a new mesh of more than 4,194,304 polys or a tree deeper than
+ *                              64 levels, more than 2^32 triangle slots, or an instance list set_instance_list refuses with
+ *                              CRGPU_ERR_UNSUPPORTED; shading is refused with the code crgpu_prepare returns.  The triangles, slot
+ *                              records, shading records and BVH records then live in a geometry block that grows by half at least
+ *                              when it is outgrown (new meshes take slots and pair regions behind the existing ones, which never
+ *                              move), the materials in a materials block replaced when B's count outgrows it; the upload's sections
+ *                              stay allocated, unread.  Framebuffers and views are not touched.  Every other edit then works on the
+ *                              grown scene.
  *   crgpu_scene_shading        the live scene's counterpart of crgpu_prepared_materials and crgpu_prepared_background (same kinds and
  *                              flags, read back from the device: min(count, material count) entries), and whether the shading kernels
  *                              run the complete node interpreter.  kinds and flags may be NULL when count is 0, the other outputs
@@ -227,6 +252,7 @@ int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instance *inst, u
 int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count);
 int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *flat, const uint32_t *meshes, uint32_t count);
 int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *flat);
+int crgpu_scene_add_objects(crgpu_scene *s, const struct crs_scene *flat);
 int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32_t count, uint32_t *material_count,
                         uint32_t *background_kind, int *complete_interpreter);
 
@@ -261,7 +287,7 @@ int crgpu_scene_shading(crgpu_scene *s, uint32_t *kinds, uint32_t *flags, uint32
  *   crgpu_view_clear / crgpu_view_read / crgpu_view_to_srgb8
  *                           zero, copy out (W*H*3 floats in the framebuffer layout) or convert to sRGB8 (crgpu_framebuffer_to_srgb8's
  *                           arithmetic and layout, W*H*3 bytes) the whole framebuffer of one view of the list.
- * crgpu_scene_set_instances, _set_instance_list, _set_meshes and _set_shading do not touch the views; every view renders the edited
+ * crgpu_scene_set_instances, _set_instance_list, _set_meshes, _set_shading and _add_objects do not touch the views; every view renders the edited
  * scene. */
 #define CRGPU_MAX_VIEWS 65536u
 int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *cams, uint32_t count);
