@@ -163,6 +163,9 @@ def lib():
             for f in ("crgpu_scene_set_views", "crgpu_scene_view_count", "crgpu_render_views", "crgpu_view_clear", "crgpu_view_read",
                       "crgpu_view_to_srgb8"):
                 getattr(L, f).restype = C.c_int
+        if hasattr(L, "crgpu_scene_set_render"):  # absent from libraries built before render-settings edits
+            L.crgpu_scene_set_render.argtypes = [P] + [C.c_uint32] * 4 + [P, C.c_uint32]
+            L.crgpu_scene_set_render.restype = C.c_int
         _lib = L
     return _lib
 
@@ -332,6 +335,17 @@ class GpuScene:
         becomes the scene camera.  Surviving views keep their framebuffers, new views start zeroed."""
         arr = (Camera * len(cameras))(*cameras)
         _check(lib().crgpu_scene_set_views(self.handle, arr, len(cameras)), "crgpu_scene_set_views")
+
+    def set_render(self, width, height, samples, bounces, cameras=None):
+        """Change image size, sample count and bounce limit (crgpu_scene_set_render): `cameras` is a sequence of Camera of the new
+        size, one per view (the first becomes the scene camera), or None to keep every camera when the size stays.  A new size
+        gives every view a new zeroed framebuffer; an unchanged size touches none."""
+        if cameras is None:
+            arr, n = None, self.view_count()
+        else:
+            arr, n = (Camera * len(cameras))(*cameras), len(cameras)
+        _check(lib().crgpu_scene_set_render(self.handle, width, height, samples, bounces, arr, n), "crgpu_scene_set_render")
+        self.W, self.H, self.samples, self.bounces = width, height, samples, bounces
 
     def view_count(self):
         n = C.c_uint32(0)

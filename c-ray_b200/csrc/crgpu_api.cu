@@ -2413,6 +2413,76 @@ extern "C" int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *ca
 	return publish(s);
 }
 
+/* ---- render settings between renders ---------------------------------------------------------------------------------------------
+ * The kernels read image size, sample count and bounce limit from the descriptor, so publishing it is all they need.  What is sized
+ * from the image is swapped here: view 0's framebuffer and the views block (at the view count, cameras and framebuffers), both new and
+ * zeroed; the sRGB8 staging buffers go back to the cache and are allocated again at the new size when next used. */
+extern "C" int crgpu_scene_set_render(crgpu_scene *s, uint32_t width, uint32_t height, uint32_t sample_count, uint32_t bounces,
+                                      const struct crs_camera *cams, uint32_t count) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	if (width == 0 || height == 0 || sample_count == 0) return fail(CRGPU_ERR_BAD_ARGUMENT, "empty image or zero samples");
+	if (count != s->view_count) return fail(CRGPU_ERR_BAD_ARGUMENT, "%u cameras for a list of %u views", count, s->view_count);
+	const bool resize = width != s->dev.image_width || height != s->dev.image_height;
+	if (!cams && resize) return fail(CRGPU_ERR_BAD_ARGUMENT, "a new image size needs a camera for each view");
+	for (uint32_t i = 0; cams && i < count; ++i)
+		if (cams[i].width != (int32_t)width || cams[i].height != (int32_t)height)
+			return fail(CRGPU_ERR_BAD_ARGUMENT, "camera %u is %dx%d, the settings render %ux%u", i, cams[i].width, cams[i].height, width, height);
+	if ((uint64_t)width * height > SIZE_MAX / (3u * sizeof(float)) / count)
+		return fail(CRGPU_ERR_NOMEM, "%u framebuffers of %ux%u do not fit the address space", count, width, height);
+	int rc = drain(s);
+	if (rc) return rc;
+	const size_t fb_floats = resize ? (size_t)width * height * 3u : s->fb_floats;
+	float *fb = s->fb;
+	DevBlock blk = s->views;
+	uint32_t cap = s->view_cap;
+	if (resize) {                                      /* every new block first: a failed allocation changes nothing */
+		void *q = nullptr;
+		if ((rc = ctx_alloc(s->device, fb_floats * sizeof(float), &q))) return rc;
+		fb = static_cast<float *>(q);
+		cap = count;
+		blk = DevBlock();
+		if (count > 1u) {
+			blk.bytes = views_bytes(cap, fb_floats);
+			if ((rc = ctx_alloc(s->device, blk.bytes, &blk.p))) { ctx_free(s->device, fb, fb_floats * sizeof(float)); return rc; }
+		}
+	}
+	std::vector<DevCamera> dc(cams ? count - 1u : 0u);
+	for (size_t i = 0; i < dc.size(); ++i) dc[i] = dev_camera(cams[i + 1u]);
+	cudaStream_t st = s->stream;
+	cudaError_t ce = cudaSuccess;
+	if (resize) ce = cudaMemsetAsync(fb, 0, fb_floats * sizeof(float), st);
+	if (ce == cudaSuccess && resize && count > 1u) ce = cudaMemsetAsync(views_fb(blk, cap), 0, (size_t)(count - 1u) * fb_floats * sizeof(float), st);
+	if (ce == cudaSuccess && !dc.empty()) ce = cudaMemcpyAsync(blk.p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, st);
+	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+	if (ce != cudaSuccess) {
+		if (resize) { ctx_free(s->device, fb, fb_floats * sizeof(float)); ctx_free(s->device, blk.p, blk.bytes); }
+		return fail(CRGPU_ERR_CUDA, "set_render: %s", cudaGetErrorString(ce));
+	}
+	/* commit */
+	const DevBlock old_views = s->views;
+	float *old_fb = s->fb;
+	uint8_t *old_fb8 = s->fb8, *old_snap8 = s->snap8;
+	const size_t old_floats = s->fb_floats;
+	if (resize) {
+		s->fb = fb; s->fb_floats = fb_floats;
+		s->views = blk; s->view_cap = cap;
+		s->fb8 = s->snap8 = nullptr;
+		unsigned staged = 2u;                          /* an image staged at the old size is dropped; a pending request stays */
+		if (s->stop_host) __atomic_compare_exchange_n(&s->stop_host[3], &staged, 0u, false, __ATOMIC_ACQ_REL, __ATOMIC_ACQUIRE);
+	}
+	s->dev.image_width = width; s->dev.image_height = height;
+	s->dev.sample_count = sample_count; s->dev.bounces = bounces;
+	if (cams) s->dev.cam = dev_camera(cams[0]);
+	rc = publish(s);
+	if (!rc && resize) {                               /* the descriptor and the scene no longer point at them */
+		ctx_free(s->device, old_fb, old_floats * sizeof(float));
+		ctx_free(s->device, old_fb8, old_floats);
+		ctx_free(s->device, old_snap8, old_floats);
+		ctx_free(s->device, old_views.p, old_views.bytes);
+	}
+	return rc;
+}
+
 extern "C" int crgpu_scene_view_count(crgpu_scene *s, uint32_t *count) {
 	if (!s || !count) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	*count = s->view_count;

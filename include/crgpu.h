@@ -298,6 +298,34 @@ int crgpu_view_clear(crgpu_scene *s, uint32_t view);
 int crgpu_view_read(crgpu_scene *s, uint32_t view, float *host_rgb);
 int crgpu_view_to_srgb8(crgpu_scene *s, uint32_t view, uint8_t *host_rgb8);
 
+/* Changing the render settings of a resident scene between renders (c-ray's crSetImageWidth / crSetImageHeight / crSetSampleCount /
+ * crSetBounces, src/c-ray.h:58-74): a viewport resize, a low-sample preview followed by the final render, another bounce limit.
+ *   crgpu_scene_set_render  sets the image size, sample count and bounce limit, and the cameras of the view list.  Like the edits above
+ *                           it first waits for the work queued on the scene's streams and leaves the scene exactly as it was when it
+ *                           fails (framebuffers, views, cameras and snapshot state included).  Afterwards the scene renders, traces and
+ *                           shades (crgpu_render_tile(s), crgpu_render_views, crgpu_trace_kat, crgpu_trace_rays, crgpu_shade_rays) the
+ *                           bits of a fresh scene of its current content, every earlier edit included, given these four settings and
+ *                           these cameras: what crscene_set_config, crgpu_prepare and crgpu_scene_create_prepared would give it.
+ *                           width, height and sample_count of 0 are refused with CRGPU_ERR_BAD_ARGUMENT, as crgpu_prepare refuses them;
+ *                           every bounce limit crgpu_prepare takes is taken, 0 included (every sample is then black).  `count` must be
+ *                           crgpu_scene_view_count and every camera width x height: cams[0] becomes the scene camera and cams[v] the
+ *                           camera of view v, taken bit for bit.  cams may be NULL only when width and height are the scene's: every
+ *                           camera is then kept.  Any other NULL, another count or a camera of another size is refused with
+ *                           CRGPU_ERR_BAD_ARGUMENT; the view list keeps its length (crgpu_scene_set_views changes it).
+ *                           With the image size unchanged no framebuffer is touched, as with every other edit.  A new size gives view
+ *                           0 and each other view a new framebuffer of that size, zeroed, and the views block room for the current
+ *                           view count only.  All new blocks are allocated first (a failure returns CRGPU_ERR_NOMEM and changes
+ *                           nothing), the scene is published, and only then the old blocks go back to the per-device cache: a pointer
+ *                           crgpu_framebuffer_device_ptr gave before a size change is dead afterwards, so a host that holds one (the
+ *                           NCCL gather) asks again.  The sRGB8 staging buffers of crgpu_framebuffer_to_srgb8 and of snapshots go back
+ *                           to the cache too and are allocated again at the new size when next used: an image staged before the size
+ *                           change is dropped, while a pending request stays pending and is served at the new size.  An armed scene
+ *                           stays armed, with its stop word and progress as they were.  The paths-in-flight budget is not changed.
+ *                           crgpu_scene_info, every rectangle check, the framebuffer and view accessors and snapshots use the new size;
+ *                           a cached tile set is checked against it before it is used again. */
+int crgpu_scene_set_render(crgpu_scene *s, uint32_t width, uint32_t height, uint32_t sample_count, uint32_t bounces,
+                           const struct crs_camera *cams, uint32_t count);
+
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
  * use) order the kernels with its own work and time them with its own events.  crgpu_use_own_stream goes
@@ -315,7 +343,8 @@ int crgpu_framebuffer_read(crgpu_scene *s, float *host_rgb, int x0, int y0, int 
 int crgpu_framebuffer_write(crgpu_scene *s, const float *host_rgb, int x0, int y0, int x1, int y1);
 /* 8-bit sRGB image of the current framebuffer (renderer.c:297-300), W*H*3 bytes, same row order. */
 int crgpu_framebuffer_to_srgb8(crgpu_scene *s, uint8_t *host_rgb8);
-/* Raw device pointer of the fp32 framebuffer (for the NCCL gather done by the multi-GPU host). */
+/* Raw device pointer of the fp32 framebuffer (for the NCCL gather done by the multi-GPU host).  A size change by
+ * crgpu_scene_set_render replaces the framebuffer: the pointer given before it is dead afterwards. */
 int crgpu_framebuffer_device_ptr(crgpu_scene *s, void **dev_ptr, size_t *bytes);
 /* Device ordinal and image size of a scene (any pointer may be NULL). */
 int crgpu_scene_info(crgpu_scene *s, int *device, int *width, int *height);
