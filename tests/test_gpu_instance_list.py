@@ -87,12 +87,13 @@ def check_list(g, doc_b, cfg=GEN, rays=None):
         b.free()
 
 
-def duplicated(doc, name):
-    """a second instance of DUP[name]'s mesh, moved by STEP[name] * 5"""
+def duplicated(doc, name, file=None, step=None):
+    """a second instance of DUP[name]'s mesh (or of the first instance of mesh file `file`), moved by STEP[name] * 5 (or `step`)"""
     d = copy.deepcopy(doc)
-    mesh = next(m for m in d["scene"]["meshes"] if m["fileName"] == DUP[name])
+    mesh = next(m for m in d["scene"]["meshes"] if m["fileName"] == (file or DUP[name]) and m.get("instances"))
     extra = copy.deepcopy(mesh["instances"][0])
-    s = STEP[name] * 5
+    extra.setdefault("transforms", [])
+    s = STEP[name] * 5 if step is None else step
     extra["transforms"].append({"type": "translate", "x": s, "y": 0.0, "z": -s})
     mesh["instances"].append(extra)
     return d

@@ -506,9 +506,10 @@ def test_refused_edits_leave_the_scene_unchanged():
 
 # ---- GPU: bundled scenes ---------------------------------------------------------------------------------------------------------
 
-def recolour_doc(name):
-    """The bundled scene's JSON with other materials and, for hdr, the other HDR environment at another offset."""
-    d = copy.deepcopy(scene_json(name))
+def recolour_doc(name, doc=None):
+    """The bundled scene's JSON (or `doc`, an edited copy of it) with other materials and, for hdr, the other HDR environment at
+    another offset."""
+    d = copy.deepcopy(scene_json(name) if doc is None else doc)
     s = d["scene"]
     if name == "hdr":
         s["ambientColor"]["hdr"] = "HDRs/rooitou_park_1k.hdr"

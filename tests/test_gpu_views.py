@@ -112,9 +112,9 @@ def scene_camera(path, W, H):
 
 def cameras(name, g, n):
     """View 0: the scene's camera; view k >= 1: the JSON camera moved by k steps and turned by 2k degrees, view 1 also with
-    another aperture and focal distance."""
-    doc = scene_doc(name)
-    step = STEP.get(name, 0.05)
+    another aperture and focal distance.  `name` is a scene's name or its JSON document."""
+    doc = scene_doc(name) if isinstance(name, str) else name
+    step = STEP.get(name, 0.05) if isinstance(name, str) else 0.05
     out = [crgpu.Camera.from_buffer_copy(g.camera)]
     for k in range(1, n):
         cam = copy.deepcopy(doc["camera"])
