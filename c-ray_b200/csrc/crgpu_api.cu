@@ -18,6 +18,8 @@
 #include <vector>
 #include <algorithm>
 #include <queue>
+#include <deque>
+#include <utility>
 #include <thread>
 #include <mutex>
 
@@ -58,17 +60,17 @@ extern "C" int crgpu_device_count(int *n) {
  * back to a per-device cache and the next scene on that device takes it from there (best fit within 2x); a cudaMalloc that
  * fails trims the cache and retries.  crgpu_device_trim() hands everything back to the driver. */
 #define CRG_MAX_DEVICES 64
-struct DevBlock { void *p = nullptr; size_t bytes = 0; };
+struct Cached { void *p; size_t bytes; };
 struct DevCtx {
 	std::mutex lock;
-	std::vector<DevBlock> cache;
+	std::vector<Cached> cache;
 	size_t cached = 0;
 };
 static DevCtx g_ctx[CRG_MAX_DEVICES];
 static DevCtx &ctx_of(int dev) { return g_ctx[dev >= 0 && dev < CRG_MAX_DEVICES ? dev : 0]; }
 
 static void ctx_trim_locked(DevCtx &c) {
-	for (DevBlock &b : c.cache) cudaFree(b.p);
+	for (Cached &b : c.cache) cudaFree(b.p);
 	c.cache.clear();
 	c.cached = 0;
 }
@@ -115,6 +117,30 @@ static void ctx_free(int dev, void *p, size_t bytes) {
 	c.cached += bytes;
 }
 static size_t ctx_cached_bytes(int dev) { DevCtx &c = ctx_of(dev); std::lock_guard<std::mutex> g(c.lock); return c.cached; }
+
+/* One allocation from the per-device cache, which it goes back to when the owner is destroyed, overwritten or released. */
+struct DevBlock {
+	int dev = 0;
+	void *p = nullptr;
+	size_t bytes = 0;
+	DevBlock() = default;
+	DevBlock(DevBlock &&o) noexcept : dev(o.dev), p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+	DevBlock &operator=(DevBlock &&o) noexcept {
+		if (this != &o) { release(); dev = o.dev; p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
+		return *this;
+	}
+	~DevBlock() { release(); }
+	void release() { ctx_free(dev, p, bytes); p = nullptr; bytes = 0; }
+	/* releases the block it holds, then takes one of `n` bytes on `device` (the calling thread's current device); empty on failure */
+	int alloc(int device, size_t n) {
+		release();
+		dev = device;
+		int rc = ctx_alloc(device, n, &p);
+		if (!rc) bytes = n;
+		return rc;
+	}
+	template <class T> T *as() const { return static_cast<T *>(p); }
+};
 
 extern "C" int crgpu_device_trim(int device) {
 	int ndev = 0;
@@ -196,29 +222,28 @@ struct crgpu_scene {
 	float pend_trace_ms = 0.f, pend_shade_ms = 0.f, pend_total_ms = 0.f;
 	DevScene dev = {};
 	DevScene *dev_copy = nullptr;    /* the same descriptor in HBM, for kernels that call noinline device functions */
-	void *slab = nullptr; size_t slab_bytes = 0;     /* the scene arrays + dev_copy */
-	void *small = nullptr; size_t small_bytes = 0;   /* hist, counts, stats */
-	float *fb = nullptr;             /* W*H*3 fp32, row H-1-y */
-	uint8_t *fb8 = nullptr;          /* lazily allocated sRGB8 staging */
+	DevBlock slab;                   /* the scene arrays + dev_copy */
+	DevBlock small;                  /* hist, counts, stats */
+	DevBlock fb;                     /* W*H*3 fp32, row H-1-y */
+	DevBlock fb8;                    /* sRGB8 staging, allocated when first used (alloc_srgb8) */
 	size_t fb_floats = 0;
 	uint64_t max_paths = 0;
 	uint64_t cap_paths = 0;          /* capacity of the wavefront buffers */
-	void *wave = nullptr; size_t wave_bytes = 0;
+	DevBlock wave;
 	int wave_sets = 0;               /* 1, or 2 when batches are overlapped on two streams (each set holds cap_paths paths) */
 	WaveBuffers wb = {};             /* set 0 */
 	WaveBuffers wb2 = {};            /* set 1: own ray / hit / radiance buffers and own hist + counts; stats shared */
 	cudaStream_t stream2 = nullptr;  /* the second stream of overlapped batches */
 	cudaEvent_t ev[4] = {};
 	cudaEvent_t evAcc[2] = {}, evFork = nullptr;   /* accumulate-order chain between the two streams */
-	uint32_t *pixels = nullptr;      /* device pixel list of the last crgpu_render_tiles tile set */
-	size_t pixel_cap = 0;
+	DevBlock pixels;                 /* device pixel list of the last crgpu_render_tiles tile set */
 	std::vector<int> pixel_key;
 	bool armed = false;              /* crgpu_stop_enable: render calls run the stop gates and the ordered commit */
 	unsigned *stop_host = nullptr;   /* pinned, mapped: [0] stop request, [1] committed pass index, [2] a call is in flight, [3] snapshot
 	                                    state (0 idle, 1 requested, 2 staged), [4] its pass index (NULL until armed once) */
 	unsigned *stop_ctl = nullptr;    /* device: [0] pass index the running average has reached, [1], [2] abandoned flags of the wave sets,
 	                                    [3] the next publish step stages a snapshot, [4] its block count (crgpu_wave.cuh) */
-	uint8_t *snap8 = nullptr;        /* W*H*3 sRGB8 snapshot staged by a publish step (allocated by the first armed call) */
+	DevBlock snap8;                  /* W*H*3 sRGB8 snapshot staged by a publish step (allocated by the first armed call) */
 	cudaStream_t snap_stream = nullptr;   /* crgpu_take_snapshot's copies: never behind the render (created when first armed) */
 	/* scene edits */
 	EditRecord rec;                  /* crgpu_prepared::rec */
@@ -257,6 +282,9 @@ static int publish(crgpu_scene *s) {
 	CU(cudaStreamSynchronize(s->stream));
 	return CRGPU_OK;
 }
+
+/* fb8 or snap8, an sRGB8 staging buffer of the image, when first used */
+static int alloc_srgb8(crgpu_scene *s, DevBlock &b) { return b.p ? CRGPU_OK : b.alloc(s->device, s->fb_floats); }
 
 /* ---- node graph checks -------------------------------------------------------------------------------------- */
 static bool node_ok(const crs_scene *f, int idx) { return idx >= 0 && (uint32_t)idx < f->node_count; }
@@ -716,22 +744,18 @@ static DevCamera dev_camera(const crs_camera &c) {
 /* all wavefront buffers of a scene are carved from ONE device block (one cudaMalloc / one cache hit per frame) */
 static int alloc_wave(crgpu_scene *s, uint64_t paths, int sets) {
 	if (paths <= s->cap_paths && sets <= s->wave_sets) return CRGPU_OK;
-	if (s->wave) {
+	if (s->wave.p) {
 		cudaStreamSynchronize(s->stream);                           /* queued kernels may still use the old block */
 		if (s->stream2) cudaStreamSynchronize(s->stream2);
-		ctx_free(s->device, s->wave, s->wave_bytes);
 	}
-	s->wave = nullptr; s->wave_bytes = 0; s->cap_paths = 0; s->wave_sets = 0;
+	s->cap_paths = 0; s->wave_sets = 0;
 	const size_t n = ((size_t)paths + 255u) & ~(size_t)255u;      /* every sub-array stays 256-byte aligned */
 	const size_t per_set = n * (9u * 16u + 2u * 4u + 1u);         /* 153 B per path */
-	const size_t bytes = per_set * (size_t)sets;
-	void *base = nullptr;
-	int rc = ctx_alloc(s->device, bytes, &base);
+	int rc = s->wave.alloc(s->device, per_set * (size_t)sets);
 	if (rc) return rc;
-	s->wave = base; s->wave_bytes = bytes;
 	for (int k = 0; k < sets; ++k) {
 		WaveBuffers &w = k ? s->wb2 : s->wb;
-		uint8_t *q = static_cast<uint8_t *>(base) + per_set * (size_t)k;
+		uint8_t *q = s->wave.as<uint8_t>() + per_set * (size_t)k;
 		auto take = [&](size_t b) { uint8_t *r = q; q += b; return r; };
 		w.stA[0] = (float4 *)take(n * 16); w.stA[1] = (float4 *)take(n * 16);
 		w.stB[0] = (float4 *)take(n * 16); w.stB[1] = (float4 *)take(n * 16);
@@ -752,14 +776,6 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	if (s->stream) cudaStreamSynchronize(s->stream);
 	if (s->own_stream && s->own_stream != s->stream) cudaStreamSynchronize(s->own_stream);
 	if (s->stream2) cudaStreamSynchronize(s->stream2);
-	ctx_free(s->device, s->slab, s->slab_bytes);
-	ctx_free(s->device, s->wave, s->wave_bytes);
-	ctx_free(s->device, s->small, s->small_bytes);
-	ctx_free(s->device, s->fb, s->fb_floats * sizeof(float));
-	ctx_free(s->device, s->fb8, s->fb_floats);
-	ctx_free(s->device, s->snap8, s->fb_floats);
-	ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
-	for (DevBlock *b : { &s->pairs, &s->insts, &s->scratch, &s->shade, &s->views, &s->geom, &s->mats }) ctx_free(s->device, b->p, b->bytes);
 	for (cudaEvent_t e : s->ev) if (e) cudaEventDestroy(e);
 	for (cudaEvent_t e : s->evAcc) if (e) cudaEventDestroy(e);
 	if (s->evFork) cudaEventDestroy(s->evFork);
@@ -767,7 +783,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	if (s->own_stream) cudaStreamDestroy(s->own_stream);
 	if (s->snap_stream) cudaStreamDestroy(s->snap_stream);
 	if (s->stop_host) cudaFreeHost(s->stop_host);
-	delete s;
+	delete s;                                        /* its blocks go back to the per-device cache */
 	return CRGPU_OK;
 }
 
@@ -1101,9 +1117,8 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	CUS(cudaEventCreateWithFlags(&s->evFork, cudaEventDisableTiming));
 
 	/* the scene: one block, one copy */
-	FAIL_IF(ctx_alloc(device, p->slab_bytes, &s->slab));
-	s->slab_bytes = p->slab_bytes;
-	uint8_t *base = static_cast<uint8_t *>(s->slab);
+	FAIL_IF(s->slab.alloc(device, p->slab_bytes));
+	uint8_t *base = s->slab.as<uint8_t>();
 	CUS(cudaMemcpyAsync(base, p->slab, p->slab_bytes, cudaMemcpyHostToDevice, s->stream));
 	if (p->texture_count) {                 /* texture table with this device's addresses */
 		std::vector<DevTexture> texs(p->texture_count);
@@ -1143,14 +1158,13 @@ extern "C" int crgpu_scene_create_prepared(const crgpu_prepared *p, int device, 
 	s->dev_copy = reinterpret_cast<DevScene *>(base + p->slab_bytes - 512);
 
 	s->fb_floats = (size_t)d.image_width * d.image_height * 3u;
-	{ void *q = nullptr; FAIL_IF(ctx_alloc(device, s->fb_floats * sizeof(float), &q)); s->fb = static_cast<float *>(q); }
-	CUS(cudaMemsetAsync(s->fb, 0, s->fb_floats * sizeof(float), s->stream));
+	FAIL_IF(s->fb.alloc(device, s->fb_floats * sizeof(float)));
+	CUS(cudaMemsetAsync(s->fb.p, 0, s->fb.bytes, s->stream));
 	{	/* per wave set: hist[1024] + counts[64] + box[CRG_BOX_SLOTS][12]; then the shared stats[80] and the stop words[16] */
 		const size_t set_bytes = 1024 * sizeof(unsigned) + 256 + CRG_BOX_SLOTS * 12 * sizeof(unsigned);
-		s->small_bytes = 2 * set_bytes + 80 * sizeof(unsigned long long) + 16 * sizeof(unsigned);
-		FAIL_IF(ctx_alloc(device, s->small_bytes, &s->small));
-		CUS(cudaMemsetAsync(s->small, 0, s->small_bytes, s->stream));
-		uint8_t *sm = static_cast<uint8_t *>(s->small);
+		FAIL_IF(s->small.alloc(device, 2 * set_bytes + 80 * sizeof(unsigned long long) + 16 * sizeof(unsigned)));
+		CUS(cudaMemsetAsync(s->small.p, 0, s->small.bytes, s->stream));
+		uint8_t *sm = s->small.as<uint8_t>();
 		s->wb.hist = reinterpret_cast<unsigned *>(sm);
 		s->wb.counts = s->wb.hist + 1024;
 		s->wb.box = s->wb.hist + 1024 + 64;
@@ -1348,11 +1362,11 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 			cur ^= 1;
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
-		crg_launch_accumulate(s->fb, wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set,
+		crg_launch_accumulate(s->fb.as<float>(), wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set,
 		                      armed && gates.publish ? s->stop_host : nullptr, vd); ++launches;
 		if (armed && gates.publish) {       /* stages a snapshot when K5 found one requested (crgpu_request_snapshot) */
 			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats,
-			                        s->fb, s->snap8, s->fb_floats, s->sm_count * 4, st);
+			                        s->fb.as<float>(), s->snap8.as<uint8_t>(), s->fb_floats, s->sm_count * 4, st);
 			++launches;
 		}
 		if (sets == 2) CU(cudaEventRecord(s->evAcc[set], st));      /* after the publish step: the next K5 reads what it wrote */
@@ -1413,12 +1427,10 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
 	const bool armed = s->armed;
-	if (armed && !s->snap8) {
+	if (armed && !s->snap8.p) {
 		CU(cudaSetDevice(s->device));
-		void *q = nullptr;
-		int arc = ctx_alloc(s->device, s->fb_floats, &q);
+		int arc = alloc_srgb8(s, s->snap8);
 		if (arc) return arc;
-		s->snap8 = static_cast<uint8_t *>(q);
 	}
 	if (armed) {
 		__atomic_store_n(&s->stop_host[1], (unsigned)pass_begin, __ATOMIC_RELEASE);
@@ -1520,22 +1532,63 @@ extern "C" int crgpu_take_snapshot(crgpu_scene *s, uint8_t *host_rgb8, int *pass
 		__atomic_store_n(&w[3], 0u, __ATOMIC_RELEASE);
 		return CRGPU_OK;
 	}
-	CU(cudaMemcpyAsync(host_rgb8, s->snap8, s->fb_floats, cudaMemcpyDeviceToHost, s->snap_stream));
+	CU(cudaMemcpyAsync(host_rgb8, s->snap8.p, s->fb_floats, cudaMemcpyDeviceToHost, s->snap_stream));
 	CU(cudaStreamSynchronize(s->snap_stream));
 	if (passes_done) *passes_done = (int)__atomic_load_n(&w[4], __ATOMIC_ACQUIRE);
 	__atomic_store_n(&w[3], 0u, __ATOMIC_RELEASE);
 	return CRGPU_OK;
 }
 
-/* ---- scene edits between renders -------------------------------------------------------------------------------------------------- */
+/* ---- scene edits between renders --------------------------------------------------------------------------------------------------
+ * One edit call's change to the scene (DESIGN §4 "Editing a resident scene"): a copy of the descriptor to edit, the blocks the call
+ * has staged, each bound for the scene member it replaces, and the layout of the pairs and instance blocks after the call.  apply()
+ * moves the staged blocks in, publishes the descriptor once and only then lets the replaced blocks go back to the per-device cache.
+ * A call that returns before apply() releases what it staged and leaves the scene as it was. */
+struct Edit {
+	crgpu_scene *s;
+	DevScene dev;
+	uint32_t pair_cap, top_off, top_cap;     /* crgpu_scene's, after the call */
+	InstParts ip;
+	uint32_t inst_cap;
+	struct Staged { DevBlock *dst; DevBlock blk; };
+	std::deque<Staged> staged;               /* a deque: stage() hands out references that later stages keep valid */
+	explicit Edit(crgpu_scene *sc)
+		: s(sc), dev(sc->dev), pair_cap(sc->pair_cap), top_off(sc->top_off), top_cap(sc->top_cap), ip(sc->ip), inst_cap(sc->inst_cap) {}
+	/* the empty block that replaces dst at apply(); staging dst again releases the block staged before */
+	DevBlock &stage(DevBlock &dst) {
+		for (Staged &b : staged) if (b.dst == &dst) { b.blk.release(); return b.blk; }
+		staged.push_back({ &dst, DevBlock() });
+		return staged.back().blk;
+	}
+	/* what dst holds after apply() */
+	const DevBlock &next(const DevBlock &dst) const {
+		for (const Staged &b : staged) if (b.dst == &dst) return b.blk;
+		return dst;
+	}
+	int apply() {
+		for (Staged &b : staged) std::swap(*b.dst, b.blk);
+		std::swap(s->dev, dev);
+		const int rc = publish(s);
+		if (rc) {                                /* the scene keeps its blocks and descriptor */
+			for (Staged &b : staged) std::swap(*b.dst, b.blk);
+			std::swap(s->dev, dev);
+			return rc;
+		}
+		s->pair_cap = pair_cap; s->top_off = top_off; s->top_cap = top_cap;
+		s->ip = ip; s->inst_cap = inst_cap;
+		return CRGPU_OK;                         /* the replaced blocks, now in `staged`, go when the edit does */
+	}
+};
+
 extern "C" int crgpu_scene_set_camera(crgpu_scene *s, const struct crs_camera *cam) {
 	if (!s || !cam) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
 	if (cam->width != (int32_t)s->dev.image_width || cam->height != (int32_t)s->dev.image_height)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "camera is %dx%d, the scene renders %ux%u", cam->width, cam->height, s->dev.image_width, s->dev.image_height);
 	int rc = drain(s);
 	if (rc) return rc;
-	s->dev.cam = dev_camera(*cam);
-	return publish(s);
+	Edit e(s);
+	e.dev.cam = dev_camera(*cam);
+	return e.apply();
 }
 
 static size_t align256(size_t b) { return (b + 255u) & ~(size_t)255u; }
@@ -1556,11 +1609,8 @@ template <class F> static int carve(int device, DevBlock &blk, F layout) {
 	Carve c = { 0, 0 };
 	layout(c);
 	if (c.bytes > blk.bytes) {
-		ctx_free(device, blk.p, blk.bytes);
-		blk = DevBlock();
-		int rc = ctx_alloc(device, c.bytes, &blk.p);
+		int rc = blk.alloc(device, c.bytes);
 		if (rc) return rc;
-		blk.bytes = c.bytes;
 	}
 	c = { reinterpret_cast<uintptr_t>(blk.p), 0 };
 	layout(c);
@@ -1569,7 +1619,7 @@ template <class F> static int carve(int device, DevBlock &blk, F layout) {
 
 /* The top-level build's part of an edit call's scratch: the BVH roots it reads, the instance boxes, centres and ray offsets, the new
  * instance records, and the new top level's pairs and primitive order, for n instances.  A list edit also stages its last-instance
- * table and instance keys there; the other edits read the instance block's table. */
+ * table and instance keys there; the other edits point `last` at the instance block's table. */
 struct TopParts {
 	float *roots, *bb, *ctr, *offs;
 	DevInstance *insts;
@@ -1614,52 +1664,40 @@ static DevBvh bvh_record(const CrgBuildResult &res, uint32_t pair_offset, uint32
 	return b;
 }
 
-/* Gives the scene a pairs block of `count` pair nodes that starts with a copy of the live ones (the uploaded pairs until the first
- * geometry edit; unedited meshes' pair offsets do not move) and swaps it in.  The block it replaces goes back to the per-device cache
- * after the publish that stops the descriptor from pointing at it. */
-static int reserve_pairs(crgpu_scene *s, uint32_t count) {
+/* Stages a pairs block of `count` pair nodes that starts with a copy of the edit's current ones (the uploaded pairs until the first
+ * geometry edit; unedited meshes' pair offsets do not move). */
+static int reserve_pairs(Edit &e, uint32_t count) {
 	DevBlock blk;
-	int rc = ctx_alloc(s->device, (size_t)count * sizeof(PairNode), &blk.p);
+	int rc = blk.alloc(e.s->device, (size_t)count * sizeof(PairNode));
 	if (rc) return rc;
-	blk.bytes = (size_t)count * sizeof(PairNode);
-	cudaError_t ce = cudaMemcpyAsync(blk.p, s->dev.pairs, (size_t)s->pair_cap * sizeof(PairNode), cudaMemcpyDeviceToDevice, s->stream);
-	if (ce != cudaSuccess) { ctx_free(s->device, blk.p, blk.bytes); return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce)); }
-	const DevBlock old = s->pairs;
-	s->pairs = blk;
-	s->pair_cap = count;
-	s->dev.pairs = static_cast<const PairNode *>(blk.p);
-	rc = publish(s);
-	if (!rc) ctx_free(s->device, old.p, old.bytes);
-	return rc;
+	CU(cudaMemcpyAsync(blk.p, e.dev.pairs, (size_t)e.pair_cap * sizeof(PairNode), cudaMemcpyDeviceToDevice, e.s->stream));
+	e.dev.pairs = blk.as<const PairNode>();
+	e.pair_cap = count;
+	e.stage(e.s->pairs) = std::move(blk);
+	return CRGPU_OK;
 }
 
-/* The first instance or mesh edit of a scene with instances gives it its instance block for the uploaded list: EditRecord::last,
- * then room for the top level's item records.  The slab's instance records and keys stay in use until a list edit. */
-static int alloc_insts(crgpu_scene *s) {
+/* The first instance or mesh edit of a scene with instances stages its instance block for the uploaded list: EditRecord::last, then
+ * room for the top level's item records.  The slab's instance records and keys stay in use until a list edit. */
+static int stage_insts(Edit &e) {
+	crgpu_scene *s = e.s;
 	if (s->insts.p) return CRGPU_OK;
 	const uint32_t n = (uint32_t)s->rec.last.size();
-	InstParts q = {};
-	int rc = carve(s->device, s->insts, [&](Carve &c) { q = take_insts(c, n, false); });
+	int rc = carve(s->device, e.stage(s->insts), [&](Carve &c) { e.ip = take_insts(c, n, false); });
 	if (rc) return rc;
-	cudaError_t ce = cudaMemcpyAsync(q.last, s->rec.last.data(), (size_t)n * 4u, cudaMemcpyHostToDevice, s->stream);
-	if (ce != cudaSuccess) {
-		ctx_free(s->device, s->insts.p, s->insts.bytes);
-		s->insts = DevBlock();
-		return fail(CRGPU_ERR_CUDA, "scene edit: %s", cudaGetErrorString(ce));
-	}
-	s->ip = q;
-	s->inst_cap = n;
+	CU(cudaMemcpyAsync(e.ip.last, s->rec.last.data(), (size_t)n * 4u, cudaMemcpyHostToDevice, s->stream));
+	e.inst_cap = n;
 	return CRGPU_OK;
 }
 
 /* Instance boxes, ray offsets and the top-level BVH of n instances into the scratch parts t, mesh boxes from t.roots.  The records
  * start from `from` (the scene's current ones), or from what t.insts already holds when it is NULL; A and Ainv from inst (device)
- * when it is not NULL.  The offsets follow t.last, or the instance block's table when it is NULL. */
+ * when it is not NULL.  The offsets follow t.last. */
 static int build_top(crgpu_scene *s, uint32_t n, const DevInstance *from, const crs_instance *inst, const TopParts &t, void *build,
                      CrgBuildResult *res) {
 	cudaStream_t st = s->stream;
 	if (from && n) CU(cudaMemcpyAsync(t.insts, from, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
-	crg_launch_instance_boxes(inst, t.insts, t.roots, t.last ? t.last : s->ip.last, n, t.bb, t.ctr, t.offs, st);
+	crg_launch_instance_boxes(inst, t.insts, t.roots, t.last, n, t.bb, t.ctr, t.offs, st);
 	CU(cudaGetLastError());
 	int rc = crg_bvh_build_pairs(t.bb, t.ctr, n, build, st, t.pairs, t.prims, res);
 	if (rc) return rc;
@@ -1667,22 +1705,22 @@ static int build_top(crgpu_scene *s, uint32_t n, const DevInstance *from, const 
 	return CRGPU_OK;
 }
 
-/* Copies a built top level of n instances over the scene's instance records, top region, item records and staged prefix, and
- * publishes the descriptor.  The BVH records the items read, the instance block and the top region must already be committed. */
-static int commit_top(crgpu_scene *s, uint32_t n, const TopParts &t, const CrgBuildResult &res) {
-	cudaStream_t st = s->stream;
-	const DevBvh top = bvh_record(res, s->top_off, 0u, s->dev.top.stage_base, s->top_stage_cap);
-	if (n) CU(cudaMemcpyAsync(const_cast<DevInstance *>(s->dev.instances), t.insts, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
-	if (res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + top.pair_offset, t.pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	crg_launch_top_items(t.prims, t.insts, s->dev.bvhs, n, s->ip.items, st);
+/* Copies a built top level of n instances over the edit's instance records, top region, item records and staged prefix, and points
+ * its descriptor at them.  The BVH records the items read, the instance block and the top region must already be in place. */
+static int commit_top(Edit &e, uint32_t n, const TopParts &t, const CrgBuildResult &res) {
+	cudaStream_t st = e.s->stream;
+	const DevBvh top = bvh_record(res, e.top_off, 0u, e.dev.top.stage_base, e.s->top_stage_cap);
+	if (n) CU(cudaMemcpyAsync(const_cast<DevInstance *>(e.dev.instances), t.insts, (size_t)n * sizeof(DevInstance), cudaMemcpyDeviceToDevice, st));
+	if (res.pairs) CU(cudaMemcpyAsync(const_cast<PairNode *>(e.dev.pairs) + top.pair_offset, t.pairs, (size_t)res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	crg_launch_top_items(t.prims, t.insts, e.dev.bvhs, n, e.ip.items, st);
 	CU(cudaGetLastError());
 	if (top.stage_count)
-		CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + top.stage_base, t.pairs, (size_t)top.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
-	s->dev.top = top;
-	s->dev.top_items = s->ip.items;
+		CU(cudaMemcpyAsync(const_cast<PairNode *>(e.dev.stage_img) + top.stage_base, t.pairs, (size_t)top.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+	e.dev.top = top;
+	e.dev.top_items = e.ip.items;
 	static const float unit[6] = { 0.f, 1.f, 0.f, 1.f, 0.f, 1.f };  /* crgpu_prepare's box of an empty top level */
-	world_box(res.node_count ? res.bounds : unit, s->dev.world_lo, s->dev.world_inv);
-	return publish(s);
+	world_box(res.node_count ? res.bounds : unit, e.dev.world_lo, e.dev.world_inv);
+	return CRGPU_OK;
 }
 
 /* Instance boxes, ray offsets and the top-level BVH of the edited instances are computed on the device, into scratch; only once the
@@ -1698,28 +1736,31 @@ extern "C" int crgpu_scene_set_instances(crgpu_scene *s, const struct crs_instan
 	int rc = drain(s);
 	if (rc) return rc;
 	if (n == 0) return CRGPU_OK;
+	Edit e(s);
 	crs_instance *dinst = nullptr;
 	TopParts t;
 	void *build = nullptr;
 	rc = carve(s->device, s->scratch, [&](Carve &c) { dinst = c.take<crs_instance>(n); t = take_top(c, s->rec.bvh_root.size(), n); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
-	if (!rc) rc = alloc_insts(s);
+	if (!rc) rc = stage_insts(e);
 	if (rc) return rc;
+	t.last = e.ip.last;
 	/* the roots in a copy of their own: packing them behind the caller's instances would cost a host copy of every instance */
 	CU(cudaMemcpyAsync(dinst, inst, (size_t)n * sizeof(crs_instance), cudaMemcpyHostToDevice, s->stream));
 	CU(cudaMemcpyAsync(t.roots, s->rec.bvh_root.data(), s->rec.bvh_root.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
 	CrgBuildResult res;
 	rc = build_top(s, n, s->dev.instances, dinst, t, build, &res);
-	if (!rc && !s->pairs.p) rc = reserve_pairs(s, s->top_off + s->top_cap);
-	if (rc) return rc;
-	return commit_top(s, n, t, res);
+	if (!rc && !s->pairs.p) rc = reserve_pairs(e, s->top_off + s->top_cap);
+	if (!rc) rc = commit_top(e, n, t, res);
+	if (!rc) rc = e.apply();
+	return rc;
 }
 
 /* ---- instance-list edits ------------------------------------------------------------------------------------------------------------
  * The new list is validated and packed on the host (pack_instances, as crgpu_prepare packs it), and its boxes, ray offsets and top level
- * are built on the device into scratch (stage_list).  Only once the build has passed the upload's checks do the blocks change
- * (commit_list): the pairs block grows when the top region cannot hold a top level of the new count, and the instance block is replaced
+ * are built on the device into scratch (stage_list).  Only once the build has passed the upload's checks are the blocks staged
+ * (grow_list): the pairs block grows when the top region cannot hold a top level of the new count, and the instance block is replaced
  * when it has no records of its own or no room for the new count.  Then the records, keys, last table, top region, item records and
- * staged prefix are committed and published, and the replaced instance block goes back to the per-device cache. */
+ * staged prefix are written (commit_list). */
 
 /* Uploads the packed list of n instances and the BVH roots (6 floats per BVH) into the scratch parts t (take_top with `list`) and builds
  * their boxes, ray offsets and top level there.  Changes nothing the kernels read. */
@@ -1735,65 +1776,56 @@ static int stage_list(crgpu_scene *s, const InstancePack &pk, uint32_t n, const 
 	return build_top(s, n, nullptr, nullptr, t, build, res);
 }
 
-/* Makes a staged list of n instances (kinds and objects from inst) the scene's: grows the top region and the instance block as needed,
- * runs before_commit (the caller's own commits, which the item records may read), then commits the list and the top level and
- * publishes the descriptor. */
-template <class F>
-static int commit_list(crgpu_scene *s, const crs_instance *inst, uint32_t n, const InstancePack &pk, const TopParts &t, const CrgBuildResult &res,
-                       F before_commit) {
+/* Stages the top region and instance block a list of n instances needs. */
+static int grow_list(Edit &e, uint32_t n) {
+	crgpu_scene *s = e.s;
 	/* the top region: the current one while it holds any top level of n instances (region_pairs(n)), else a new one behind every pair
 	 * of the block; mesh regions never move.  A region that has to move grows by half at least, so that adding instances a few at a
 	 * time does not leave a trail of abandoned regions. */
-	uint32_t top_off = s->top_off, top_cap = s->top_cap;
-	if (region_pairs(n) > top_cap) {
-		const uint64_t want = (uint64_t)top_cap + top_cap / 2u;
-		top_cap = want > region_pairs(n) ? (uint32_t)want : region_pairs(n);
-		if (s->pairs.p) top_off = s->pair_cap;            /* before the first geometry edit the reserved region is simply larger */
+	const bool block = e.next(s->pairs).p != nullptr;
+	if (region_pairs(n) > e.top_cap) {
+		const uint64_t want = (uint64_t)e.top_cap + e.top_cap / 2u;
+		e.top_cap = want > region_pairs(n) ? (uint32_t)want : region_pairs(n);
+		if (block) e.top_off = e.pair_cap;                /* before the first geometry edit the reserved region is simply larger */
 	}
-	const uint64_t need = (uint64_t)top_off + top_cap;
+	const uint64_t need = (uint64_t)e.top_off + e.top_cap;
 	if (need > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "instance list: more pair nodes than the scene can address");
 	int rc;
-	if (!s->pairs.p || need > s->pair_cap) {
-		rc = reserve_pairs(s, (uint32_t)(need > s->pair_cap ? need : s->pair_cap));
+	if (!block || need > e.pair_cap) {
+		rc = reserve_pairs(e, (uint32_t)(need > e.pair_cap ? need : e.pair_cap));
 		if (rc) return rc;
 	}
 	/* the instance block: kept while it has records of its own and room for n, else a new one (growing by half at least) */
-	DevBlock old;
-	if (!s->ip.recs || n > s->inst_cap) {
-		const uint64_t grown = (uint64_t)s->inst_cap + s->inst_cap / 2u;
-		const uint32_t cap = s->ip.recs && grown > n ? (uint32_t)(grown < 4194304u ? grown : 4194304u) : n;
-		DevBlock blk;
-		InstParts q = {};
-		rc = carve(s->device, blk, [&](Carve &c) { q = take_insts(c, cap, true); });
+	if (!e.ip.recs || n > e.inst_cap) {
+		const uint64_t grown = (uint64_t)e.inst_cap + e.inst_cap / 2u;
+		const uint32_t cap = e.ip.recs && grown > n ? (uint32_t)(grown < 4194304u ? grown : 4194304u) : n;
+		rc = carve(s->device, e.stage(s->insts), [&](Carve &c) { e.ip = take_insts(c, cap, true); });
 		if (rc) return rc;
-		old = s->insts;
-		s->insts = blk;
-		s->ip = q;
-		s->inst_cap = cap;
+		e.inst_cap = cap;
 	}
+	return CRGPU_OK;
+}
 
-	/* commit */
-	rc = before_commit();
-	if (rc) return rc;
-	cudaStream_t st = s->stream;
+/* Writes a built list of n instances (stage_list) and its top level into the blocks grow_list staged. */
+static int commit_list(Edit &e, uint32_t n, const TopParts &t, const CrgBuildResult &res) {
+	cudaStream_t st = e.s->stream;
 	if (n) {
-		CU(cudaMemcpyAsync(s->ip.last, t.last, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
-		CU(cudaMemcpyAsync(s->ip.keys, t.keys, n, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(e.ip.last, t.last, (size_t)n * 4u, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(e.ip.keys, t.keys, n, cudaMemcpyDeviceToDevice, st));
 	}
-	s->dev.instances = s->ip.recs;
-	s->dev.inst_key = s->ip.keys;
-	s->dev.instance_count = n;
-	s->top_off = top_off;
-	s->top_cap = top_cap;
-	rc = commit_top(s, n, t, res);
-	if (rc) return rc;
-	ctx_free(s->device, old.p, old.bytes);                   /* the descriptor no longer points at it */
+	e.dev.instances = e.ip.recs;
+	e.dev.inst_key = e.ip.keys;
+	e.dev.instance_count = n;
+	return commit_top(e, n, t, res);
+}
+
+/* the host records of a committed list of n instances */
+static void record_list(crgpu_scene *s, const crs_instance *inst, uint32_t n, const InstancePack &pk) {
 	EditRecord &r = s->rec;
 	r.inst_kind.resize(n);
 	r.inst_object.resize(n);
 	for (uint32_t i = 0; i < n; ++i) { r.inst_kind[i] = inst[i].kind; r.inst_object[i] = inst[i].object; }
 	r.last = pk.last;
-	return CRGPU_OK;
 }
 
 extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_instance *inst, uint32_t count) {
@@ -1806,14 +1838,17 @@ extern "C" int crgpu_scene_set_instance_list(crgpu_scene *s, const struct crs_in
 	rc = drain(s);
 	if (rc) return rc;
 	const uint32_t n = count;
+	Edit e(s);
 	TopParts t;
 	void *build = nullptr;
 	rc = carve(s->device, s->scratch, [&](Carve &c) { t = take_top(c, s->rec.bvh_root.size(), n, true); build = c.take<uint8_t>(crg_bvh_scratch_bytes(n)); });
-	if (rc) return rc;
 	CrgBuildResult res;
-	rc = stage_list(s, pk, n, s->rec.bvh_root, t, build, &res);
-	if (rc) return rc;
-	return commit_list(s, inst, n, pk, t, res, [] { return CRGPU_OK; });
+	if (!rc) rc = stage_list(s, pk, n, s->rec.bvh_root, t, build, &res);
+	if (!rc) rc = grow_list(e, n);
+	if (!rc) rc = commit_list(e, n, t, res);
+	if (!rc) rc = e.apply();
+	if (!rc) record_list(s, inst, n, pk);
+	return rc;
 }
 
 /* ---- mesh edits ---------------------------------------------------------------------------------------------------------------------
@@ -1908,13 +1943,13 @@ static int build_meshes(crgpu_scene *s, const crs_scene *f, std::vector<MeshEdit
 
 /* Gives each mesh of `edits` that has no region yet (region[mesh] == UINT32_MAX) its own region of pair nodes behind every pair of the
  * block, in one reserve_pairs; the first geometry edit also reserves the top region behind the uploaded pairs. */
-static int reserve_regions(crgpu_scene *s, std::vector<uint32_t> &region, const std::vector<MeshEdit> &edits) {
-	const uint32_t first = s->pairs.p ? s->pair_cap : s->top_off + s->top_cap;
+static int reserve_regions(Edit &ed, std::vector<uint32_t> &region, const std::vector<MeshEdit> &edits) {
+	const uint32_t first = ed.next(ed.s->pairs).p ? ed.pair_cap : ed.top_off + ed.top_cap;
 	uint64_t add = 0;
 	for (const MeshEdit &e : edits) if (region[e.mesh] == 0xffffffffu) add += region_pairs(e.n);
 	if ((uint64_t)first + add > 0xffffffffull / sizeof(PairNode)) return fail(CRGPU_ERR_UNSUPPORTED, "mesh edit: more pair nodes than the scene can address");
-	if (first + add <= s->pair_cap) return CRGPU_OK;
-	int rc = reserve_pairs(s, first + (uint32_t)add);
+	if (first + add <= ed.pair_cap) return CRGPU_OK;
+	int rc = reserve_pairs(ed, first + (uint32_t)add);
 	if (rc) return rc;
 	uint32_t next = first;
 	for (const MeshEdit &e : edits)
@@ -1931,15 +1966,16 @@ struct GeomParts {
 	ShadePoly *spolys;
 	DevBvh *bvhs;
 };
-static GeomParts geom_live(const crgpu_scene *s) {
-	return { const_cast<PackedTri *>(s->dev.tris), const_cast<uint32_t *>(s->dev.slot_poly), const_cast<uint8_t *>(s->dev.slot_key),
-	         const_cast<ShadePoly *>(s->dev.spolys), const_cast<DevBvh *>(s->dev.bvhs) };
+static GeomParts geom_live(const DevScene &d) {
+	return { const_cast<PackedTri *>(d.tris), const_cast<uint32_t *>(d.slot_poly), const_cast<uint8_t *>(d.slot_key),
+	         const_cast<ShadePoly *>(d.spolys), const_cast<DevBvh *>(d.bvhs) };
 }
 
-/* Copies a built mesh over its pair region, its slots from slot_offset and its polys from poly_offset in the sections g. */
-static int commit_mesh(crgpu_scene *s, const MeshEdit &e, const GeomParts &g, uint32_t region, uint32_t slot_offset, uint32_t poly_offset) {
-	cudaStream_t st = s->stream;
-	if (e.res.pairs) CU(cudaMemcpyAsync(static_cast<PairNode *>(s->pairs.p) + region, e.pairs, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+/* Copies a built mesh over its pair region in the edit's pairs, its slots from slot_offset and its polys from poly_offset in the
+ * sections g. */
+static int commit_mesh(const Edit &ed, const MeshEdit &e, const GeomParts &g, uint32_t region, uint32_t slot_offset, uint32_t poly_offset) {
+	cudaStream_t st = ed.s->stream;
+	if (e.res.pairs) CU(cudaMemcpyAsync(const_cast<PairNode *>(ed.dev.pairs) + region, e.pairs, (size_t)e.res.pairs * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	CU(cudaMemcpyAsync(g.tris + slot_offset, e.tris, (size_t)e.n * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
 	CU(cudaMemcpyAsync(g.slot_poly + slot_offset, e.slot, (size_t)e.n * 4u, cudaMemcpyDeviceToDevice, st));
 	CU(cudaMemcpyAsync(g.slot_key + slot_offset, e.keys, e.n, cudaMemcpyDeviceToDevice, st));
@@ -1981,6 +2017,7 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	const uint32_t ninst = (uint32_t)s->rec.inst_kind.size();
 	uint32_t nmax = ninst;
 	for (const MeshEdit &e : edits) nmax = e.n > nmax ? e.n : nmax;
+	Edit ed(s);
 	TopParts t;
 	void *build = nullptr;
 	rc = carve(s->device, s->scratch, [&](Carve &c) {
@@ -2000,73 +2037,71 @@ extern "C" int crgpu_scene_set_meshes(crgpu_scene *s, const struct crs_scene *fl
 	memset(&top, 0, sizeof top);
 	if (ninst) {
 		CU(cudaMemcpyAsync(t.roots, roots.data(), roots.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-		rc = alloc_insts(s);
+		rc = stage_insts(ed);
+		t.last = ed.ip.last;
 		if (!rc) rc = build_top(s, ninst, s->dev.instances, nullptr, t, build, &top);
 		if (rc) return rc;
 	}
-	rc = reserve_regions(s, s->mesh_region, edits);
+	std::vector<uint32_t> region = s->mesh_region;
+	rc = reserve_regions(ed, region, edits);
 	if (rc) return rc;
 
-	/* commit: each mesh's region, slot and poly ranges, BVH record and staged prefix, then the instances and the top level */
-	const GeomParts g = geom_live(s);
+	/* each mesh's region, slot and poly ranges, BVH record and staged prefix, then the instances and the top level */
+	const GeomParts g = geom_live(ed.dev);
+	std::vector<DevBvh> bvhs = s->bvhs;
 	for (const MeshEdit &e : edits) {
-		DevBvh &b = s->bvhs[e.bvh];
-		const uint32_t region = s->mesh_region[e.mesh];
-		rc = commit_mesh(s, e, g, region, b.slot_offset, s->rec.meshes[e.mesh].poly_offset);
+		DevBvh &b = bvhs[e.bvh];
+		rc = commit_mesh(ed, e, g, region[e.mesh], b.slot_offset, s->rec.meshes[e.mesh].poly_offset);
 		if (rc) return rc;
-		b = bvh_record(e.res, region, b.slot_offset, b.stage_base, s->stage_cap[e.bvh]);
+		b = bvh_record(e.res, region[e.mesh], b.slot_offset, b.stage_base, s->stage_cap[e.bvh]);
 		CU(cudaMemcpyAsync(g.bvhs + e.bvh, &b, sizeof b, cudaMemcpyHostToDevice, st));
 		if (b.stage_count)
-			CU(cudaMemcpyAsync(const_cast<PairNode *>(s->dev.stage_img) + b.stage_base, e.pairs, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
+			CU(cudaMemcpyAsync(const_cast<PairNode *>(ed.dev.stage_img) + b.stage_base, e.pairs, (size_t)b.stage_count * sizeof(PairNode), cudaMemcpyDeviceToDevice, st));
 	}
+	if (ninst && (rc = commit_top(ed, ninst, t, top))) return rc;
+	if ((rc = ed.apply())) return rc;
 	s->rec.bvh_root = roots;
-	if (ninst) return commit_top(s, ninst, t, top);
-	return publish(s);
+	s->bvhs = bvhs;
+	s->mesh_region = region;
+	return CRGPU_OK;
 }
 
 /* ---- shading edits ------------------------------------------------------------------------------------------------------------------
  * The records whose size the material count fixes (materials, flat records, K4's key order) are rewritten in place; the node graph,
  * texture table and texel data, whose sizes may change, go into a new shading block that replaces the previous one.  Every check and
  * the fold run first and the block is filled before anything the kernels read changes. */
-struct ShadeBlock {
-	DevBlock blk;
-	crs_node *nodes;
-	DevTexture *texs;
-};
-/* The node graph, texture table (with the block's addresses) and texel data of `flat` in a new shading block, uploaded and waited for. */
-static int upload_shading(crgpu_scene *s, const crs_scene *flat, ShadingFold &sh, ShadeBlock &out) {
+/* The node graph, texture table (with the block's addresses) and texel data of `flat` in a staged shading block, uploaded and waited
+ * for, and the edit's descriptor pointed at them. */
+static int upload_shading(Edit &e, const crs_scene *flat, ShadingFold &sh) {
+	crgpu_scene *s = e.s;
+	crs_node *nodes = nullptr;
+	DevTexture *texs = nullptr;
 	uint8_t *data = nullptr;
-	out = ShadeBlock();
-	int rc = carve(s->device, out.blk, [&](Carve &c) { out.nodes = c.take<crs_node>(flat->node_count); out.texs = c.take<DevTexture>(sh.texs.size()); data = c.take<uint8_t>(flat->texdata_bytes); });
+	int rc = carve(s->device, e.stage(s->shade), [&](Carve &c) { nodes = c.take<crs_node>(flat->node_count); texs = c.take<DevTexture>(sh.texs.size()); data = c.take<uint8_t>(flat->texdata_bytes); });
 	if (rc) return rc;
 	for (DevTexture &t : sh.texs) t.data = data + (uintptr_t)t.data;
 	cudaStream_t st = s->stream;
-	cudaError_t ce = cudaSuccess;
-	if (flat->node_count) ce = cudaMemcpyAsync(out.nodes, flat->nodes, (size_t)flat->node_count * sizeof(crs_node), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && !sh.texs.empty()) ce = cudaMemcpyAsync(out.texs, sh.texs.data(), sh.texs.size() * sizeof(DevTexture), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess && flat->texdata_bytes) ce = cudaMemcpyAsync(data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) { ctx_free(s->device, out.blk.p, out.blk.bytes); out.blk = DevBlock(); return fail(CRGPU_ERR_CUDA, "shading edit: %s", cudaGetErrorString(ce)); }
+	if (flat->node_count) CU(cudaMemcpyAsync(nodes, flat->nodes, (size_t)flat->node_count * sizeof(crs_node), cudaMemcpyHostToDevice, st));
+	if (!sh.texs.empty()) CU(cudaMemcpyAsync(texs, sh.texs.data(), sh.texs.size() * sizeof(DevTexture), cudaMemcpyHostToDevice, st));
+	if (flat->texdata_bytes) CU(cudaMemcpyAsync(data, flat->texdata, (size_t)flat->texdata_bytes, cudaMemcpyHostToDevice, st));
+	CU(cudaStreamSynchronize(st));
+	e.dev.nodes = nodes;
+	e.dev.textures = texs;
 	return CRGPU_OK;
 }
-/* Writes the fold's materials (flat->material_count of them), flat records and key order over dev.materials, dev.flat and dev.key_order,
- * points the descriptor at the uploaded block and returns the block it replaces in `old` (free it after the publish). */
-static int commit_shading(crgpu_scene *s, const crs_scene *flat, const ShadingFold &sh, const ShadeBlock &b, DevBlock &old) {
-	cudaStream_t st = s->stream;
+/* Writes the fold's materials (flat->material_count of them), flat records and key order over the edit's dev.materials, dev.flat and
+ * dev.key_order, and sets its background. */
+static int commit_shading(Edit &e, const crs_scene *flat, const ShadingFold &sh) {
+	cudaStream_t st = e.s->stream;
 	const size_t nm = flat->material_count;
 	if (nm) {
-		CU(cudaMemcpyAsync(const_cast<DevMaterial *>(s->dev.materials), sh.mats.data(), nm * sizeof(DevMaterial), cudaMemcpyHostToDevice, st));
-		CU(cudaMemcpyAsync(const_cast<DevFlat *>(s->dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<DevMaterial *>(e.dev.materials), sh.mats.data(), nm * sizeof(DevMaterial), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(const_cast<DevFlat *>(e.dev.flat), sh.flat.data(), nm * sizeof(DevFlat), cudaMemcpyHostToDevice, st));
 	}
-	CU(cudaMemcpyAsync(const_cast<uint8_t *>(s->dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
-	s->dev.nodes = b.nodes;
-	s->dev.textures = b.texs;
-	s->dev.bg = sh.bg;
-	s->dev.flat_keys = sh.flat_keys;
-	s->dev.background = flat->background;
-	s->xnodes = sh.xnodes;
-	old = s->shade;
-	s->shade = b.blk;
+	CU(cudaMemcpyAsync(const_cast<uint8_t *>(e.dev.key_order), sh.order.data(), sh.order.size(), cudaMemcpyHostToDevice, st));
+	e.dev.bg = sh.bg;
+	e.dev.flat_keys = sh.flat_keys;
+	e.dev.background = flat->background;
 	return CRGPU_OK;
 }
 
@@ -2079,13 +2114,11 @@ extern "C" int crgpu_scene_set_shading(crgpu_scene *s, const struct crs_scene *f
 	if (rc) return rc;
 	rc = drain(s);
 	if (rc) return rc;
-	ShadeBlock b;
-	rc = upload_shading(s, flat, sh, b);
-	if (rc) return rc;
-	DevBlock old;
-	rc = commit_shading(s, flat, sh, b, old);
-	if (!rc) rc = publish(s);
-	if (!rc) ctx_free(s->device, old.p, old.bytes);   /* the descriptor no longer points at it */
+	Edit e(s);
+	rc = upload_shading(e, flat, sh);
+	if (!rc) rc = commit_shading(e, flat, sh);
+	if (!rc) rc = e.apply();
+	if (!rc) s->xnodes = sh.xnodes;
 	return rc;
 }
 
@@ -2174,6 +2207,7 @@ extern "C" int crgpu_scene_add_objects(crgpu_scene *s, const struct crs_scene *f
 	InstancePack pk;
 	if ((rc = pack_instances(B.instances, n, B.spheres, B.sphere_count, B.meshes, B.mesh_count, B.material_count, CRGPU_ERR_BAD_ARGUMENT, pk))) return rc;
 	if ((rc = drain(s))) return rc;
+	Edit ed(s);
 
 	/* build into scratch: the new meshes, in BVH order (a fresh load gives them slots in that order), then the top level */
 	std::sort(edits.begin(), edits.end(), [](const MeshEdit &a, const MeshEdit &b) { return a.bvh < b.bvh; });
@@ -2206,56 +2240,47 @@ extern "C" int crgpu_scene_add_objects(crgpu_scene *s, const struct crs_scene *f
 	CrgBuildResult top;
 	if ((rc = stage_list(s, pk, n, roots, t, build, &top))) return rc;
 
-	/* grow: shading block, geometry block, materials block, the new meshes' pair regions */
+	/* stage: shading block, geometry block, materials block, the new meshes' pair regions, the list's top region and instance block */
 	cudaStream_t st = s->stream;
-	ShadeBlock shb;
-	if ((rc = upload_shading(s, flat, sh, shb))) return rc;
-	DevBlock geom, mats;
-	auto drop = [&](int code) { for (DevBlock *b : { &shb.blk, &geom, &mats }) ctx_free(s->device, b->p, b->bytes); return code; };
-	GeomParts g = geom_live(s);
+	if ((rc = upload_shading(ed, flat, sh))) return rc;
+	GeomParts g = geom_live(ed.dev);
 	const uint32_t slot_need = (uint32_t)slots;
 	uint32_t slot_cap = s->slot_cap, poly_cap = s->poly_cap, bvh_cap = s->bvh_cap;
-	if (slot_need > slot_cap || B.poly_count > poly_cap || B.bvh_count > bvh_cap) {
+	const bool grow_geom = slot_need > slot_cap || B.poly_count > poly_cap || B.bvh_count > bvh_cap;
+	if (grow_geom) {
 		slot_cap = grown_cap(slot_cap, slot_need); poly_cap = grown_cap(poly_cap, B.poly_count); bvh_cap = grown_cap(bvh_cap, B.bvh_count);
-		if ((rc = carve(s->device, geom, [&](Carve &c) { g = take_geom(c, slot_cap, poly_cap, bvh_cap); }))) return drop(rc);
-		const GeomParts live = geom_live(s);
+		if ((rc = carve(s->device, ed.stage(s->geom), [&](Carve &c) { g = take_geom(c, slot_cap, poly_cap, bvh_cap); }))) return rc;
+		const GeomParts live = geom_live(s->dev);
 		const size_t ns = s->slot_count;
-		cudaError_t ce = cudaMemcpyAsync(g.tris, live.tris, ns * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st);
-		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.slot_poly, live.slot_poly, ns * 4u, cudaMemcpyDeviceToDevice, st);
-		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.slot_key, live.slot_key, ns, cudaMemcpyDeviceToDevice, st);
-		if (ce == cudaSuccess) ce = cudaMemcpyAsync(g.spolys, live.spolys, (size_t)s->poly_count * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st);
-		if (ce != cudaSuccess) return drop(fail(CRGPU_ERR_CUDA, "add_objects: %s", cudaGetErrorString(ce)));
+		CU(cudaMemcpyAsync(g.tris, live.tris, ns * sizeof(PackedTri), cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(g.slot_poly, live.slot_poly, ns * 4u, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(g.slot_key, live.slot_key, ns, cudaMemcpyDeviceToDevice, st));
+		CU(cudaMemcpyAsync(g.spolys, live.spolys, (size_t)s->poly_count * sizeof(ShadePoly), cudaMemcpyDeviceToDevice, st));
 	}
+	const bool grow_mats = B.material_count > s->mat_cap;
 	MatParts mp = { const_cast<DevMaterial *>(s->dev.materials), const_cast<DevFlat *>(s->dev.flat) };
-	if (B.material_count > s->mat_cap &&
-	    (rc = carve(s->device, mats, [&](Carve &c) { mp.mats = c.take<DevMaterial>(B.material_count); mp.flat = c.take<DevFlat>(B.material_count); })))
-		return drop(rc);
+	if (grow_mats &&
+	    (rc = carve(s->device, ed.stage(s->mats), [&](Carve &c) { mp.mats = c.take<DevMaterial>(B.material_count); mp.flat = c.take<DevFlat>(B.material_count); })))
+		return rc;
 	std::vector<uint32_t> region = s->mesh_region;
 	region.resize(B.mesh_count, 0xffffffffu);
-	if ((rc = reserve_regions(s, region, edits))) return drop(rc);
+	if ((rc = reserve_regions(ed, region, edits)) || (rc = grow_list(ed, n))) return rc;
 
-	/* commit, inside the list's commit: the BVH records the item records read must be in place first */
-	DevBlock old_shade, old_geom, old_mats;
-	rc = commit_list(s, B.instances, n, pk, t, top, [&]() -> int {
-		uint32_t slot = s->slot_count;
-		for (const MeshEdit &e : edits) {
-			int r = commit_mesh(s, e, g, region[e.mesh], slot, B.meshes[e.mesh].poly_offset);
-			if (r) return r;
-			bvhs[e.bvh] = bvh_record(e.res, region[e.mesh], slot, 0u, 0u);
-			slot += e.n;
-		}
-		CU(cudaMemcpyAsync(g.bvhs, bvhs.data(), bvhs.size() * sizeof(DevBvh), cudaMemcpyHostToDevice, st));
-		s->dev.tris = g.tris; s->dev.slot_poly = g.slot_poly; s->dev.slot_key = g.slot_key; s->dev.spolys = g.spolys; s->dev.bvhs = g.bvhs;
-		s->dev.materials = mp.mats; s->dev.flat = mp.flat;
-		int r = commit_shading(s, flat, sh, shb, old_shade);
-		if (r) return r;
-		if (geom.p) { old_geom = s->geom; s->geom = geom; s->slot_cap = slot_cap; s->poly_cap = poly_cap; s->bvh_cap = bvh_cap; }
-		if (mats.p) { old_mats = s->mats; s->mats = mats; s->mat_cap = B.material_count; }
-		geom = mats = shb.blk = DevBlock();                   /* the scene owns them now */
-		return CRGPU_OK;
-	});
-	if (rc) return drop(rc);
-	for (DevBlock *b : { &old_shade, &old_geom, &old_mats }) ctx_free(s->device, b->p, b->bytes);   /* the descriptor no longer points at them */
+	/* write: the new meshes and the BVH records (the list's item records read them), the shading, then the list and its top level */
+	uint32_t slot = s->slot_count;
+	for (const MeshEdit &e : edits) {
+		if ((rc = commit_mesh(ed, e, g, region[e.mesh], slot, B.meshes[e.mesh].poly_offset))) return rc;
+		bvhs[e.bvh] = bvh_record(e.res, region[e.mesh], slot, 0u, 0u);
+		slot += e.n;
+	}
+	CU(cudaMemcpyAsync(g.bvhs, bvhs.data(), bvhs.size() * sizeof(DevBvh), cudaMemcpyHostToDevice, st));
+	ed.dev.tris = g.tris; ed.dev.slot_poly = g.slot_poly; ed.dev.slot_key = g.slot_key; ed.dev.spolys = g.spolys; ed.dev.bvhs = g.bvhs;
+	ed.dev.materials = mp.mats; ed.dev.flat = mp.flat;
+	if ((rc = commit_shading(ed, flat, sh)) || (rc = commit_list(ed, n, t, top)) || (rc = ed.apply())) return rc;
+	if (grow_geom) { s->slot_cap = slot_cap; s->poly_cap = poly_cap; s->bvh_cap = bvh_cap; }
+	if (grow_mats) s->mat_cap = B.material_count;
+	s->xnodes = sh.xnodes;
+	record_list(s, B.instances, n, pk);
 	s->material_count = B.material_count;
 	s->slot_count = slot_need;
 	s->poly_count = B.poly_count;
@@ -2326,23 +2351,18 @@ static int tile_set(crgpu_scene *s, const int *rects, int nrects, uint64_t views
 		unsigned acc = 0u;
 		for (int i = 0; i < nrects; ++i) { offs[(size_t)i] = acc; acc += (unsigned)((rects[4 * i + 2] - rects[4 * i]) * (rects[4 * i + 3] - rects[4 * i + 1])); }
 		const size_t need = (size_t)total * sizeof(uint32_t) + (size_t)nrects * 20u + 256u;
-		if (s->pixel_cap * sizeof(uint32_t) < need) {
+		if (s->pixels.bytes < need) {
 			CU(cudaStreamSynchronize(s->stream));       /* the previous list may still be in use by queued kernels */
-			ctx_free(s->device, s->pixels, s->pixel_cap * sizeof(uint32_t));
-			s->pixels = nullptr; s->pixel_cap = 0;
-			void *q = nullptr;
-			int arc = ctx_alloc(s->device, need, &q);
+			int arc = s->pixels.alloc(s->device, need);
 			if (arc) return arc;
-			s->pixels = static_cast<uint32_t *>(q);
-			s->pixel_cap = (need + 3u) / 4u;
 		}
 		/* rectangle table behind the pixel list (same block); both copies are from pageable memory, i.e. staged before the call
 		 * returns, and ordered before the kernel on the scene's stream */
-		uint8_t *tab = reinterpret_cast<uint8_t *>(s->pixels) + (((size_t)total * sizeof(uint32_t) + 255u) & ~(size_t)255u);
+		uint8_t *tab = s->pixels.as<uint8_t>() + (((size_t)total * sizeof(uint32_t) + 255u) & ~(size_t)255u);
 		CU(cudaMemcpyAsync(tab, rects, (size_t)nrects * 16u, cudaMemcpyHostToDevice, s->stream));
 		CU(cudaMemcpyAsync(tab + (size_t)nrects * 16u, offs.data(), (size_t)nrects * 4u, cudaMemcpyHostToDevice, s->stream));
 		CU(cudaStreamSynchronize(s->stream));           /* offs is a local; costs ~20 us, once per tile set */
-		crg_launch_pixel_list(s->pixels, reinterpret_cast<const int4 *>(tab), reinterpret_cast<const unsigned *>(tab + (size_t)nrects * 16u), nrects,
+		crg_launch_pixel_list(s->pixels.as<uint32_t>(), reinterpret_cast<const int4 *>(tab), reinterpret_cast<const unsigned *>(tab + (size_t)nrects * 16u), nrects,
 		                      crg_path_order().blocked, s->stream);
 		CU(cudaGetLastError());
 		s->pixel_key.swap(key);
@@ -2358,7 +2378,7 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 	if (rc) return rc;
 	TileDesc td;
 	memset(&td, 0, sizeof td);
-	td.pixels = s->pixels;
+	td.pixels = s->pixels.as<uint32_t>();
 	return render_call(s, td, total, pass_begin, pass_count, flags, stats);
 }
 
@@ -2367,7 +2387,7 @@ extern "C" int crgpu_render_tiles(crgpu_scene *s, const int *rects, int nrects, 
 static size_t views_cam_bytes(uint32_t cap) { return align256((size_t)(cap - 1u) * sizeof(DevCamera)); }
 static size_t views_bytes(uint32_t cap, size_t fb_floats) { return views_cam_bytes(cap) + (size_t)(cap - 1u) * fb_floats * sizeof(float); }
 static float *views_fb(const DevBlock &b, uint32_t cap) { return b.p ? reinterpret_cast<float *>(static_cast<uint8_t *>(b.p) + views_cam_bytes(cap)) : nullptr; }
-static float *view_fb(const crgpu_scene *s, uint32_t v) { return v ? views_fb(s->views, s->view_cap) + (size_t)(v - 1u) * s->fb_floats : s->fb; }
+static float *view_fb(const crgpu_scene *s, uint32_t v) { return v ? views_fb(s->views, s->view_cap) + (size_t)(v - 1u) * s->fb_floats : s->fb.as<float>(); }
 
 extern "C" int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *cams, uint32_t count) {
 	if (!s || !cams) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
@@ -2380,37 +2400,24 @@ extern "C" int crgpu_scene_set_views(crgpu_scene *s, const struct crs_camera *ca
 	if (rc) return rc;
 	std::vector<DevCamera> dc(count - 1u);
 	for (uint32_t i = 1; i < count; ++i) dc[i - 1u] = dev_camera(cams[i]);
-	DevBlock blk = s->views;
-	uint32_t cap = s->view_cap;
-	if (count > cap) {                                   /* a larger block; the surviving views' framebuffers move into it */
-		cap = count;
-		blk.bytes = views_bytes(cap, s->fb_floats);
-		rc = ctx_alloc(s->device, blk.bytes, &blk.p);
-		if (rc) return rc;
-	}
-	const bool moved = blk.p != s->views.p;
+	Edit e(s);
+	const bool grow = count > s->view_cap;               /* a larger block; the surviving views' framebuffers move into it */
+	const uint32_t cap = grow ? count : s->view_cap;
+	if (grow && (rc = e.stage(s->views).alloc(s->device, views_bytes(cap, s->fb_floats)))) return rc;
+	const DevBlock &blk = e.next(s->views);
 	const uint32_t keep = s->view_count < count ? s->view_count : count;     /* views 0 .. keep - 1 keep their pixels */
 	float *fbs = views_fb(blk, cap);
 	const size_t fb_bytes = s->fb_floats * sizeof(float);
 	cudaStream_t st = s->stream;
-	cudaError_t ce = cudaSuccess;
-	if (moved && keep > 1u) ce = cudaMemcpyAsync(fbs, views_fb(s->views, s->view_cap), (size_t)(keep - 1u) * fb_bytes, cudaMemcpyDeviceToDevice, st);
-	if (ce == cudaSuccess && count > keep) ce = cudaMemsetAsync(fbs + (size_t)(keep - 1u) * s->fb_floats, 0, (size_t)(count - keep) * fb_bytes, st);
-	if (ce == cudaSuccess && count > 1u) ce = cudaMemcpyAsync(blk.p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) {
-		if (moved) ctx_free(s->device, blk.p, blk.bytes);
-		return fail(CRGPU_ERR_CUDA, "set_views: %s", cudaGetErrorString(ce));
-	}
-	/* commit */
-	if (moved) {
-		ctx_free(s->device, s->views.p, s->views.bytes);
-		s->views = blk;
-		s->view_cap = cap;
-	}
+	if (grow && keep > 1u) CU(cudaMemcpyAsync(fbs, views_fb(s->views, s->view_cap), (size_t)(keep - 1u) * fb_bytes, cudaMemcpyDeviceToDevice, st));
+	if (count > keep) CU(cudaMemsetAsync(fbs + (size_t)(keep - 1u) * s->fb_floats, 0, (size_t)(count - keep) * fb_bytes, st));
+	if (count > 1u) CU(cudaMemcpyAsync(blk.p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, st));
+	CU(cudaStreamSynchronize(st));
+	e.dev.cam = dev_camera(cams[0]);
+	if ((rc = e.apply())) return rc;
 	s->view_count = count;
-	s->dev.cam = dev_camera(cams[0]);
-	return publish(s);
+	s->view_cap = cap;
+	return CRGPU_OK;
 }
 
 /* ---- render settings between renders ---------------------------------------------------------------------------------------------
@@ -2432,55 +2439,32 @@ extern "C" int crgpu_scene_set_render(crgpu_scene *s, uint32_t width, uint32_t h
 	int rc = drain(s);
 	if (rc) return rc;
 	const size_t fb_floats = resize ? (size_t)width * height * 3u : s->fb_floats;
-	float *fb = s->fb;
-	DevBlock blk = s->views;
-	uint32_t cap = s->view_cap;
-	if (resize) {                                      /* every new block first: a failed allocation changes nothing */
-		void *q = nullptr;
-		if ((rc = ctx_alloc(s->device, fb_floats * sizeof(float), &q))) return rc;
-		fb = static_cast<float *>(q);
-		cap = count;
-		blk = DevBlock();
-		if (count > 1u) {
-			blk.bytes = views_bytes(cap, fb_floats);
-			if ((rc = ctx_alloc(s->device, blk.bytes, &blk.p))) { ctx_free(s->device, fb, fb_floats * sizeof(float)); return rc; }
-		}
+	const uint32_t cap = resize ? count : s->view_cap;
+	Edit e(s);
+	if (resize) {                                      /* new zeroed framebuffers (no views block for one view); the sRGB8 staging goes */
+		DevBlock &fb = e.stage(s->fb), &views = e.stage(s->views);
+		e.stage(s->fb8);
+		e.stage(s->snap8);
+		if ((rc = fb.alloc(s->device, fb_floats * sizeof(float)))) return rc;
+		if (count > 1u && (rc = views.alloc(s->device, views_bytes(cap, fb_floats)))) return rc;
+		CU(cudaMemsetAsync(fb.p, 0, fb.bytes, s->stream));
+		if (count > 1u) CU(cudaMemsetAsync(views_fb(views, cap), 0, (size_t)(count - 1u) * fb_floats * sizeof(float), s->stream));
 	}
 	std::vector<DevCamera> dc(cams ? count - 1u : 0u);
 	for (size_t i = 0; i < dc.size(); ++i) dc[i] = dev_camera(cams[i + 1u]);
-	cudaStream_t st = s->stream;
-	cudaError_t ce = cudaSuccess;
-	if (resize) ce = cudaMemsetAsync(fb, 0, fb_floats * sizeof(float), st);
-	if (ce == cudaSuccess && resize && count > 1u) ce = cudaMemsetAsync(views_fb(blk, cap), 0, (size_t)(count - 1u) * fb_floats * sizeof(float), st);
-	if (ce == cudaSuccess && !dc.empty()) ce = cudaMemcpyAsync(blk.p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, st);
-	if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-	if (ce != cudaSuccess) {
-		if (resize) { ctx_free(s->device, fb, fb_floats * sizeof(float)); ctx_free(s->device, blk.p, blk.bytes); }
-		return fail(CRGPU_ERR_CUDA, "set_render: %s", cudaGetErrorString(ce));
-	}
-	/* commit */
-	const DevBlock old_views = s->views;
-	float *old_fb = s->fb;
-	uint8_t *old_fb8 = s->fb8, *old_snap8 = s->snap8;
-	const size_t old_floats = s->fb_floats;
+	if (!dc.empty()) CU(cudaMemcpyAsync(e.next(s->views).p, dc.data(), dc.size() * sizeof(DevCamera), cudaMemcpyHostToDevice, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	e.dev.image_width = width; e.dev.image_height = height;
+	e.dev.sample_count = sample_count; e.dev.bounces = bounces;
+	if (cams) e.dev.cam = dev_camera(cams[0]);
+	if ((rc = e.apply())) return rc;
 	if (resize) {
-		s->fb = fb; s->fb_floats = fb_floats;
-		s->views = blk; s->view_cap = cap;
-		s->fb8 = s->snap8 = nullptr;
+		s->fb_floats = fb_floats;
+		s->view_cap = cap;
 		unsigned staged = 2u;                          /* an image staged at the old size is dropped; a pending request stays */
 		if (s->stop_host) __atomic_compare_exchange_n(&s->stop_host[3], &staged, 0u, false, __ATOMIC_ACQ_REL, __ATOMIC_ACQUIRE);
 	}
-	s->dev.image_width = width; s->dev.image_height = height;
-	s->dev.sample_count = sample_count; s->dev.bounces = bounces;
-	if (cams) s->dev.cam = dev_camera(cams[0]);
-	rc = publish(s);
-	if (!rc && resize) {                               /* the descriptor and the scene no longer point at them */
-		ctx_free(s->device, old_fb, old_floats * sizeof(float));
-		ctx_free(s->device, old_fb8, old_floats);
-		ctx_free(s->device, old_snap8, old_floats);
-		ctx_free(s->device, old_views.p, old_views.bytes);
-	}
-	return rc;
+	return CRGPU_OK;
 }
 
 extern "C" int crgpu_scene_view_count(crgpu_scene *s, uint32_t *count) {
@@ -2507,7 +2491,7 @@ extern "C" int crgpu_render_views(crgpu_scene *s, uint32_t first_view, uint32_t 
 	vd.p0 = 0u;
 	TileDesc td;
 	memset(&td, 0, sizeof td);
-	td.pixels = s->pixels;
+	td.pixels = s->pixels.as<uint32_t>();
 	return render_call(s, td, npix * view_count, pass_begin, pass_count, flags, stats, &vd);
 }
 
@@ -2536,17 +2520,23 @@ extern "C" int crgpu_view_read(crgpu_scene *s, uint32_t view, float *host_rgb) {
 	return CRGPU_OK;
 }
 
+/* view v's image as sRGB8 (view 0: the scene's framebuffer), through fb8 */
+static int to_srgb8(crgpu_scene *s, uint32_t v, uint8_t *host_rgb8) {
+	CU(cudaSetDevice(s->device));
+	int rc = alloc_srgb8(s, s->fb8);
+	if (rc) return rc;
+	crg_launch_to_srgb8(view_fb(s, v), s->fb8.as<uint8_t>(), s->fb_floats, s->sm_count * 8, s->stream);
+	CU(cudaGetLastError());
+	CU(cudaMemcpyAsync(host_rgb8, s->fb8.p, s->fb_floats, cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
 extern "C" int crgpu_view_to_srgb8(crgpu_scene *s, uint32_t view, uint8_t *host_rgb8) {
 	int rc = check_view(s, view);
 	if (rc) return rc;
 	if (!host_rgb8) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	CU(cudaSetDevice(s->device));
-	if (!s->fb8) { void *q = nullptr; int arc = ctx_alloc(s->device, s->fb_floats, &q); if (arc) return arc; s->fb8 = static_cast<uint8_t *>(q); }
-	crg_launch_to_srgb8(view_fb(s, view), s->fb8, s->fb_floats, s->sm_count * 8, s->stream);
-	CU(cudaGetLastError());
-	CU(cudaMemcpyAsync(host_rgb8, s->fb8, s->fb_floats, cudaMemcpyDeviceToHost, s->stream));
-	CU(cudaStreamSynchronize(s->stream));
-	return CRGPU_OK;
+	return to_srgb8(s, view, host_rgb8);
 }
 
 extern "C" int crgpu_get_stats(crgpu_scene *s, struct crgpu_stats *stats) {
@@ -2591,7 +2581,7 @@ extern "C" int crgpu_use_own_stream(crgpu_scene *s) {
 extern "C" int crgpu_framebuffer_clear(crgpu_scene *s) {
 	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
 	CU(cudaSetDevice(s->device));
-	CU(cudaMemsetAsync(s->fb, 0, s->fb_floats * sizeof(float), s->stream));
+	CU(cudaMemsetAsync(s->fb.p, 0, s->fb.bytes, s->stream));
 	CU(cudaStreamSynchronize(s->stream));
 	return CRGPU_OK;
 }
@@ -2607,8 +2597,8 @@ static int fb_copy(crgpu_scene *s, float *host, int x0, int y0, int x1, int y1, 
 	const size_t row0 = H - (size_t)y1, rows = (size_t)(y1 - y0);
 	const size_t off = (row0 * W + (size_t)x0) * 3u;
 	const size_t pitch = W * 3u * sizeof(float), width = (size_t)(x1 - x0) * 3u * sizeof(float);
-	if (to_host) CU(cudaMemcpy2DAsync(host + off, pitch, s->fb + off, pitch, width, rows, cudaMemcpyDeviceToHost, s->stream));
-	else CU(cudaMemcpy2DAsync(s->fb + off, pitch, host + off, pitch, width, rows, cudaMemcpyHostToDevice, s->stream));
+	if (to_host) CU(cudaMemcpy2DAsync(host + off, pitch, s->fb.as<float>() + off, pitch, width, rows, cudaMemcpyDeviceToHost, s->stream));
+	else CU(cudaMemcpy2DAsync(s->fb.as<float>() + off, pitch, host + off, pitch, width, rows, cudaMemcpyHostToDevice, s->stream));
 	CU(cudaStreamSynchronize(s->stream));
 	return CRGPU_OK;
 }
@@ -2621,18 +2611,12 @@ extern "C" int crgpu_framebuffer_write(crgpu_scene *s, const float *host_rgb, in
 
 extern "C" int crgpu_framebuffer_to_srgb8(crgpu_scene *s, uint8_t *host_rgb8) {
 	if (!s || !host_rgb8) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	CU(cudaSetDevice(s->device));
-	if (!s->fb8) { void *q = nullptr; int arc = ctx_alloc(s->device, s->fb_floats, &q); if (arc) return arc; s->fb8 = static_cast<uint8_t *>(q); }
-	crg_launch_to_srgb8(s->fb, s->fb8, s->fb_floats, s->sm_count * 8, s->stream);
-	CU(cudaGetLastError());
-	CU(cudaMemcpyAsync(host_rgb8, s->fb8, s->fb_floats, cudaMemcpyDeviceToHost, s->stream));
-	CU(cudaStreamSynchronize(s->stream));
-	return CRGPU_OK;
+	return to_srgb8(s, 0, host_rgb8);
 }
 
 extern "C" int crgpu_framebuffer_device_ptr(crgpu_scene *s, void **dev_ptr, size_t *bytes) {
 	if (!s || !dev_ptr) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
-	*dev_ptr = s->fb;
+	*dev_ptr = s->fb.p;
 	if (bytes) *bytes = s->fb_floats * sizeof(float);
 	return CRGPU_OK;
 }

@@ -2,7 +2,8 @@
  * A stand-in for the handful of CUDA runtime calls libcrgpu's HOST code makes (device memory = malloc, copies = memcpy,
  * kernel launches = no-ops), so that the host half of crgpu_scene_create — validation, BVH re-layout into pair nodes,
  * triangle packing, shading records — can be exercised, timed and its upload bytes pinned in the CPU test suite
- * (tests/test_create_host.py).  Nothing is rendered: there is no CPU path for the kernels. */
+ * (tests/test_create_host.py), and so that the edit calls' block bookkeeping can be checked (tests/test_edit_blocks_host.py).
+ * Nothing is rendered: there is no CPU path for the kernels. */
 #include <stdlib.h>
 #include <string.h>
 #include <stdio.h>
@@ -21,8 +22,17 @@ cudaError_t cudaGetDevice(int *d) { *d = 0; return 0; }
 cudaError_t cudaDeviceSynchronize(void) { note("devsync",0,0); return 0; }
 cudaError_t cudaGetLastError(void) { return 0; }
 const char *cudaGetErrorString(cudaError_t e) { (void)e; return "stub"; }
-cudaError_t cudaMalloc(void **p, size_t n) { *p = malloc(n ? n : 1); return *p ? 0 : 2; }
-cudaError_t cudaFree(void *p) { free(p); return 0; }
+/* device allocations still live, and a switch that fails cudaMalloc from its k-th call on (tests/stub/edit_blocks_harness.c) */
+static long g_live, g_mallocs, g_fail_from = -1;
+long stub_live_allocs(void) { return g_live; }
+void stub_fail_malloc_from(long k) { g_mallocs = 0; g_fail_from = k; }   /* k counts calls from now, 1-based; k < 0 lifts it */
+cudaError_t cudaMalloc(void **p, size_t n) {
+	if (g_fail_from >= 0 && ++g_mallocs >= g_fail_from) { *p = NULL; return 2; }   /* cudaErrorMemoryAllocation */
+	*p = malloc(n ? n : 1);
+	if (*p) ++g_live;
+	return *p ? 0 : 2;
+}
+cudaError_t cudaFree(void *p) { if (p) --g_live; free(p); return 0; }
 cudaError_t cudaHostAlloc(void **p, size_t n, unsigned f) { (void)f; *p = malloc(n ? n : 1); return *p ? 0 : 2; }
 cudaError_t cudaFreeHost(void *p) { free(p); return 0; }
 cudaError_t cudaMemcpy(void *d, const void *s, size_t n, int k) { (void)k; note("memcpy",s,n); memcpy(d, s, n); t_last=now_(); return 0; }
