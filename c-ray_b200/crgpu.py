@@ -53,6 +53,12 @@ class Stats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "pad"}
 
 
+class Adaptive(C.Structure):
+    """struct crgpu_adaptive: the rule of an adaptive round (crgpu_adaptive_round)"""
+    _fields_ = [("min_passes", C.c_uint32), ("round_passes", C.c_uint32), ("pass_end", C.c_uint32), ("threshold", C.c_float),
+                ("floor", C.c_float)]
+
+
 class TraceOpts(C.Structure):
     """struct crgpu_trace_opts: the launch variant of the traversal kernel (crgpu_trace_rays)"""
     _fields_ = [(n, C.c_int32) for n in ("count", "minb", "defer", "refill", "burst", "inst_min")] + [("order", C.c_void_p)]
@@ -166,6 +172,13 @@ def lib():
         if hasattr(L, "crgpu_scene_set_render"):  # absent from libraries built before render-settings edits
             L.crgpu_scene_set_render.argtypes = [P] + [C.c_uint32] * 4 + [P, C.c_uint32]
             L.crgpu_scene_set_render.restype = C.c_int
+        if hasattr(L, "crgpu_adaptive_round"):    # absent from libraries built before adaptive rounds
+            L.crgpu_adaptive_reset.argtypes = [P]
+            L.crgpu_adaptive_round.argtypes = [P, P, C.c_int, C.POINTER(Adaptive), C.c_uint, C.POINTER(Stats), C.POINTER(C.c_uint32),
+                                               C.POINTER(C.c_int), C.POINTER(C.c_int)]
+            L.crgpu_adaptive_read.argtypes = [P, P, P]
+            for f in ("crgpu_adaptive_reset", "crgpu_adaptive_round", "crgpu_adaptive_read"):
+                getattr(L, f).restype = C.c_int
         _lib = L
     return _lib
 
@@ -346,6 +359,52 @@ class GpuScene:
             arr, n = (Camera * len(cameras))(*cameras), len(cameras)
         _check(lib().crgpu_scene_set_render(self.handle, width, height, samples, bounces, arr, n), "crgpu_scene_set_render")
         self.W, self.H, self.samples, self.bounces = width, height, samples, bounces
+
+    def adaptive_reset(self):
+        """Give every pixel of view 0 a fresh adaptive record: 0 passes, err +inf, not done (crgpu_adaptive_reset)."""
+        _check(lib().crgpu_adaptive_reset(self.handle), "crgpu_adaptive_reset")
+
+    def adaptive_round(self, rects, min_passes, round_passes, threshold, floor, pass_end=None, flags=0):
+        """One adaptive round over the tile set [(x0, y0, x1, y1), ...] (crgpu_adaptive_round).  Returns a dict: the call's stats (none
+        with FLAG_ASYNC), "active", "pass_begin", "pass_end" (the passes [pass_begin, pass_end) rendered for the active pixels) and, on
+        an armed scene, "stopped"."""
+        st = Stats()
+        a = Adaptive(min_passes, round_passes, self.samples if pass_end is None else pass_end, threshold, floor)
+        arr = np.ascontiguousarray(rects, dtype=np.int32).reshape(-1, 4)
+        active, pb, pe = C.c_uint32(0), C.c_int(0), C.c_int(0)
+        rc = lib().crgpu_adaptive_round(self.handle, arr.ctypes.data, len(arr), C.byref(a), flags, C.byref(st), C.byref(active), C.byref(pb),
+                                        C.byref(pe))
+        d = self._render_result(rc, flags, st, "crgpu_adaptive_round") or {}
+        d.update(active=active.value, pass_begin=pb.value, pass_end=pe.value)
+        return d
+
+    def adaptive_read(self):
+        """(passes uint32 [H, W], err float32 [H, W]) of every pixel, in the framebuffer layout (as read() gives the image)."""
+        n = np.empty((self.H, self.W), dtype=np.uint32)
+        err = np.empty((self.H, self.W), dtype=np.float32)
+        _check(lib().crgpu_adaptive_read(self.handle, n.ctypes.data, err.ctypes.data), "crgpu_adaptive_read")
+        return n, err
+
+    def render_adaptive(self, rects, min_passes, round_passes, threshold, floor, pass_end=None):
+        """Adaptive rounds over the tile set until no pixel is active, or until an armed round is stopped (synchronous).  Does not
+        reset: call adaptive_reset (and clear) first for a new frame.  Returns the stats summed over the rounds, with "rounds" and, on
+        an armed scene, "stopped"."""
+        total = {n: 0 for n, _ in Stats._fields_ if n != "pad"}
+        total["rounds"] = 0
+        while True:
+            d = self.adaptive_round(rects, min_passes, round_passes, threshold, floor, pass_end)
+            for k in Stats._fields_:
+                if k[0] != "pad":
+                    total[k[0]] += d[k[0]]
+            if d["active"] == 0:
+                break
+            total["rounds"] += 1
+            if d.get("stopped"):
+                total["stopped"] = True
+                return total
+        if getattr(self, "armed", False):
+            total["stopped"] = False
+        return total
 
     def view_count(self):
         n = C.c_uint32(0)

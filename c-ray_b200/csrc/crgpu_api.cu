@@ -12,6 +12,7 @@
 #define CRG_TAIL_FROM 6      /* first bounce at which the tail kernel may take over (it only does when <= 16384 rays are left) */
 
 #include <cstdio>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <cstdarg>
@@ -273,6 +274,11 @@ struct crgpu_scene {
 	uint32_t view_cap = 1;           /* views the block has room for (1: no block) */
 	DevBlock views;                  /* NULL until the first set_views of more than one view: view_cap - 1 cameras, then view_cap - 1
 	                                    framebuffers (views_layout); grows only */
+	/* adaptive rounds (crgpu_adaptive_reset / _round / _read) */
+	DevBlock adapt;                  /* NULL until the first reset and after a size change: view 0's pixel records, the active list and
+	                                    the select's scan scratch (AdaptParts) */
+	unsigned *adapt_host = nullptr;  /* pinned, mapped: [0] active count, [1] min and [2] max count of the last select */
+	std::vector<int> adapt_key;      /* the last tile set found to have no overlapping tiles */
 };
 
 /* K1 and K2 take the host descriptor s->dev by value; K3, the tail kernel and the KAT read its HBM copy s->dev_copy.  Writes the
@@ -783,6 +789,7 @@ extern "C" int crgpu_scene_destroy(crgpu_scene *s) {
 	if (s->own_stream) cudaStreamDestroy(s->own_stream);
 	if (s->snap_stream) cudaStreamDestroy(s->snap_stream);
 	if (s->stop_host) cudaFreeHost(s->stop_host);
+	if (s->adapt_host) cudaFreeHost(s->adapt_host);
 	delete s;                                        /* its blocks go back to the per-device cache */
 	return CRGPU_OK;
 }
@@ -1300,7 +1307,7 @@ static uint64_t enqueue_bounce(const crgpu_scene *s, const WaveBuffers &wb, int 
 /* The batch loop: passes [pass_begin, +pass_count) over one piece of at most max_paths pixels (pass_count > 0).  vd: NULL, or the
  * piece's views (a views call: K1 and K5 in their views instantiations). */
 static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, const Gates &gates,
-                          const ViewDesc *vd) {
+                          const ViewDesc *vd, AdaptPix *adapt) {
 	const bool armed = s->armed;
 	const bool count = (flags & CRGPU_FLAG_COUNT) != 0;
 	const bool timing = (flags & CRGPU_FLAG_TIME_KERNELS) != 0;
@@ -1363,7 +1370,7 @@ static int render_batches(crgpu_scene *s, const TileDesc &base, uint64_t tile_pi
 		}
 		if (sets == 2 && bi > 0) CU(cudaStreamWaitEvent(st, s->evAcc[set ^ 1], 0));      /* pass order of the running average */
 		crg_launch_accumulate(s->fb.as<float>(), wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, grid, st, armed ? s->stop_ctl : nullptr, set,
-		                      armed && gates.publish ? s->stop_host : nullptr, vd); ++launches;
+		                      armed && gates.publish ? s->stop_host : nullptr, vd, adapt); ++launches;
 		if (armed && gates.publish) {       /* stages a snapshot when K5 found one requested (crgpu_request_snapshot) */
 			crg_launch_stop_publish(s->stop_ctl, set, s->stop_host, td.pass_begin, td.pass_count, gates.call_pixels * (uint64_t)td.pass_count, wb.stats,
 			                        s->fb.as<float>(), s->snap8.as<uint8_t>(), s->fb_floats, s->sm_count * 4, st);
@@ -1421,9 +1428,10 @@ static int split_pieces(const crgpu_scene *s, const TileDesc &base, uint64_t til
  * [0, committed) and a later call for [committed, end) finishes it bit for bit; several pieces are walked pass-major, each batch of
  * passes over every piece, so that one pass count describes the set.  Only the first piece of a pass batch takes a stop (the later
  * ones complete a pass batch whose first piece was added), which bounds its latency by one pass batch over the whole set.
- * vd: NULL, or the views of a views call over its whole (view, pixel) set of tile_pixels pairs (crgpu_render_views). */
+ * vd: NULL, or the views of a views call over its whole (view, pixel) set of tile_pixels pairs (crgpu_render_views).  adapt: NULL, or
+ * the pixel records of an adaptive round, which K5 updates with every pass it adds (crgpu_adaptive_round). */
 static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixels, int pass_begin, int pass_count, unsigned flags, struct crgpu_stats *stats,
-                       const ViewDesc *vd = nullptr) {
+                       const ViewDesc *vd = nullptr, AdaptPix *adapt = nullptr) {
 	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
 	const bool armed = s->armed;
@@ -1442,7 +1450,8 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 	if (pass_count > 0 && tile_pixels > 0) rc = split_pieces(s, base, tile_pixels, vd, pieces);   /* an empty call renders nothing */
 	if (!armed || pieces.size() < 2) {
 		for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
-			rc = render_batches(s, pieces[k].td, pieces[k].pixels, pass_begin, pass_count, flags, { true, true, true, tile_pixels }, vd ? &pieces[k].vd : nullptr);
+			rc = render_batches(s, pieces[k].td, pieces[k].pixels, pass_begin, pass_count, flags, { true, true, true, tile_pixels }, vd ? &pieces[k].vd : nullptr,
+			                    adapt);
 	} else {
 		uint64_t widest = 1;
 		for (const Piece &p : pieces) widest = p.pixels > widest ? p.pixels : widest;
@@ -1452,7 +1461,7 @@ static int render_call(crgpu_scene *s, const TileDesc &base, uint64_t tile_pixel
 			const int n = pass_begin + pass_count - pb < passes ? pass_begin + pass_count - pb : passes;
 			for (size_t k = 0; rc == CRGPU_OK && k < pieces.size(); ++k)
 				rc = render_batches(s, pieces[k].td, pieces[k].pixels, pb, n, flags, { k == 0, k + 1 == pieces.size(), false, tile_pixels },
-				                    vd ? &pieces[k].vd : nullptr);
+				                    vd ? &pieces[k].vd : nullptr, adapt);
 		}
 	}
 	if (armed) {
@@ -2445,6 +2454,7 @@ extern "C" int crgpu_scene_set_render(crgpu_scene *s, uint32_t width, uint32_t h
 		DevBlock &fb = e.stage(s->fb), &views = e.stage(s->views);
 		e.stage(s->fb8);
 		e.stage(s->snap8);
+		e.stage(s->adapt);                             /* the pixel records are of the old size: a round needs a new reset */
 		if ((rc = fb.alloc(s->device, fb_floats * sizeof(float)))) return rc;
 		if (count > 1u && (rc = views.alloc(s->device, views_bytes(cap, fb_floats)))) return rc;
 		CU(cudaMemsetAsync(fb.p, 0, fb.bytes, s->stream));
@@ -2493,6 +2503,127 @@ extern "C" int crgpu_render_views(crgpu_scene *s, uint32_t first_view, uint32_t 
 	memset(&td, 0, sizeof td);
 	td.pixels = s->pixels.as<uint32_t>();
 	return render_call(s, td, npix * view_count, pass_begin, pass_count, flags, stats, &vd);
+}
+
+/* ---- adaptive rounds ----------------------------------------------------------------------------------------------------------------
+ * The adaptive block: W*H pixel records (AdaptPix, framebuffer order), then the select's scratch for a tile set of up to W*H pixels: the
+ * active list, the flags and their inclusive scan, the scan's block sums, and the min / max words. */
+struct AdaptParts {
+	AdaptPix *recs;
+	uint32_t *active;
+	unsigned long long *flags, *incl, *sums, *sums2;
+	unsigned *mm;
+};
+static size_t adapt_carve(void *base, size_t npix, AdaptParts *p) {
+	size_t off = 0;
+	auto take = [&](size_t bytes) { void *q = base ? static_cast<uint8_t *>(base) + off : nullptr; off += align256(bytes); return q; };
+	p->recs = (AdaptPix *)take(npix * sizeof(AdaptPix));
+	p->active = (uint32_t *)take(npix * 4u);
+	p->flags = (unsigned long long *)take(npix * 8u);
+	p->incl = (unsigned long long *)take(npix * 8u);
+	p->sums = (unsigned long long *)take(8u * (npix / 1024u + 1u));
+	p->sums2 = (unsigned long long *)take(8u * (npix / (1024u * 1024u) + 1u));
+	p->mm = (unsigned *)take(8u);
+	return off;
+}
+
+extern "C" int crgpu_adaptive_reset(crgpu_scene *s) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	int rc = drain(s);                                                /* an asynchronous round may still update the records */
+	if (rc) return rc;
+	const size_t npix = (size_t)s->dev.image_width * s->dev.image_height;
+	if (npix > (1ull << 30)) return fail(CRGPU_ERR_UNSUPPORTED, "adaptive rounds need images of at most 2^30 pixels");
+	if (!s->adapt_host) {
+		void *p = nullptr;
+		CU(cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable));
+		s->adapt_host = static_cast<unsigned *>(p);
+	}
+	AdaptParts p;
+	if (!s->adapt.p && (rc = s->adapt.alloc(s->device, adapt_carve(nullptr, npix, &p)))) return rc;
+	adapt_carve(s->adapt.p, npix, &p);
+	crg_launch_adapt_reset(p.recs, npix, s->stream);
+	CU(cudaGetLastError());
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+/* no pixel of the tile set listed twice: K5 would add two passes to it at once.  The last set found clean is remembered. */
+static int check_disjoint(crgpu_scene *s, const int *rects, int nrects) {
+	std::vector<int> key(rects, rects + 4 * (size_t)nrects);
+	if (key == s->adapt_key) return CRGPU_OK;
+	const size_t W = s->dev.image_width;
+	std::vector<uint8_t> seen(W * s->dev.image_height, 0u);
+	for (int i = 0; i < nrects; ++i) {
+		const int *r = rects + 4 * i;
+		for (int y = r[1]; y < r[3]; ++y)
+			for (int x = r[0]; x < r[2]; ++x) {
+				uint8_t &b = seen[(size_t)y * W + (size_t)x];
+				if (b) return fail(CRGPU_ERR_BAD_ARGUMENT, "tile %d [%d,%d)x[%d,%d) overlaps an earlier tile at (%d, %d)", i, r[0], r[2], r[1], r[3], x, y);
+				b = 1u;
+			}
+	}
+	s->adapt_key.swap(key);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, unsigned flags,
+                                    struct crgpu_stats *stats, uint32_t *active, int *pass_begin, int *pass_end_of_round) {
+	if (!s || !a || !active || !pass_begin || !pass_end_of_round) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (a->min_passes < 2u || a->round_passes < 1u || a->pass_end < 1u || a->pass_end > s->dev.sample_count)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "min_passes %u (>= 2), round_passes %u (>= 1) or pass_end %u (1 .. %u) out of range", a->min_passes,
+		            a->round_passes, a->pass_end, s->dev.sample_count);
+	if (!std::isfinite(a->threshold) || a->threshold < 0.f || !std::isfinite(a->floor) || !(a->floor > 0.f))
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "threshold %g must be finite and >= 0, floor %g finite and > 0", (double)a->threshold, (double)a->floor);
+	if (!s->adapt.p) return fail(CRGPU_ERR_BAD_ARGUMENT, "no adaptive state at this image size: call crgpu_adaptive_reset");
+	uint64_t npix = 0;
+	int rc = tile_set(s, rects, nrects, 0, &npix);
+	if (rc) return rc;
+	if ((rc = check_disjoint(s, rects, nrects))) return rc;
+	AdaptParts p;
+	adapt_carve(s->adapt.p, (size_t)s->dev.image_width * s->dev.image_height, &p);
+	const AdaptParams ap = { a->min_passes, a->round_passes, a->pass_end, a->threshold, a->floor };
+	const int W = (int)s->dev.image_width, H = (int)s->dev.image_height;
+	const unsigned n = (unsigned)npix;
+	const uint32_t *pixels = s->pixels.as<uint32_t>();
+	CU(cudaMemsetAsync(p.mm, 0, 8u, s->stream));
+	crg_launch_adapt_select(pixels, n, p.recs, W, H, ap, p.flags, p.mm, s->stream);
+	const int scans = crg_scan64(p.flags, p.incl, p.sums, p.sums2, n, s->stream);
+	crg_launch_adapt_compact(pixels, n, p.recs, W, H, ap, p.flags, p.incl, p.active, p.mm, s->adapt_host, s->stream);
+	CU(cudaGetLastError());
+	s->pend_launches += 2u + (uint64_t)scans;
+	CU(cudaStreamSynchronize(s->stream));                            /* the round's one synchronisation: the active count and its passes */
+	const unsigned count = __atomic_load_n(&s->adapt_host[0], __ATOMIC_ACQUIRE);
+	const unsigned lo = __atomic_load_n(&s->adapt_host[1], __ATOMIC_ACQUIRE), hi = __atomic_load_n(&s->adapt_host[2], __ATOMIC_ACQUIRE);
+	if (count && lo != hi)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "the tile set's active pixels hold %u to %u passes: finish the overlapping tile set first", lo, hi);
+	*active = count;
+	if (!count) {
+		*pass_begin = *pass_end_of_round = (int)a->pass_end;
+		return flags & CRGPU_FLAG_ASYNC ? CRGPU_OK : crgpu_get_stats(s, stats);
+	}
+	unsigned next = lo < a->min_passes ? a->min_passes : a->min_passes + ((lo - a->min_passes) / a->round_passes + 1u) * a->round_passes;
+	if (next > a->pass_end) next = a->pass_end;
+	*pass_begin = (int)lo;
+	*pass_end_of_round = (int)next;
+	TileDesc td;
+	memset(&td, 0, sizeof td);
+	td.pixels = p.active;
+	return render_call(s, td, count, (int)lo, (int)(next - lo), flags, stats, nullptr, p.recs);
+}
+
+extern "C" int crgpu_adaptive_read(crgpu_scene *s, uint32_t *passes, float *err) {
+	if (!s) return fail(CRGPU_ERR_BAD_ARGUMENT, "scene is NULL");
+	if (!s->adapt.p) return fail(CRGPU_ERR_BAD_ARGUMENT, "no adaptive state at this image size: call crgpu_adaptive_reset");
+	const size_t npix = (size_t)s->dev.image_width * s->dev.image_height;
+	std::vector<AdaptPix> h(npix);
+	CU(cudaSetDevice(s->device));
+	CU(cudaMemcpyAsync(h.data(), s->adapt.p, npix * sizeof(AdaptPix), cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	for (size_t i = 0; i < npix; ++i) {
+		if (passes) passes[i] = h[i].n & ~CRG_ADAPT_DONE;
+		if (err) err[i] = h[i].err;
+	}
+	return CRGPU_OK;
 }
 
 static int check_view(const crgpu_scene *s, uint32_t view) {

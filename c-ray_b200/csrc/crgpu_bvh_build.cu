@@ -444,7 +444,7 @@ struct DevBuf {
 
 #define CUB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return crg_fail(e_ == cudaErrorMemoryAllocation ? CRGPU_ERR_NOMEM : CRGPU_ERR_CUDA, "crgpu_bvh_build: %s: %s", #call, cudaGetErrorString(e_)); } while (0)
 
-static int scan64(const unsigned long long *in, unsigned long long *out, unsigned long long *sums, unsigned long long *sums2, uint32_t n, cudaStream_t st) {
+int crg_scan64(const unsigned long long *in, unsigned long long *out, unsigned long long *sums, unsigned long long *sums2, uint32_t n, cudaStream_t st) {
 	const uint32_t nb = (n + BVB_SCAN_BLOCK - 1u) / BVB_SCAN_BLOCK;
 	k_scan_blocks<<<nb, 256, 0, st>>>(in, out, sums, n);
 	if (nb > 1u) {
@@ -455,8 +455,9 @@ static int scan64(const unsigned long long *in, unsigned long long *out, unsigne
 			k_scan_add<<<(nb + 255u) / 256u, 256, 0, st>>>(sums, sums2, nb);
 		}
 		k_scan_add<<<(n + 255u) / 256u, 256, 0, st>>>(out, sums, n);
+		return nb2 > 1u ? 5 : 3;
 	}
-	return 0;
+	return 1;
 }
 
 /* The records of a build: the scratch's 2n until a level could need more, then a device array of their own.  A tree needs more than
@@ -513,10 +514,10 @@ static int build_tree(const float *bb, const float *ctr, uint32_t n, const Scrat
 		k_bin<<<gn, 256, 0, st>>>(bb, ctr, s.prims, s.owner, recs, s.bins, n);
 		k_split<<<go, 128, 0, st>>>(bb, s.prims, recs, open_list, nopen, s.bins);
 		k_flag<<<gn, 256, 0, st>>>(ctr, s.prims, s.owner, recs, s.flags, n);
-		scan64(s.flags, s.S1, s.sums, s.sums2, n, st);
+		crg_scan64(s.flags, s.S1, s.sums, s.sums2, n, st);
 		k_mid<<<go, 128, 0, st>>>(recs, open_list, nopen, s.S1);
 		k_misplaced<<<gn, 256, 0, st>>>(s.owner, recs, s.flags, s.mis, n);
-		scan64(s.mis, s.S2, s.sums, s.sums2, n, st);
+		crg_scan64(s.mis, s.S2, s.sums, s.sums2, n, st);
 		k_scatter_right<<<gn, 256, 0, st>>>(s.owner, recs, s.mis, s.S2, s.tmpR, n);
 		k_swap<<<gn, 256, 0, st>>>(s.owner, recs, s.mis, s.S2, s.tmpR, s.prims, n);
 		k_children<<<go, 128, 0, st>>>(recs, open_list, nopen, next_list, counters);

@@ -53,3 +53,9 @@ struct CrgMeshRepack {
 };
 CRG_WEAK void crg_launch_mesh_repack(const CrgMeshRepack &m, const int32_t *prims, PackedTri *tris, uint32_t *slot_poly, uint8_t *keys,
                                      ShadePoly *spolys, cudaStream_t st);
+
+/* The builder's inclusive prefix sum of n 64-bit words (the two 32-bit halves summed independently: each must stay below 2^32), for
+ * n <= 2^30, enqueued on st.  `in` may be `out`.  sums holds ceil(n / 1024) words and sums2 ceil(n / 2^20) (at most 1024) words of
+ * scratch.  Returns the number of kernels it launched. */
+CRG_WEAK int crg_scan64(const unsigned long long *in, unsigned long long *out, unsigned long long *sums, unsigned long long *sums2, uint32_t n,
+                        cudaStream_t st);

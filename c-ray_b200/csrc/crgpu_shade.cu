@@ -328,11 +328,13 @@ __global__ void __launch_bounds__(128) k_tail(const DevScene *__restrict__ scp, 
  * publish step left.
  * VIEWS (crgpu_render_views): px is a piece pixel of the view-major numbering (ViewDesc) and goes to its view's framebuffer with the
  * same walk and arithmetic.  Armed, a views call stages no snapshot: block 0 clears gate[3] so that its publish steps stay one
- * thread's work, and a request stays pending. */
-template <bool ARMED, bool VIEWS>
+ * thread's work, and a request stays pending.
+ * ADAPTIVE (crgpu_adaptive_round, never with VIEWS): each pass added to a pixel also goes into its record, in pass order: n + 1 and
+ * the Welford update of the mean and M2 of the sample's luminance, fp32 under the library's IEEE flags. */
+template <bool ARMED, bool VIEWS, bool ADAPTIVE = false>
 __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, const float4 *__restrict__ L, TileDesc td,
 													 int image_width, int image_height, unsigned *__restrict__ gate, int set,
-													 const unsigned *__restrict__ snap_host, ViewDesc vd) {
+													 const unsigned *__restrict__ snap_host, ViewDesc vd, AdaptPix *__restrict__ adapt = nullptr) {
 	if (ARMED && VIEWS && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = 0u;
 	else if (ARMED && snap_host && blockIdx.x == 0 && threadIdx.x == 0) gate[3] = crg_ld_sys(snap_host + 3) == 1u ? 1u : 0u;
 	if (ARMED && (gate[1 + set] != 0u || gate[0] != (unsigned)td.pass_begin)) return;
@@ -346,8 +348,11 @@ __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, cons
 			crg_pixel_xy(td, tp, x, y);
 			if (v) img = vd.fb + (size_t)(v - 1u) * vd.fb_floats;
 		} else crg_pixel_xy(td, px, x, y);
-		float *dst = img + ((size_t)x + (size_t)(image_height - (y + 1)) * (size_t)image_width) * 3u;  /* texture.c:24-28 */
+		const size_t pi = (size_t)x + (size_t)(image_height - (y + 1)) * (size_t)image_width;
+		float *dst = img + pi * 3u;                                                                      /* texture.c:24-28 */
 		float r = dst[0], g = dst[1], b = dst[2];
+		AdaptPix rec;
+		if (ADAPTIVE) rec = adapt[pi];
 		/* the pixel's passes in pass order (crg_path_pass_pixel): within a pass group its paths are `step` apart, and the whole groups
 		 * start P * tile_pixels apart, so only the first group and a last, shorter one need the map.  With P = 1 this is the
 		 * pass-major walk L[pass * tile_pixels + px]; with Q = 4 the quarter-warps of a block read 64 contiguous bytes per pass. */
@@ -360,6 +365,13 @@ __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, cons
 				const float k = (float)(completed - 1);
 				const float t = cr_div(1.0f, (float)completed);
 				r = (r * k + s.x) * t; g = (g * k + s.y) * t; b = (b * k + s.z) * t;
+				if (ADAPTIVE) {
+					const float lum = (0.2126f * s.x + 0.7152f * s.y) + 0.0722f * s.z;
+					++rec.n;
+					const float d = lum - rec.mean;
+					rec.mean = rec.mean + cr_div(d, (float)(rec.n & ~CRG_ADAPT_DONE));
+					rec.m2 = rec.m2 + d * (lum - rec.mean);
+				}
 			}
 			c0 += pc;
 			if (c0 >= npass) break;
@@ -367,6 +379,68 @@ __global__ void __launch_bounds__(256) k_accumulate(float *__restrict__ fb, cons
 			else { pc = npass - c0; id = crg_path_id(c0, px, tile_pixels, npass, P, Q); }
 		}
 		dst[0] = r; dst[1] = g; dst[2] = b;
+		if (ADAPTIVE) adapt[pi] = rec;
+	}
+}
+
+/* ---- adaptive rounds: the convergence test and the active list ----------------------------------------------------------------- */
+/* a test point: min_passes + j round_passes below pass_end */
+__device__ __forceinline__ bool crg_adapt_test_point(unsigned k, const AdaptParams &a) {
+	return k >= a.min_passes && k < a.pass_end && (k - a.min_passes) % a.round_passes == 0u;
+}
+/* the pixel's record after the test at its count; returns whether it was tested */
+__device__ __forceinline__ bool crg_adapt_test(AdaptPix &p, const AdaptParams &a) {
+	const unsigned n = p.n & ~CRG_ADAPT_DONE;
+	if ((p.n & CRG_ADAPT_DONE) || !crg_adapt_test_point(n, a)) return false;
+	const float fn = (float)n;
+	p.err = cr_div(__fsqrt_rn(cr_div(cr_div(p.m2, (float)(n - 1u)), fn)), p.mean > a.floor ? p.mean : a.floor);
+	if (p.err < a.threshold) p.n |= CRG_ADAPT_DONE;                  /* a NaN error never stops a pixel */
+	return true;
+}
+__device__ __forceinline__ size_t crg_adapt_index(uint32_t xy, int W, int H) {
+	return (size_t)(xy & 0xffffu) + (size_t)(H - 1 - (int)(xy >> 16)) * (size_t)W;
+}
+
+__global__ void k_adapt_reset(AdaptPix *recs, size_t n) {
+	for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+		recs[i] = AdaptPix{ 0u, 0.f, 0.f, __int_as_float(0x7f800000) };
+}
+
+/* the warps walk the list warp-uniformly, so each warp reduces its min and max before one atomic each */
+__global__ void __launch_bounds__(256) k_adapt_select(const uint32_t *__restrict__ pixels, unsigned npix, const AdaptPix *__restrict__ recs,
+                                                      int W, int H, AdaptParams a, unsigned long long *__restrict__ flags, unsigned *mm) {
+	const unsigned lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+	for (unsigned w0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w0 < npix; w0 += stride) {
+		const unsigned i = w0 + lane;
+		unsigned lo = 0u, hi = 0u;
+		if (i < npix) {
+			AdaptPix p = recs[crg_adapt_index(pixels[i], W, H)];
+			crg_adapt_test(p, a);
+			const unsigned n = p.n & ~CRG_ADAPT_DONE;
+			const bool act = !(p.n & CRG_ADAPT_DONE) && n < a.pass_end;
+			flags[i] = act ? 1ull : 0ull;
+			if (act) { lo = ~n; hi = n; }
+		}
+		lo = __reduce_max_sync(0xffffffffu, lo);
+		hi = __reduce_max_sync(0xffffffffu, hi);
+		if (lane == 0u && lo) { atomicMax(mm, lo); atomicMax(mm + 1, hi); }
+	}
+}
+
+__global__ void __launch_bounds__(256) k_adapt_compact(const uint32_t *__restrict__ pixels, unsigned npix, AdaptPix *__restrict__ recs, int W, int H,
+                                                       AdaptParams a, const unsigned long long *__restrict__ flags,
+                                                       const unsigned long long *__restrict__ incl, uint32_t *__restrict__ active,
+                                                       const unsigned *__restrict__ mm, unsigned *host) {
+	const unsigned count = (unsigned)incl[npix - 1u], lo = ~mm[0], hi = mm[1];
+	const bool go = count == 0u || lo == hi;                           /* else the round is refused and changes nothing */
+	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += gridDim.x * blockDim.x) {
+		if (i == 0u) { host[0] = count; host[1] = lo; host[2] = hi; }
+		if (!go) continue;
+		const uint32_t xy = pixels[i];
+		const size_t pi = crg_adapt_index(xy, W, H);
+		AdaptPix p = recs[pi];
+		if (crg_adapt_test(p, a)) recs[pi] = p;
+		if (flags[i]) active[incl[i] - 1ull] = xy;
 	}
 }
 
@@ -525,12 +599,27 @@ void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigne
 	k_libm<<<256, 256, 0, st>>>(fn, x, y, out, n);
 }
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st, unsigned *gate, int set,
-                           const unsigned *snap_host, const ViewDesc *vd) {
-	if (vd) {
+                           const unsigned *snap_host, const ViewDesc *vd, AdaptPix *adapt) {
+	if (adapt) {
+		if (gate) k_accumulate<true, false, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, snap_host, ViewDesc{}, adapt);
+		else k_accumulate<false, false, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr, ViewDesc{}, adapt);
+	} else if (vd) {
 		if (gate) k_accumulate<true, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, nullptr, *vd);
 		else k_accumulate<false, true><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr, *vd);
 	} else if (gate) k_accumulate<true, false><<<grid, 256, 0, st>>>(fb, L, td, W, H, gate, set, snap_host, ViewDesc{});
 	else k_accumulate<false, false><<<grid, 256, 0, st>>>(fb, L, td, W, H, nullptr, 0, nullptr, ViewDesc{});
+}
+void crg_launch_adapt_reset(AdaptPix *recs, size_t n, cudaStream_t st) { k_adapt_reset<<<1024, 256, 0, st>>>(recs, n); }
+void crg_launch_adapt_select(const uint32_t *pixels, unsigned npix, const AdaptPix *recs, int W, int H, const AdaptParams &a,
+                             unsigned long long *flags, unsigned *mm, cudaStream_t st) {
+	const unsigned grid = (npix + 255u) / 256u < 4096u ? (npix + 255u) / 256u : 4096u;
+	k_adapt_select<<<grid, 256, 0, st>>>(pixels, npix, recs, W, H, a, flags, mm);
+}
+void crg_launch_adapt_compact(const uint32_t *pixels, unsigned npix, AdaptPix *recs, int W, int H, const AdaptParams &a,
+                              const unsigned long long *flags, const unsigned long long *incl, uint32_t *active, const unsigned *mm,
+                              unsigned *host, cudaStream_t st) {
+	const unsigned grid = (npix + 255u) / 256u < 4096u ? (npix + 255u) / 256u : 4096u;
+	k_adapt_compact<<<grid, 256, 0, st>>>(pixels, npix, recs, W, H, a, flags, incl, active, mm, host);
 }
 void crg_launch_to_srgb8(const float *fb, uint8_t *out, size_t n, int grid, cudaStream_t st) {
 	k_to_srgb8<<<grid, 256, 0, st>>>(fb, out, n);

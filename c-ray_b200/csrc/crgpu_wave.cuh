@@ -206,12 +206,34 @@ int crg_launch_shade(const DevScene *dsc, const WaveBuffers &wb, int cur, int de
 bool crg_shade_flat_order(const ShadeKnobs &kn);
 /* the libm stand-ins of crgpu_math.cuh one by one (crgpu_libm_eval) */
 void crg_launch_libm(int fn, const float *x, const float *y, float *out, unsigned n, cudaStream_t st);
+/* ---- adaptive rounds (crgpu_adaptive_round) -------------------------------------------------------------------------------------
+ * Every pixel of view 0 has one record, at its framebuffer index (x + (H - 1 - y) W): the passes its framebuffer holds, the Welford
+ * mean and M2 of their luminance, and the error of its last convergence test.  Only K5 <ADAPTIVE> adds passes to a record, and only
+ * passes it commits; the select kernels test and mark pixels done. */
+#define CRG_ADAPT_DONE 0x80000000u   /* AdaptPix::n: the pixel has converged */
+struct AdaptPix { uint32_t n; float mean, m2, err; };
+struct AdaptParams { unsigned min_passes, round_passes, pass_end; float threshold, floor; };
+/* every record of n to { 0, 0, 0, +inf } */
+void crg_launch_adapt_reset(AdaptPix *recs, size_t n, cudaStream_t st);
+/* select, step 1 of 2: for pixel i of the list (x | y << 16), whether it stays active after the test at its count (flags[i] = 0 or 1),
+ * and into mm the max of ~n and of n over the active pixels (mm zeroed before) */
+void crg_launch_adapt_select(const uint32_t *pixels, unsigned npix, const AdaptPix *recs, int W, int H, const AdaptParams &a,
+                             unsigned long long *flags, unsigned *mm, cudaStream_t st);
+/* step 2, after the inclusive scan incl of flags: when every active pixel has the same count (or none is active) each tested pixel
+ * takes its error and done bit and each active pixel its place in the active list; in any case host[0..2] = active count, min and
+ * max count */
+void crg_launch_adapt_compact(const uint32_t *pixels, unsigned npix, AdaptPix *recs, int W, int H, const AdaptParams &a,
+                              const unsigned long long *flags, const unsigned long long *incl, uint32_t *active, const unsigned *mm,
+                              unsigned *host, cudaStream_t st);
+
 /* gate: NULL, or the stop words of an armed scene (below): K5 then adds the batch only if wave set `set`'s batch was not abandoned
  * and the committed pass index equals td.pass_begin.  snap_host: NULL, or (a batch that publishes) the host words, whose snapshot
  * state K5 reads once into gate[3] for the publish step.  vd: NULL, or the views of a views call (K5 <ARMED, VIEWS = true>: each
- * (view, pixel) into its view's framebuffer; armed, it clears gate[3], so a views call never stages a snapshot) */
+ * (view, pixel) into its view's framebuffer; armed, it clears gate[3], so a views call never stages a snapshot).  adapt: NULL, or
+ * the records of an adaptive round (K5 <ADAPTIVE = true>, never with vd): each added pass also updates its pixel's record. */
 void crg_launch_accumulate(float *fb, const float4 *L, const TileDesc &td, int W, int H, int grid, cudaStream_t st,
-                           unsigned *gate = nullptr, int set = 0, const unsigned *snap_host = nullptr, const ViewDesc *vd = nullptr);
+                           unsigned *gate = nullptr, int set = 0, const unsigned *snap_host = nullptr, const ViewDesc *vd = nullptr,
+                           AdaptPix *adapt = nullptr);
 
 /* ---- stopping an armed scene at a pass boundary (crgpu_stop_enable) ----------------------------------------------------------------
  * ctl (device memory): [0] the pass index the running average has reached in this call, [1 + set] wave set `set`'s batch was

@@ -113,6 +113,10 @@ struct renderer {
 	void *comm;                    /* crgpu_comm*: persistent NCCL communicator (in-process group or this rank's membership) */
 	int commMembers;               /* size of the group `comm` was created for */
 	bool renderBufferPinned;
+	/* adaptive sampling (crhostSetAdaptive): the workers render their shares in adaptive rounds (crgpu_adaptive_round) */
+	bool adaptive;
+	float adaptiveThreshold;
+	uint32_t *adaptivePasses;      /* W*H pass counts of the last adaptive frame, framebuffer order (NULL before one) */
 };
 
 /* tile dispatcher */
@@ -150,6 +154,13 @@ void crhostConfigure(struct renderer *r, int gpus, unsigned tileWidth, unsigned 
  * least min_prims primitives; on == 0 goes back to the host builder.  Same tree either way.  Also switched on by the environment
  * variable CRAY_GPU_BVH=<min_prims> (read by loadSceneFile / loadSceneBuf). */
 void crhostUseGpuBvh(int on, int device, unsigned min_prims);
+/* Adaptive sampling (crgpu_adaptive_round, DESIGN §4 "Rendering adaptively"): with on != 0 every later frame stops sampling a pixel once
+ * its error estimate falls below `threshold` (finite, >= 0; 0 renders every pass), testing first at min(16, samples) passes (at least
+ * 2) and then every 16, relative to a mean luminance of at least 0.01.  Those three are choices, not measurements.  Returns -1 and
+ * changes nothing for a bad threshold.  crhostAdaptivePasses: the W*H pass counts of the last adaptive frame in framebuffer order (row
+ * H-1-y first), the tiles of this process only in a ranked job; NULL before one. */
+int crhostSetAdaptive(struct renderer *r, int on, float threshold);
+const uint32_t *crhostAdaptivePasses(const struct renderer *r);
 void crhostImageSize(const struct renderer *r, unsigned *w, unsigned *h, int *samples, int *bounces);
 void *crhostComm(struct renderer *r);
 const void *crhostPrepared(struct renderer *r);

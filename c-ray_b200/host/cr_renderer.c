@@ -20,6 +20,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <math.h>
 #include <time.h>
 
 /* The NCCL tile gather lives in its own library (libcrgpu_nccl.so) and is loaded on first use: a single-GPU render never
@@ -100,6 +101,14 @@ static void gpu_bvh_from_env(void) {
 	const char *e = getenv("CRAY_GPU_BVH");
 	if (e && *e) crhostUseGpuBvh(1, 0, (unsigned)strtoul(e, NULL, 10));
 }
+
+int crhostSetAdaptive(struct renderer *r, int on, float threshold) {
+	if (!r || (on && !(isfinite(threshold) && threshold >= 0.f))) return -1;
+	r->adaptive = on != 0;
+	r->adaptiveThreshold = threshold;
+	return 0;
+}
+const uint32_t *crhostAdaptivePasses(const struct renderer *r) { return r ? r->adaptivePasses : NULL; }
 
 static void drop_prepared(struct renderer *r) { if (r->prepared) { crgpu_prepared_free(r->prepared); r->prepared = NULL; } }
 
@@ -299,12 +308,18 @@ void *gpuRenderThread(void *arg) {
 		if (got == 0) break;
 		ts->currentTileNum = nums[0];
 		ts->tiles = got;
-		/* The share is ONE armed, asynchronous call.  Like renderThread's loop (renderer.c:271-320), this thread polls about every
-		 * 16 ms: it publishes the committed passes, forwards renderAborted and the pause flags as a stop (the call ends at the next
-		 * pass boundary), waits while paused, and resumes from the committed pass: the frame is the same bit for bit. */
+		/* The share is ONE armed, asynchronous call (adaptive: one per round).  Like renderThread's loop (renderer.c:271-320), this thread
+		 * polls about every 16 ms: it publishes the committed passes, forwards renderAborted and the pause flags as a stop (the call ends at
+		 * the next pass boundary), waits while paused, and resumes from the committed pass: the frame is the same bit for bit. */
 		const int spp = r->prefs.sampleCount;
 		const double t0 = now_s();
 		int rc = crgpu_stop_enable(ts->gpu, 1);
+		/* adaptive rounds: the pixels of the share start from a fresh record, and each round's select picks the pixels to render */
+		const struct crgpu_adaptive rule = { spp < 16 ? (spp < 2 ? 2u : (uint32_t)spp) : 16u, 16u, (uint32_t)spp, r->adaptiveThreshold, 0.01f };
+		uint64_t share_pixels = 0, paths_done = 0;
+		for (int i = 0; i < got; ++i) share_pixels += (uint64_t)(rects[4 * i + 2] - rects[4 * i]) * (uint64_t)(rects[4 * i + 3] - rects[4 * i + 1]);
+		if (rc == CRGPU_OK && r->adaptive) rc = crgpu_adaptive_reset(ts->gpu);
+		bool finished = false;
 		int begin = 0;
 		/* The live preview: like renderThread, which writes each pixel's running average into the 8-bit image after every pass
 		 * (renderer.c:294-300), but at most every CR_PREVIEW_INTERVAL_MS.  The worker asks for a snapshot when its committed pass has
@@ -317,16 +332,27 @@ void *gpuRenderThread(void *arg) {
 		int shown = 0;
 		bool asked = false;
 		double last_snap = t0;
-		while (rc == CRGPU_OK && begin < spp) {
-			rc = crgpu_render_tiles(ts->gpu, rects, got, begin, spp - begin, CRGPU_FLAG_ASYNC, NULL);
+		while (rc == CRGPU_OK) {
+			int from = begin;
+			uint32_t active = 0;
+			if (r->adaptive) {
+				int to = 0;
+				rc = crgpu_adaptive_round(ts->gpu, rects, got, &rule, CRGPU_FLAG_ASYNC, NULL, &active, &from, &to);
+				if (rc == CRGPU_OK && active == 0) { finished = true; break; }
+			} else {
+				if (begin >= spp) { finished = true; break; }
+				rc = crgpu_render_tiles(ts->gpu, rects, got, begin, spp - begin, CRGPU_FLAG_ASYNC, NULL);
+			}
 			if (rc != CRGPU_OK) break;
-			int done = begin, busy = 1;
+			int done = from, busy = 1;
 			bool stopping = false;
 			for (;;) {
 				crgpu_progress(ts->gpu, &done, &busy);
 				ts->completedSamples = done;
-				ts->totalSamples = (uint64_t)done * (uint64_t)got;                    /* tile-passes done, renderer.c:307 */
-				if (done > 0) ts->avgSampleTime = (long)(1e6 * (now_s() - t0) / ((double)done * got));
+				/* tile-passes done, renderer.c:307; adaptive: the pixel-passes committed, in tiles of the share's mean size */
+				ts->totalSamples = r->adaptive ? (paths_done + (uint64_t)(done - from) * active) * (uint64_t)got / (share_pixels ? share_pixels : 1u)
+				                               : (uint64_t)done * (uint64_t)got;
+				if (ts->totalSamples > 0) ts->avgSampleTime = (long)(1e6 * (now_s() - t0) / (double)ts->totalSamples);
 				if (asked || !busy) {
 					/* with the call over, take answers from the framebuffer: a stop or pause shows its committed passes at once (a
 					 * finished share needs no snapshot: renderFrame's image follows) */
@@ -350,8 +376,9 @@ void *gpuRenderThread(void *arg) {
 			rc = crgpu_get_stats(ts->gpu, &st);
 			if (rc != CRGPU_OK) break;
 			ts->rays += st.rays;
+			paths_done += st.paths;
 			begin = done;
-			if (begin >= spp) break;
+			if (!r->adaptive && begin >= spp) { finished = true; break; }
 			while ((ts->paused || r->state.paused) && !r->state.renderAborted) sleep_ms(16);   /* renderer.c:310-312 */
 			if (r->state.renderAborted) break;
 			rc = crgpu_clear_stop(ts->gpu);
@@ -365,7 +392,7 @@ void *gpuRenderThread(void *arg) {
 		}
 		for (int i = 0; i < got; ++i) {
 			r->state.renderTiles[nums[i]].isRendering = false;                    /* renderer.c:315-316 */
-			r->state.renderTiles[nums[i]].renderComplete = begin >= spp;
+			r->state.renderTiles[nums[i]].renderComplete = finished;
 		}
 		ts->currentTileNum = -1;
 		break;                                                                    /* the worker's whole share was one trip */
@@ -377,6 +404,29 @@ void *gpuRenderThread(void *arg) {
 	pthread_cond_broadcast(&r->state.doneCond);
 	pthread_mutex_unlock(&r->state.doneMutex);
 	return NULL;
+}
+
+/* the pass counts of an adaptive frame: each tile's from the worker that rendered it (a rank: its own tiles only) */
+static int collect_passes(struct renderer *r, int n, bool ranked) {
+	const size_t W = r->prefs.imageWidth, H = r->prefs.imageHeight;
+	free(r->adaptivePasses);
+	r->adaptivePasses = calloc(W * H, sizeof(uint32_t));
+	uint32_t *mine = malloc(W * H * sizeof(uint32_t));
+	int err = r->adaptivePasses && mine ? 0 : CRGPU_ERR_NOMEM;
+	for (int t = 0; !err && t < n; ++t) {
+		const int who = ranked ? r->rank : t;
+		if (crgpu_adaptive_read(r->state.threadStates[t].gpu, mine, NULL) != CRGPU_OK) { err = CRGPU_ERR_CUDA; break; }
+		for (int i = 0; i < r->state.tileCount; ++i) {
+			const struct renderTile *tl = &r->state.renderTiles[i];
+			if (r->state.tileOwner[i] != who) continue;
+			for (int y = tl->begin.y; y < tl->end.y; ++y) {
+				const size_t off = (H - 1u - (size_t)y) * W + (size_t)tl->begin.x;
+				memcpy(r->adaptivePasses + off, mine + off, (size_t)(tl->end.x - tl->begin.x) * sizeof(uint32_t));
+			}
+		}
+	}
+	free(mine);
+	return err;
 }
 
 static double floor_div(double a, double b) { return (double)(long long)(a / b); }
@@ -504,6 +554,7 @@ struct texture8 *renderFrame(struct renderer *r) {
 		if (!err && crgpu_framebuffer_to_srgb8(root_scene, output->data) != CRGPU_OK) err = CRGPU_ERR_CUDA;            /* renderer.c:297-300 */
 	}
 	r->state.renderSeconds = now_s() - t0;
+	if (!err && r->adaptive) err = collect_passes(r, n, ranked);
 	for (int t = 0; t < n; ++t) if (r->state.threadStates[t].gpu) { crgpu_scene_destroy(r->state.threadStates[t].gpu); r->state.threadStates[t].gpu = NULL; }
 	if (!r->prefs.quiet && !err && !discard) {
 		const double samples = (double)W * H * r->prefs.sampleCount;
@@ -571,6 +622,7 @@ void destroyRenderer(struct renderer *r) {                       /* renderer.c:3
 	free_render_buffer(r);
 	free(r->state.renderTiles); free(r->state.tileOwner); free(r->state.threads); free(r->state.threadStates);
 	free(r->state.preview);
+	free(r->adaptivePasses);
 	pthread_mutex_destroy(&r->state.previewMutex);
 	pthread_mutex_destroy(&r->state.tileMutex);
 	pthread_mutex_destroy(&r->state.doneMutex);

@@ -326,6 +326,47 @@ int crgpu_view_to_srgb8(crgpu_scene *s, uint32_t view, uint8_t *host_rgb8);
 int crgpu_scene_set_render(crgpu_scene *s, uint32_t width, uint32_t height, uint32_t sample_count, uint32_t bounces,
                            const struct crs_camera *cams, uint32_t count);
 
+/* Rendering adaptively (DESIGN §4 "Rendering adaptively"): each pixel stops taking passes once its error estimate falls below a
+ * threshold, so flat sky or a diffuse wall far from any caustic stops early while noisy pixels go on to pass_end.  Every pixel of view 0
+ * has a record: n, the passes its framebuffer holds; the Welford mean and M2 of their luminance y = (0.2126 r + 0.7152 g) + 0.0722 b;
+ * the error of its last test; and a done bit.  Only K5 updates n, mean and M2, and only for the passes it commits.  The test points are
+ * k = min_passes + j round_passes below pass_end; at one, err = sqrt(M2 / (n - 1) / n) / max(mean, floor) (fp32), and the pixel is done
+ * when err < threshold (a NaN err never stops it).  The decision depends on the pixel's own samples only, and paths are seeded by
+ * (pixel, pass, sample count) only, so a pixel that holds n passes holds bit for bit what crgpu_render_tiles(rects, 0, n) gives it on a
+ * cleared framebuffer, whatever the tiling, pieces, paths in flight, path order, worker split or stops in between.
+ *   crgpu_adaptive_reset  allocates the adaptive block from the per-device cache the first time (16 B of record per pixel, plus the
+ *                         active list and the select's scratch: 44 B per pixel in all) and sets every record to n = 0, err = +inf, not
+ *                         done.  It waits for the scene's queued work.  crgpu_scene_set_render with a new size drops the block: a round
+ *                         is then refused until the next reset.  No other edit touches the records, as edits leave framebuffers alone.
+ *                         The block goes back to the cache at crgpu_scene_destroy.
+ *   crgpu_adaptive_round  one round over the tile set `rects` (as crgpu_render_tiles takes it, sharing its cached pixel list): a select
+ *                         step tests each pixel of the set that is not done and whose n is a test point, then compacts the pixels that
+ *                         are not done and have n < pass_end, in list order, into the active list and reads back their number and the
+ *                         min and max of their n (the round's one synchronisation).  With min = max = k it renders passes [k, next) of
+ *                         the active pixels as crgpu_render_tiles renders a pixel set (pieces, batches, flags, stop gates, progress,
+ *                         snapshots), where next is the smallest test point above k, capped at pass_end.  It returns *active, and
+ *                         *pass_begin = k, *pass_end_of_round = next; with no active pixel it renders nothing, returns CRGPU_OK and sets
+ *                         both to pass_end.  An armed round that is stopped returns CRGPU_STOPPED; the next round resumes from the
+ *                         committed pass.  stats as for crgpu_render_tiles (paths: the pixel-passes rendered), kernel_launches including
+ *                         the select's.  A NULL scene, a, active, pass_begin or pass_end_of_round, a field of `a` out of range, a
+ *                         scene with no adaptive block, a tile list crgpu_render_tiles refuses, tiles that overlap (K5 would add one
+ *                         pixel twice at once), and active pixels of different counts (two overlapping tile sets left at different
+ *                         passes) are refused with CRGPU_ERR_BAD_ARGUMENT; a refused round changes no record and no framebuffer pixel.
+ *                         Rounds work on view 0 only.
+ *   crgpu_adaptive_read   waits for the scene's stream and copies n and err of every pixel (W*H each, framebuffer order: row H-1-y
+ *                         first); either pointer may be NULL. */
+struct crgpu_adaptive {
+	uint32_t min_passes;    /* >= 2: the first convergence test is at this pass count */
+	uint32_t round_passes;  /* >= 1: later tests every round_passes passes */
+	uint32_t pass_end;      /* 1 .. the scene's sample_count: no pixel goes beyond it */
+	float    threshold;     /* finite, >= 0: a pixel stops when err < threshold (so 0 never stops a pixel early) */
+	float    floor;         /* finite, > 0: the mean luminance below which err is taken relative to `floor` */
+};
+int crgpu_adaptive_reset(crgpu_scene *s);
+int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, unsigned flags,
+                         struct crgpu_stats *stats, uint32_t *active, int *pass_begin, int *pass_end_of_round);
+int crgpu_adaptive_read(crgpu_scene *s, uint32_t *passes, float *err);
+
 /* Run on a caller-owned CUDA stream (a `cudaStream_t` passed as void*; NULL means the legacy default
  * stream, as everywhere in CUDA).  Lets a host that already has a stream (e.g. the one its NCCL collectives
  * use) order the kernels with its own work and time them with its own events.  crgpu_use_own_stream goes
