@@ -59,6 +59,12 @@ class Adaptive(C.Structure):
                 ("floor", C.c_float)]
 
 
+# struct crgpu_adaptive_record: a pixel's adaptive record (crgpu_adaptive_write / crgpu_adaptive_records); bit 31 of n is ADAPTIVE_DONE
+ADAPT_RECORD_DTYPE = np.dtype([("n", "<u4"), ("mean", "<f4"), ("m2", "<f4"), ("err", "<f4")])
+assert ADAPT_RECORD_DTYPE.itemsize == 16
+ADAPTIVE_DONE = 0x80000000
+
+
 class TraceOpts(C.Structure):
     """struct crgpu_trace_opts: the launch variant of the traversal kernel (crgpu_trace_rays)"""
     _fields_ = [(n, C.c_int32) for n in ("count", "minb", "defer", "refill", "burst", "inst_min")] + [("order", C.c_void_p)]
@@ -178,6 +184,14 @@ def lib():
                                                C.POINTER(C.c_int), C.POINTER(C.c_int)]
             L.crgpu_adaptive_read.argtypes = [P, P, P]
             for f in ("crgpu_adaptive_reset", "crgpu_adaptive_round", "crgpu_adaptive_read"):
+                getattr(L, f).restype = C.c_int
+        if hasattr(L, "crgpu_adaptive_select"):   # absent from libraries built before the adaptive kernels' test entry points
+            L.crgpu_accumulate_samples.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, P]
+            L.crgpu_adaptive_write.argtypes = [P, P]
+            L.crgpu_adaptive_records.argtypes = [P, P]
+            L.crgpu_adaptive_select.argtypes = [P, P, C.c_int, C.POINTER(Adaptive), P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                                C.POINTER(C.c_uint32)]
+            for f in ("crgpu_accumulate_samples", "crgpu_adaptive_write", "crgpu_adaptive_records", "crgpu_adaptive_select"):
                 getattr(L, f).restype = C.c_int
         _lib = L
     return _lib
@@ -405,6 +419,43 @@ class GpuScene:
         if getattr(self, "armed", False):
             total["stopped"] = False
         return total
+
+    def adaptive_records(self):
+        """Every pixel's whole record (ADAPT_RECORD_DTYPE [H, W], the framebuffer layout) (crgpu_adaptive_records)."""
+        out = np.empty((self.H, self.W), dtype=ADAPT_RECORD_DTYPE)
+        _check(lib().crgpu_adaptive_records(self.handle, out.ctypes.data), "crgpu_adaptive_records")
+        return out
+
+    def adaptive_write(self, recs):
+        """Load every pixel's record from ADAPT_RECORD_DTYPE [H, W] (crgpu_adaptive_write)."""
+        recs = np.ascontiguousarray(recs, dtype=ADAPT_RECORD_DTYPE)
+        assert recs.shape == (self.H, self.W)
+        _check(lib().crgpu_adaptive_write(self.handle, recs.ctypes.data), "crgpu_adaptive_write")
+
+    def adaptive_select(self, rects, min_passes, round_passes, threshold, floor, pass_end=None):
+        """A round's select, scan and compaction without its render (crgpu_adaptive_select): (active list uint32 x | y << 16, least
+        count, largest count)."""
+        a = Adaptive(min_passes, round_passes, self.samples if pass_end is None else pass_end, threshold, floor)
+        arr = np.ascontiguousarray(rects, dtype=np.int32).reshape(-1, 4)
+        npix = int(((arr[:, 2] - arr[:, 0]).astype(np.int64) * (arr[:, 3] - arr[:, 1])).sum())
+        active = np.empty(max(npix, 1), dtype=np.uint32)
+        count, lo, hi = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        _check(lib().crgpu_adaptive_select(self.handle, arr.ctypes.data, len(arr), C.byref(a), active.ctypes.data, C.byref(count),
+                                           C.byref(lo), C.byref(hi)), "crgpu_adaptive_select")
+        return active[:count.value].copy(), lo.value, hi.value
+
+    def accumulate_samples(self, rects, pass_begin, L, order=-1, adaptive=False):
+        """K5 on given radiance (crgpu_accumulate_samples): L is float32 [npix, passes, 4] in the tile set's list order, added to the
+        framebuffer as passes [pass_begin, +passes) under path order `order` (-1: the process's); with `adaptive` the records take
+        them too.  Returns the tile set's pixel list (uint32 x | y << 16)."""
+        arr = np.ascontiguousarray(rects, dtype=np.int32).reshape(-1, 4)
+        L = np.ascontiguousarray(L, dtype=np.float32)
+        npix = int(((arr[:, 2] - arr[:, 0]).astype(np.int64) * (arr[:, 3] - arr[:, 1])).sum())
+        assert L.ndim == 3 and L.shape[0] == npix and L.shape[2] == 4
+        pixels = np.empty(max(npix, 1), dtype=np.uint32)
+        _check(lib().crgpu_accumulate_samples(self.handle, arr.ctypes.data, len(arr), pass_begin, L.shape[1], order, 1 if adaptive else 0,
+                                              L.ctypes.data, pixels.ctypes.data), "crgpu_accumulate_samples")
+        return pixels[:npix]
 
     def view_count(self):
         n = C.c_uint32(0)

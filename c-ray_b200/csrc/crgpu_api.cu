@@ -2566,9 +2566,12 @@ static int check_disjoint(crgpu_scene *s, const int *rects, int nrects) {
 	return CRGPU_OK;
 }
 
-extern "C" int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, unsigned flags,
-                                    struct crgpu_stats *stats, uint32_t *active, int *pass_begin, int *pass_end_of_round) {
-	if (!s || !a || !active || !pass_begin || !pass_end_of_round) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+/* A round's select step over the tile set: test and flag (k_adapt_select), scan, compact (k_adapt_compact), then the one synchronisation.
+ * On success p holds the carved adaptive block, whose active list has *count pixels, all at *lo = *hi passes (with none active, *lo =
+ * 0xffffffff and *hi = 0).  Refused: fields of a out of range, no adaptive block, a bad or overlapping tile set, and active pixels of
+ * different counts (which the compaction leaves unrecorded). */
+static int adapt_select(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, AdaptParts &p, unsigned *count,
+                        unsigned *lo, unsigned *hi) {
 	if (a->min_passes < 2u || a->round_passes < 1u || a->pass_end < 1u || a->pass_end > s->dev.sample_count)
 		return fail(CRGPU_ERR_BAD_ARGUMENT, "min_passes %u (>= 2), round_passes %u (>= 1) or pass_end %u (1 .. %u) out of range", a->min_passes,
 		            a->round_passes, a->pass_end, s->dev.sample_count);
@@ -2579,7 +2582,6 @@ extern "C" int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects
 	int rc = tile_set(s, rects, nrects, 0, &npix);
 	if (rc) return rc;
 	if ((rc = check_disjoint(s, rects, nrects))) return rc;
-	AdaptParts p;
 	adapt_carve(s->adapt.p, (size_t)s->dev.image_width * s->dev.image_height, &p);
 	const AdaptParams ap = { a->min_passes, a->round_passes, a->pass_end, a->threshold, a->floor };
 	const int W = (int)s->dev.image_width, H = (int)s->dev.image_height;
@@ -2592,10 +2594,21 @@ extern "C" int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects
 	CU(cudaGetLastError());
 	s->pend_launches += 2u + (uint64_t)scans;
 	CU(cudaStreamSynchronize(s->stream));                            /* the round's one synchronisation: the active count and its passes */
-	const unsigned count = __atomic_load_n(&s->adapt_host[0], __ATOMIC_ACQUIRE);
-	const unsigned lo = __atomic_load_n(&s->adapt_host[1], __ATOMIC_ACQUIRE), hi = __atomic_load_n(&s->adapt_host[2], __ATOMIC_ACQUIRE);
-	if (count && lo != hi)
-		return fail(CRGPU_ERR_BAD_ARGUMENT, "the tile set's active pixels hold %u to %u passes: finish the overlapping tile set first", lo, hi);
+	*count = __atomic_load_n(&s->adapt_host[0], __ATOMIC_ACQUIRE);
+	*lo = __atomic_load_n(&s->adapt_host[1], __ATOMIC_ACQUIRE);
+	*hi = __atomic_load_n(&s->adapt_host[2], __ATOMIC_ACQUIRE);
+	if (*count && *lo != *hi)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "the tile set's active pixels hold %u to %u passes: finish the overlapping tile set first", *lo, *hi);
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_adaptive_round(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, unsigned flags,
+                                    struct crgpu_stats *stats, uint32_t *active, int *pass_begin, int *pass_end_of_round) {
+	if (!s || !a || !active || !pass_begin || !pass_end_of_round) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	AdaptParts p;
+	unsigned count = 0u, lo = 0u, hi = 0u;
+	int rc = adapt_select(s, rects, nrects, a, p, &count, &lo, &hi);
+	if (rc) return rc;
 	*active = count;
 	if (!count) {
 		*pass_begin = *pass_end_of_round = (int)a->pass_end;
@@ -2623,6 +2636,89 @@ extern "C" int crgpu_adaptive_read(crgpu_scene *s, uint32_t *passes, float *err)
 		if (passes) passes[i] = h[i].n & ~CRG_ADAPT_DONE;
 		if (err) err[i] = h[i].err;
 	}
+	return CRGPU_OK;
+}
+
+/* ---- test entry points of K5 and of a round's select (include/crgpu.h) ---------------------------------------------------------- */
+static_assert(sizeof(crgpu_adaptive_record) == sizeof(AdaptPix) && CRGPU_ADAPTIVE_DONE == CRG_ADAPT_DONE, "crgpu_adaptive_record is AdaptPix");
+
+extern "C" int crgpu_accumulate_samples(crgpu_scene *s, const int *rects, int nrects, int pass_begin, int pass_count, int order, int adaptive,
+                                        const float *L, uint32_t *pixels_out) {
+	if (!s || !L) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (order < -1 || order >= CRG_PATH_ORDERS) return fail(CRGPU_ERR_BAD_ARGUMENT, "path order %d outside -1 .. %d", order, CRG_PATH_ORDERS - 1);
+	if (adaptive && !s->adapt.p) return fail(CRGPU_ERR_BAD_ARGUMENT, "no adaptive state at this image size: call crgpu_adaptive_reset");
+	if (pass_begin < 0 || pass_count < 0 || (uint64_t)pass_begin + (uint64_t)pass_count > s->dev.sample_count)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "passes [%d,%d) outside [0,%u)", pass_begin, pass_begin + pass_count, s->dev.sample_count);
+	uint64_t npix = 0;
+	int rc = tile_set(s, rects, nrects, 0, &npix);
+	if (rc) return rc;
+	const uint64_t paths = npix * (uint64_t)pass_count;
+	if (paths > s->max_paths)
+		return fail(CRGPU_ERR_BAD_ARGUMENT, "%llu pixels x %d passes are more than the %llu paths in flight", (unsigned long long)npix, pass_count,
+		            (unsigned long long)s->max_paths);
+	if ((rc = drain(s)) || (rc = alloc_wave(s, paths ? paths : 1, 1))) return rc;
+	const PathOrder po = order < 0 ? crg_path_order() : crg_path_order_of(order);
+	std::vector<float4> h(paths);
+	for (uint64_t px = 0; px < npix; ++px)
+		for (int pl = 0; pl < pass_count; ++pl) {
+			const float *v = L + (px * (uint64_t)pass_count + (uint64_t)pl) * 4u;
+			h[crg_path_id((unsigned)pl, (unsigned)px, (unsigned)npix, (unsigned)pass_count, po.p, po.q)] = make_float4(v[0], v[1], v[2], v[3]);
+		}
+	if (paths) {
+		CU(cudaMemcpyAsync(s->wb.L, h.data(), paths * sizeof(float4), cudaMemcpyHostToDevice, s->stream));
+		TileDesc td;
+		memset(&td, 0, sizeof td);
+		td.pixels = s->pixels.as<uint32_t>();
+		td.npix = (unsigned)npix;
+		td.order = po;
+		td.pass_begin = pass_begin;
+		td.pass_count = pass_count;
+		AdaptParts p = {};
+		if (adaptive) adapt_carve(s->adapt.p, (size_t)s->dev.image_width * s->dev.image_height, &p);
+		crg_launch_accumulate(s->fb.as<float>(), s->wb.L, td, (int)s->dev.image_width, (int)s->dev.image_height, s->sm_count * 8, s->stream, nullptr, 0,
+		                      nullptr, nullptr, p.recs);
+		CU(cudaGetLastError());
+		s->pend_launches += 1u;
+	}
+	if (pixels_out && npix) CU(cudaMemcpyAsync(pixels_out, s->pixels.p, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_adaptive_write(crgpu_scene *s, const struct crgpu_adaptive_record *recs) {
+	if (!s || !recs) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (!s->adapt.p) return fail(CRGPU_ERR_BAD_ARGUMENT, "no adaptive state at this image size: call crgpu_adaptive_reset");
+	int rc = drain(s);
+	if (rc) return rc;
+	const size_t npix = (size_t)s->dev.image_width * s->dev.image_height;
+	CU(cudaMemcpyAsync(s->adapt.p, recs, npix * sizeof(AdaptPix), cudaMemcpyHostToDevice, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_adaptive_records(crgpu_scene *s, struct crgpu_adaptive_record *recs_out) {
+	if (!s || !recs_out) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	if (!s->adapt.p) return fail(CRGPU_ERR_BAD_ARGUMENT, "no adaptive state at this image size: call crgpu_adaptive_reset");
+	int rc = drain(s);
+	if (rc) return rc;
+	const size_t npix = (size_t)s->dev.image_width * s->dev.image_height;
+	CU(cudaMemcpyAsync(recs_out, s->adapt.p, npix * sizeof(AdaptPix), cudaMemcpyDeviceToHost, s->stream));
+	CU(cudaStreamSynchronize(s->stream));
+	return CRGPU_OK;
+}
+
+extern "C" int crgpu_adaptive_select(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, uint32_t *active_out,
+                                     uint32_t *count_out, uint32_t *lo_out, uint32_t *hi_out) {
+	if (!s || !a || !active_out || !count_out || !lo_out || !hi_out) return fail(CRGPU_ERR_BAD_ARGUMENT, "NULL argument");
+	AdaptParts p;
+	unsigned count = 0u, lo = 0u, hi = 0u;
+	int rc = adapt_select(s, rects, nrects, a, p, &count, &lo, &hi);
+	if (rc) return rc;
+	if (count) {
+		CU(cudaMemcpyAsync(active_out, p.active, (size_t)count * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+		CU(cudaStreamSynchronize(s->stream));
+	}
+	*count_out = count; *lo_out = lo; *hi_out = hi;
 	return CRGPU_OK;
 }
 

@@ -463,6 +463,37 @@ enum { CRGPU_LIBM_SIN, CRGPU_LIBM_COS, CRGPU_LIBM_TAN, CRGPU_LIBM_LOG, CRGPU_LIB
        CRGPU_LIBM_ASIN, CRGPU_LIBM_POW, CRGPU_LIBM_POW5, CRGPU_LIBM_SINCOS_SIN, CRGPU_LIBM_SINCOS_COS, CRGPU_LIBM_COUNT };
 int crgpu_libm_eval(int device, int fn, const float *x, const float *y, float *out, uint32_t n);
 
+/* Test entry points of the accumulation kernel (K5) and of an adaptive round's select, scan and compaction, on given samples and
+ * records instead of rendered ones (tests/test_gpu_adaptive_kernels.py).
+ *   crgpu_accumulate_samples  passes [pass_begin, +pass_count) of the tile set `rects` (as crgpu_render_tiles takes it) from given
+ *                         radiance: L holds npix x pass_count x 4 floats, pixel by pixel in the tile set's list order, then pass by
+ *                         pass (the fourth float is not read).  Each sample goes to the slot of the wave buffers' radiance that path
+ *                         order `order` (0..7, or -1: the process's CRGPU_PATH_ORDER) gives its (pass, pixel), and K5 runs with the
+ *                         grid and tile descriptor of an unarmed render call, over the scene's framebuffer; with `adaptive` it runs
+ *                         the adaptive instantiation, which also updates the pixels' records (crgpu_adaptive_reset first).
+ *                         pixels_out (may be NULL) receives the list: npix words x | y << 16.  Refused with CRGPU_ERR_BAD_ARGUMENT: a
+ *                         NULL scene or L, an order out of range, adaptive without records, a tile list crgpu_render_tiles refuses,
+ *                         passes outside [0, sample_count), and npix x pass_count above the paths in flight.
+ *   crgpu_adaptive_write / crgpu_adaptive_records  load / copy out the whole record of every pixel of view 0 (W*H, framebuffer
+ *                         order, as crgpu_adaptive_read).  Each waits for the scene's stream.
+ *   crgpu_adaptive_select the select, scan and compaction of crgpu_adaptive_round (the same code, refused in the same cases, with the
+ *                         same records left behind) without the render that follows: active_out (room for the tile set's pixels)
+ *                         receives the active list, *count_out its length, *lo_out and *hi_out the least and the largest count of
+ *                         its pixels (0xffffffff and 0 with none active).  Refused active pixels of different counts name both in the
+ *                         error text. */
+struct crgpu_adaptive_record {
+	uint32_t n;             /* passes taken; bit 31 (CRGPU_ADAPTIVE_DONE): the pixel has converged */
+	float    mean, m2;      /* Welford mean and M2 of the luminance of those passes */
+	float    err;           /* the error of the last test (+inf before the first) */
+};
+#define CRGPU_ADAPTIVE_DONE 0x80000000u
+int crgpu_accumulate_samples(crgpu_scene *s, const int *rects, int nrects, int pass_begin, int pass_count, int order, int adaptive,
+                             const float *L, uint32_t *pixels_out);
+int crgpu_adaptive_write(crgpu_scene *s, const struct crgpu_adaptive_record *recs);
+int crgpu_adaptive_records(crgpu_scene *s, struct crgpu_adaptive_record *recs_out);
+int crgpu_adaptive_select(crgpu_scene *s, const int *rects, int nrects, const struct crgpu_adaptive *a, uint32_t *active_out,
+                          uint32_t *count_out, uint32_t *lo_out, uint32_t *hi_out);
+
 /* The path order of the frame path (CRGPU_PATH_ORDER, c-ray_b200/csrc/crgpu_wave.cuh), evaluated on the host for order `order`
  * (0..7): for a batch of npix pixels and pass_count passes, pass_out[id] and pixel_out[id] are the pass and pixel (local to the
  * batch) that path id renders, id_out[pass * npix + pixel] is the path id of that pair (any of the three may be NULL); and, when
